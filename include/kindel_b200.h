@@ -198,9 +198,21 @@ int kdl_diagnose(const kdl_batch* batch, kdl_diag* diag_dev, void* stream);
 /* K2 -- per-position vote.  Replaces kindel/kindel.py:402-424 + 369-381 for every slot.
  * calls[s] : bits 0-2 = emitted base (0..4 = A,C,G,T,N; a tie emits N), bits 4-5 = change code
  *            (0 none, 1 'D' -> nothing emitted, 2 'N' -> 'N' emitted, 3 'I' -> insertion string
- *            precedes the base).  min_depth_ceil = ceil(min_depth). */
+ *            precedes the base), bit 7 = 0 (kdl_vote_iupac sets it for a multi-base call, below).
+ *            min_depth_ceil = ceil(min_depth). */
 int kdl_vote(const int32_t* counts, int64_t n_slots, int64_t min_depth_ceil, uint8_t* calls,
              void* stream);
+
+/* K2 with IUPAC ambiguity codes (extension; the reference has no such option), 0 <= threshold <= 1, else (or NaN)
+ * KDL_ERR_INVALID_ARG.  The D, N and I decisions are kdl_vote's and so is every 'D' / 'N' call byte; only the base
+ * of a slot that emits one differs.  With D = A + C + G + T (N excluded): D == 0 emits N; otherwise
+ * L(b) = sum of the counts of all bases with count >= count(b), v = the largest count(b) > 0 with
+ * (double)L(b) >= threshold * (double)D (one correctly rounded multiply), and the call is the set
+ * S = {b : count(b) >= v}.  |S| = 1: the base code, as kdl_vote writes it.  |S| >= 2:
+ * calls[s] = 0x80 | change << 4 | mask, mask A=1 C=2 G=4 T=8 (the BAM nibble, letter "=ACMGRSVTWYHKDBN"[mask]);
+ * bit 7 is never set by kdl_vote. */
+int kdl_vote_iupac(const int32_t* counts, int64_t n_slots, int64_t min_depth_ceil, double threshold, uint8_t* calls,
+                   void* stream);
 
 /* Derived per-position columns of the `alignment` tuple (kindel/kindel.py:83-96) + the ACGT depth
  * used by build_report (kindel.py:450).  out[5][n_slots] int32: consensus_depth, clip_start_depth,
@@ -217,8 +229,8 @@ int kdl_cdr_flags(const int32_t* counts, int64_t n_slots, int64_t slot_lo, int64
                   double clip_decay_threshold, uint8_t* flags, uint8_t* bases, void* stream);
 
 /* K5 -- the consensus text of every contig from the call bytes (reference kindel/kindel.py:413-424): nothing for a
- * 'D' call, the base letter (N for an 'N' call or a tie) otherwise, preceded by the insertion string for an 'I'
- * call.  The strings of the 'I' slots come from the caller (ins_slot ascending, bytes ins_bytes[ins_off[k] ..
+ * 'D' call, the base letter (N for an 'N' call or a tie; the IUPAC letter of a bit-7 call) otherwise, preceded by the
+ * insertion string for an 'I' call.  The strings of the 'I' slots come from the caller (ins_slot ascending, bytes ins_bytes[ins_off[k] ..
  * ins_off[k+1]) as they are to be printed: the modal inserted string in lower case, or "N" for a tie).
  * offsets: device uint32[n_slots + 1], out: offsets[s] = where slot s's text starts in `out`, offsets[n_slots] = total;
  * contig c's sequence is out[offsets[contig_slot[c]] .. offsets[contig_slot[c] + contig_len[c]]).
@@ -274,6 +286,9 @@ typedef struct kdl_exchange {
 int kdl_exchange_signal(const kdl_exchange* x, int32_t epoch, void* stream);
 int kdl_exchange_vote(const kdl_exchange* x, int64_t n_slots, int64_t min_depth_ceil, int32_t epoch,
                       void* stream);
+/* K2x with the IUPAC vote of kdl_vote_iupac (same threshold rule, same call bytes as one table). */
+int kdl_exchange_vote_iupac(const kdl_exchange* x, int64_t n_slots, int64_t min_depth_ceil, double threshold,
+                            int32_t epoch, void* stream);
 int kdl_exchange_wait(const kdl_exchange* x, int32_t epoch, void* stream);
 
 /* Count tables that peer GPUs (other processes of the same node) can map: plain cudaMalloc

@@ -106,6 +106,7 @@ _PROTOTYPES = {
     "kdl_diagnose": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p]),
     "kdl_unmask": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_int64, C.c_void_p]),
     "kdl_vote": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "kdl_vote_iupac": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
     "kdl_derive": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "kdl_cdr_flags": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_assemble_scratch_words": (C.c_int64, [C.c_int64]),
@@ -117,6 +118,8 @@ _PROTOTYPES = {
                                         C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_exchange_signal": (C.c_int, [C.POINTER(KdlExchange), C.c_int32, C.c_void_p]),
     "kdl_exchange_vote": (C.c_int, [C.POINTER(KdlExchange), C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
+    "kdl_exchange_vote_iupac": (C.c_int, [C.POINTER(KdlExchange), C.c_int64, C.c_int64, C.c_double, C.c_int32,
+                                          C.c_void_p]),
     "kdl_exchange_wait": (C.c_int, [C.POINTER(KdlExchange), C.c_int32, C.c_void_p]),
     "kdl_table_alloc": (C.c_int, [C.c_int64, C.POINTER(C.c_void_p)]),
     "kdl_table_free": (C.c_int, [C.c_void_p]),

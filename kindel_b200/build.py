@@ -26,6 +26,8 @@ ORACLE_DIR = os.path.join(ROOT, "oracle", "_build")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "libkindel_oracle.so")
 QORACLE_SRC = os.path.join(ROOT, "oracle", "kindel_qoracle.c")
 QORACLE_LIB = os.path.join(ORACLE_DIR, "libkindel_qoracle.so")
+IORACLE_SRC = os.path.join(ROOT, "oracle", "kindel_ioracle.c")
+IORACLE_LIB = os.path.join(ORACLE_DIR, "libkindel_ioracle.so")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -70,8 +72,9 @@ def build_engine(force: bool = False, verbose: bool = False) -> str:
 
 
 def build_oracle(force: bool = False) -> str:
-    """Both C checkers (the pileup restatement and its base-quality-masking variant); returns the first's path."""
-    for src, lib in ((ORACLE_SRC, ORACLE_LIB), (QORACLE_SRC, QORACLE_LIB)):
+    """The C checkers (the pileup restatement, its base-quality-masking variant and the IUPAC vote); returns the
+    first's path."""
+    for src, lib in ((ORACLE_SRC, ORACLE_LIB), (QORACLE_SRC, QORACLE_LIB), (IORACLE_SRC, IORACLE_LIB)):
         if not force and _newer(lib, [src, os.path.abspath(__file__)]):
             continue
         os.makedirs(ORACLE_DIR, exist_ok=True)

@@ -17,12 +17,12 @@ from . import __version__
 
 
 def consensus(bam_path, realign=False, min_depth=1, min_overlap=7, clip_decay_threshold=0.1, mask_ends=50,
-              trim_ends=False, uppercase=False, gpus=None, **filters):
+              trim_ends=False, uppercase=False, gpus=None, iupac_threshold=None, **filters):
     """Infer consensus sequence(s) from alignment in SAM/BAM format"""
     from . import kindel
 
     res = kindel.bam_to_consensus(bam_path, realign, min_depth, min_overlap, clip_decay_threshold, mask_ends,
-                                  trim_ends, uppercase, devices=gpus, **filters)
+                                  trim_ends, uppercase, devices=gpus, iupac_threshold=iupac_threshold, **filters)
     print("\n".join(res.refs_reports.values()), file=sys.stderr)
     for record in res.consensuses:
         print(f">{record.name}")
@@ -83,6 +83,12 @@ def _add_filters(p):
                    help="skip records with any of these FLAG bits set (decimal or 0x...)")
 
 
+def _iupac_threshold(text: str) -> float:
+    from .kindel import check_iupac_threshold
+
+    return check_iupac_threshold(float(text))  # ValueError (NaN, outside [0, 1]) -> argparse error
+
+
 def _filters(a) -> dict:
     return dict(min_base_quality=a.min_base_quality, min_mapq=a.min_mapq, exclude_flags=a.exclude_flags)
 
@@ -107,9 +113,13 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("-u", "--uppercase", action="store_true", help="close gaps using uppercase alphabet")
     _add_gpus(p)
     _add_filters(p)
+    # extension (not in the reference's CLI): IUPAC ambiguity codes for mixed sites, off by default
+    p.add_argument("--iupac-threshold", type=_iupac_threshold, default=None, metavar="F",
+                   help="emit the IUPAC code of the fewest most frequent bases that reach this fraction (0-1) of "
+                        "the depth instead of the majority base")
     p.set_defaults(func=lambda a: consensus(a.bam_path, a.realign, a.min_depth, a.min_overlap,
                                             a.clip_decay_threshold, a.mask_ends, a.trim_ends, a.uppercase, a.gpus,
-                                            **_filters(a)))
+                                            a.iupac_threshold, **_filters(a)))
 
     p = sub.add_parser("weights", help=weights.__doc__, description=weights.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")

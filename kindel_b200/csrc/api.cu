@@ -241,7 +241,21 @@ int kdl_vote(const int32_t* counts, int64_t n_slots, int64_t min_depth_ceil, uin
     const long long quads = n_slots / 4;
     const long long grid = (quads + 255) / 256;
     kdl::vote_kernel<false><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(
-        counts, none, n_slots, 0, n_slots, min_depth_ceil, calls, nullptr);
+        counts, none, n_slots, 0, n_slots, min_depth_ceil, calls, nullptr, kdl::MajorityVote{});
+    return check_launch();
+}
+
+static bool valid_threshold(double t) { return t >= 0.0 && t <= 1.0; }  // false for NaN
+
+int kdl_vote_iupac(const int32_t* counts, int64_t n_slots, int64_t min_depth_ceil, double threshold, uint8_t* calls,
+                   void* stream) {
+    if (!counts || !calls || n_slots <= 0 || (n_slots & 3) || !valid_threshold(threshold)) return KDL_ERR_INVALID_ARG;
+    kdl::Peers none;
+    none.n = 0;
+    const long long quads = n_slots / 4;
+    const long long grid = (quads + 255) / 256;
+    kdl::vote_kernel<false, kdl::IupacVote><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(
+        counts, none, n_slots, 0, n_slots, min_depth_ceil, calls, nullptr, kdl::IupacVote{threshold});
     return check_launch();
 }
 
@@ -300,8 +314,9 @@ int kdl_exchange_wait(const kdl_exchange* x, int32_t epoch, void* stream) {
     return check_launch();
 }
 
-int kdl_exchange_vote(const kdl_exchange* x, int64_t n_slots, int64_t min_depth_ceil, int32_t epoch,
-                      void* stream) {
+extern "C++" template <class Vote>  // (a template cannot have C linkage)
+int exchange_vote(const kdl_exchange* x, int64_t n_slots, int64_t min_depth_ceil, int32_t epoch, Vote vote,
+                  void* stream) {
     if (n_slots <= 0 || (n_slots & 3)) return KDL_ERR_INVALID_ARG;
     kdl::Exchange e;
     int rc = make_exchange(x, &e, n_slots);
@@ -312,8 +327,20 @@ int kdl_exchange_vote(const kdl_exchange* x, int64_t n_slots, int64_t min_depth_
     const long long cap = (long long)sm_count() * 8;
     if (grid > cap) grid = cap;
     if (grid < 1) grid = 1;  // an empty slice still has to take part in the flag protocol
-    kdl::vote_exchange_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(e, n_slots, min_depth_ceil, epoch);
+    kdl::vote_exchange_kernel<Vote><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(e, n_slots, min_depth_ceil, epoch,
+                                                                                     vote);
     return check_launch();
+}
+
+int kdl_exchange_vote(const kdl_exchange* x, int64_t n_slots, int64_t min_depth_ceil, int32_t epoch,
+                      void* stream) {
+    return exchange_vote(x, n_slots, min_depth_ceil, epoch, kdl::MajorityVote{}, stream);
+}
+
+int kdl_exchange_vote_iupac(const kdl_exchange* x, int64_t n_slots, int64_t min_depth_ceil, double threshold,
+                            int32_t epoch, void* stream) {
+    if (!valid_threshold(threshold)) return KDL_ERR_INVALID_ARG;
+    return exchange_vote(x, n_slots, min_depth_ceil, epoch, kdl::IupacVote{threshold}, stream);
 }
 
 int kdl_cdr_flags(const int32_t* counts, int64_t n_slots, int64_t slot_lo, int64_t slot_hi,
@@ -394,7 +421,7 @@ int kdl_vote_peers_sparse(const int32_t* const* peer_counts, const int64_t* foot
     const long long quads = (slot_hi - slot_lo) / 4;
     const long long grid = (quads + 255) / 256;
     kdl::vote_kernel<true><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(
-        nullptr, peers, n_slots, slot_lo, slot_hi, min_depth_ceil, calls, reduced);
+        nullptr, peers, n_slots, slot_lo, slot_hi, min_depth_ceil, calls, reduced, kdl::MajorityVote{});
     return check_launch();
 }
 

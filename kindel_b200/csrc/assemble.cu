@@ -7,7 +7,8 @@
 //                           row; pairing, LCS merge and patching stay on the host (sequential, tiny).
 //   K5 `assemble_*_kernel`  the consensus text itself (kindel.py:413-424): emitted length per position (0 for a
 //                           deletion call, 1 for a base or an N, 1 + len for an insertion), an exclusive scan over the
-//                           whole slot space, and a scatter of the base letters and the insertion strings.  One pass
+//                           whole slot space, and a scatter of the base letters (or IUPAC codes) and the insertion
+//                           strings.  One pass
 //                           serves every contig: contig c's sequence is out[off[slot_c] .. off[slot_c + L_c]).
 //
 // The float compares of the reference are restated exactly: `clip / (depth + del + 1) > 0.5` is 2 clip > depth + del + 1
@@ -167,7 +168,9 @@ assemble_scatter_kernel(AssembleArgs a, const uint32_t* __restrict__ block_sums,
                 const uint32_t b0 = a.ins_off[j];
                 for (uint32_t q = 0; q + 1u < n[k]; ++q) out[p++] = a.ins_bytes[b0 + q];
             }
-            out[p] = (uint8_t)("ACGTN"[(c & 7u) > 4u ? 4u : (c & 7u)]);
+            // bit 7: a multi-base IUPAC call, bits 0-3 its base set as a BAM nibble (kdl_vote_iupac)
+            out[p] = (c & 0x80u) ? (uint8_t)("=ACMGRSVTWYHKDBN"[c & 15u])
+                                 : (uint8_t)("ACGTN"[(c & 7u) > 4u ? 4u : (c & 7u)]);
         }
         off += n[k];
     }

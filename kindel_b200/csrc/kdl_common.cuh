@@ -85,4 +85,62 @@ __device__ __forceinline__ unsigned vote_slot(int a, int c, int g, int t, int n,
     return (change << 4) | (unsigned)code;
 }
 
+// descending compare-exchange: x keeps the larger value
+__device__ __forceinline__ void cx_desc(int& x, int& y) {
+    const int hi = x > y ? x : y, lo = x > y ? y : x;
+    x = hi;
+    y = lo;
+}
+
+// The emitted base of the IUPAC vote (extension: `iupac_threshold` t in [0, 1]).  D = A + C + G + T (N is not an
+// allele, as in kindel.py:404).  L(b) = sum of the counts of every base with count >= count(b); v = the largest
+// count(b) > 0 with L(b) >= t * D; the call is the set S = {b : count(b) >= v}, so tied bases enter together.
+// The comparison is ONE correctly rounded double multiply and a compare (no add: nothing can be contracted).
+// The four counts are sorted by a fixed compare-exchange network; the prefix sums p_k of the sorted counts never
+// decrease, so the first p_k >= t * D names v (p_k <= L(x_k), and every larger count's tie group ends before k).
+// Returns the base code 0..3 when |S| = 1, 4 (N) when D = 0, else 0x80 | mask with mask A=1 C=2 G=4 T=8 (the BAM
+// nibble: the letter is "=ACMGRSVTWYHKDBN"[mask]).  No data-dependent branch.
+__device__ __forceinline__ unsigned iupac_base(int a, int c, int g, int t, double threshold) {
+    int x0 = a, x1 = c, x2 = g, x3 = t;
+    cx_desc(x0, x1);
+    cx_desc(x2, x3);
+    cx_desc(x0, x2);
+    cx_desc(x1, x3);
+    cx_desc(x1, x2);
+    const long long p0 = x0, p1 = p0 + x1, p2 = p1 + x2, d = p2 + x3;  // counts < 2^31: the sums need 64 bits
+    const double need = threshold * (double)d;
+    const int v = (double)p0 >= need ? x0 : (double)p1 >= need ? x1 : (double)p2 >= need ? x2 : x3;
+    const unsigned mask = (unsigned)(a >= v) | ((unsigned)(c >= v) << 1) | ((unsigned)(g >= v) << 2) |
+                          ((unsigned)(t >= v) << 3);
+    const unsigned single = (mask >> 1) - (mask >> 3);  // 1, 2, 4, 8 -> 0, 1, 2, 3
+    const unsigned code = (mask & (mask - 1u)) ? (0x80u | mask) : single;
+    return d == 0 ? 4u : code;
+}
+
+// vote_slot with the IUPAC base: the D / N / I decisions and their order are vote_slot's; only the base differs
+__device__ __forceinline__ unsigned vote_slot_iupac(int a, int c, int g, int t, int del, int ins, long long depth_next,
+                                                    long long min_depth_ceil, double threshold) {
+    const long long depth = (long long)a + c + g + t;
+    if (2ll * del > depth) return (1u << 4) | 4u;
+    if (depth < min_depth_ceil) return (2u << 4) | 4u;
+    const long long thr = depth < depth_next ? depth : depth_next;
+    const unsigned change = (2ll * ins > thr) ? 3u : 0u;
+    return (change << 4) | iupac_base(a, c, g, t, threshold);
+}
+
+// Vote policies of K2 / K2x (template arguments of vote_kernel and vote_exchange_kernel)
+struct MajorityVote {  // the reference's vote
+    __device__ __forceinline__ unsigned operator()(int a, int c, int g, int t, int n, int del, int ins,
+                                                   long long depth_next, long long min_depth_ceil) const {
+        return vote_slot(a, c, g, t, n, del, ins, depth_next, min_depth_ceil);
+    }
+};
+struct IupacVote {  // ambiguity codes below a frequency threshold
+    double threshold;
+    __device__ __forceinline__ unsigned operator()(int a, int c, int g, int t, int, int del, int ins,
+                                                   long long depth_next, long long min_depth_ceil) const {
+        return vote_slot_iupac(a, c, g, t, del, ins, depth_next, min_depth_ceil, threshold);
+    }
+};
+
 }  // namespace kdl

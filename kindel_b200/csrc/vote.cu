@@ -1,5 +1,5 @@
-// vote.cu -- K2: per-position majority vote; K2d: derived depth columns; K2p: fused cross-GPU
-// count reduction + vote over NVLink peer memory.
+// vote.cu -- K2: per-position majority vote (or, as an extension, the IUPAC vote); K2d: derived depth columns;
+// K2p: fused cross-GPU count reduction + vote over NVLink peer memory.
 //
 // K2 restates, for every table slot at once, the body of consensus_sequence
 // (kindel/kindel.py:402-424) with consensus() (kindel.py:369-381) inlined.  It is a pure streaming
@@ -49,12 +49,14 @@ __device__ __forceinline__ int load1(const int32_t* __restrict__ counts, const P
     }
 }
 
-// n_slots % 4 == 0, slot_lo % 4 == 0.  One thread = 4 slots.
-template <bool kPeers>
+// n_slots % 4 == 0, slot_lo % 4 == 0.  One thread = 4 slots.  Vote: MajorityVote (the reference's) or IupacVote
+// (kdl_common.cuh); the policy argument comes last and defaults to the majority, so the majority instantiations keep
+// their code and their callers.
+template <bool kPeers, class Vote = MajorityVote>
 __global__ void __launch_bounds__(256)
 vote_kernel(const int32_t* __restrict__ counts, Peers peers, long long n_slots, long long slot_lo,
             long long slot_hi, long long min_depth_ceil, uint8_t* __restrict__ calls,
-            int32_t* __restrict__ reduced) {
+            int32_t* __restrict__ reduced, Vote vote = Vote()) {
     const long long quad = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long s = slot_lo + quad * 4;
     const bool active = s < slot_hi;
@@ -85,10 +87,10 @@ vote_kernel(const int32_t* __restrict__ counts, Peers peers, long long n_slots, 
     const long long d1 = (long long)v[0].y + v[1].y + v[2].y + v[3].y;
     const long long d2 = (long long)v[0].z + v[1].z + v[2].z + v[3].z;
     const long long d3 = (long long)v[0].w + v[1].w + v[2].w + v[3].w;
-    const unsigned c0 = vote_slot(v[0].x, v[1].x, v[2].x, v[3].x, v[4].x, v[5].x, v[6].x, d1, min_depth_ceil);
-    const unsigned c1 = vote_slot(v[0].y, v[1].y, v[2].y, v[3].y, v[4].y, v[5].y, v[6].y, d2, min_depth_ceil);
-    const unsigned c2 = vote_slot(v[0].z, v[1].z, v[2].z, v[3].z, v[4].z, v[5].z, v[6].z, d3, min_depth_ceil);
-    const unsigned c3 = vote_slot(v[0].w, v[1].w, v[2].w, v[3].w, v[4].w, v[5].w, v[6].w, dn, min_depth_ceil);
+    const unsigned c0 = vote(v[0].x, v[1].x, v[2].x, v[3].x, v[4].x, v[5].x, v[6].x, d1, min_depth_ceil);
+    const unsigned c1 = vote(v[0].y, v[1].y, v[2].y, v[3].y, v[4].y, v[5].y, v[6].y, d2, min_depth_ceil);
+    const unsigned c2 = vote(v[0].z, v[1].z, v[2].z, v[3].z, v[4].z, v[5].z, v[6].z, d3, min_depth_ceil);
+    const unsigned c3 = vote(v[0].w, v[1].w, v[2].w, v[3].w, v[4].w, v[5].w, v[6].w, dn, min_depth_ceil);
     *reinterpret_cast<uint32_t*>(calls + s) = c0 | (c1 << 8) | (c2 << 16) | (c3 << 24);
 }
 
@@ -151,8 +153,9 @@ __global__ void __launch_bounds__(256) exchange_gather_kernel(Exchange x, int ep
     }
 }
 
+template <class Vote = MajorityVote>
 __global__ void __launch_bounds__(256)
-vote_exchange_kernel(Exchange x, long long n_slots, long long min_depth_ceil, int epoch) {
+vote_exchange_kernel(Exchange x, long long n_slots, long long min_depth_ceil, int epoch, Vote vote = Vote()) {
     // this kernel runs after the rank's pileup kernels in stream order, so its own table is complete:
     // CTA 0 publishes that to every peer (kdl_exchange_signal is then optional) ...
     if (blockIdx.x == 0 && threadIdx.x < x.peers.n) {
@@ -222,10 +225,10 @@ vote_exchange_kernel(Exchange x, long long n_slots, long long min_depth_ceil, in
             const long long d1 = (long long)v[0].y + v[1].y + v[2].y + v[3].y;
             const long long d2 = (long long)v[0].z + v[1].z + v[2].z + v[3].z;
             const long long d3 = (long long)v[0].w + v[1].w + v[2].w + v[3].w;
-            const unsigned c0 = vote_slot(v[0].x, v[1].x, v[2].x, v[3].x, v[4].x, v[5].x, v[6].x, d1, min_depth_ceil);
-            const unsigned c1 = vote_slot(v[0].y, v[1].y, v[2].y, v[3].y, v[4].y, v[5].y, v[6].y, d2, min_depth_ceil);
-            const unsigned c2 = vote_slot(v[0].z, v[1].z, v[2].z, v[3].z, v[4].z, v[5].z, v[6].z, d3, min_depth_ceil);
-            const unsigned c3 = vote_slot(v[0].w, v[1].w, v[2].w, v[3].w, v[4].w, v[5].w, v[6].w, dn, min_depth_ceil);
+            const unsigned c0 = vote(v[0].x, v[1].x, v[2].x, v[3].x, v[4].x, v[5].x, v[6].x, d1, min_depth_ceil);
+            const unsigned c1 = vote(v[0].y, v[1].y, v[2].y, v[3].y, v[4].y, v[5].y, v[6].y, d2, min_depth_ceil);
+            const unsigned c2 = vote(v[0].z, v[1].z, v[2].z, v[3].z, v[4].z, v[5].z, v[6].z, d3, min_depth_ceil);
+            const unsigned c3 = vote(v[0].w, v[1].w, v[2].w, v[3].w, v[4].w, v[5].w, v[6].w, dn, min_depth_ceil);
             *reinterpret_cast<uint32_t*>(calls + s) = c0 | (c1 << 8) | (c2 << 16) | (c3 << 24);
         }
     }
@@ -268,8 +271,12 @@ derive_kernel(const int32_t* __restrict__ counts, long long n_slots, int32_t* __
 }
 
 template __global__ void vote_kernel<false>(const int32_t*, Peers, long long, long long, long long,
-                                            long long, uint8_t*, int32_t*);
+                                            long long, uint8_t*, int32_t*, MajorityVote);
 template __global__ void vote_kernel<true>(const int32_t*, Peers, long long, long long, long long,
-                                           long long, uint8_t*, int32_t*);
+                                           long long, uint8_t*, int32_t*, MajorityVote);
+template __global__ void vote_kernel<false, IupacVote>(const int32_t*, Peers, long long, long long, long long,
+                                                       long long, uint8_t*, int32_t*, IupacVote);
+template __global__ void vote_exchange_kernel<MajorityVote>(Exchange, long long, long long, int, MajorityVote);
+template __global__ void vote_exchange_kernel<IupacVote>(Exchange, long long, long long, int, IupacVote);
 
 }  // namespace kdl

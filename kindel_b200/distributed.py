@@ -304,10 +304,15 @@ class ShardedConsensus:
         """This rank's own count table of the most recent step (NOT reduced, except in allreduce mode)."""
         return self.table[self.epoch & 1].t
 
-    def step(self, min_depth=1, timers=None):
+    def step(self, min_depth=1, timers=None, iupac_threshold=None):
         """K1 on the shard, exchange, vote.  Returns the complete call bytes on every rank.
-        `timers`: optional pair of CUDA events recorded around K1 (bench.py's roofline leg)."""
+        `timers`: optional pair of CUDA events recorded around K1 (bench.py's roofline leg).
+        iupac_threshold (extension): the IUPAC vote (kdl_vote_iupac) in "fused" and "allreduce" mode; "peer" mode
+        has no such vote and raises ValueError."""
         torch, dist, engine = self.torch, self.dist, self.engine
+        iupac_threshold = engine.check_iupac_threshold(iupac_threshold)
+        if iupac_threshold is not None and self.mode == "peer":
+            raise ValueError("iupac_threshold needs exchange mode 'fused' or 'allreduce', not 'peer'")
         self.epoch += 1
         par = self.epoch & 1
         table = self.table[par]
@@ -325,15 +330,20 @@ class ShardedConsensus:
         if self.mode == "fused":
             st = int(torch.cuda.current_stream(self.device).cuda_stream)
             with torch.cuda.device(self.device):
-                _ffi.check(self.lib.kdl_exchange_vote(C.byref(self.xstruct[par]), self.n_slots, int(math.ceil(min_depth)),
-                                                      self.epoch, st), "kdl_exchange_vote")
+                if iupac_threshold is None:
+                    _ffi.check(self.lib.kdl_exchange_vote(C.byref(self.xstruct[par]), self.n_slots,
+                                                          int(math.ceil(min_depth)), self.epoch, st), "kdl_exchange_vote")
+                else:
+                    _ffi.check(self.lib.kdl_exchange_vote_iupac(C.byref(self.xstruct[par]), self.n_slots,
+                                                                int(math.ceil(min_depth)), iupac_threshold, self.epoch,
+                                                                st), "kdl_exchange_vote_iupac")
                 _ffi.check(self.lib.kdl_exchange_wait(C.byref(self.xstruct[par]), self.epoch, st), "kdl_exchange_wait")
             return self.tables.calls[par]
         if self.mode == "allreduce":
             dist.all_reduce(table.t[: _ffi.KDL_NVOTE_COL], op=dist.ReduceOp.SUM, group=self.group)
             if getattr(self, "_calls_ar", None) is None:
                 self._calls_ar = torch.empty(self.n_slots, dtype=torch.uint8, device=self.device)
-            return engine.vote(table.t, min_depth, out=self._calls_ar)
+            return engine.vote(table.t, min_depth, out=self._calls_ar, iupac_threshold=iupac_threshold)
         # "peer": every table complete before anybody reads it over NVLink
         dist.barrier(group=self.group)
         lo, hi = self.slices[self.rank]
@@ -396,7 +406,8 @@ def _free_port() -> int:
         return sk.getsockname()[1]
 
 
-def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode: str, plan: str):
+def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode: str, plan: str,
+                iupac_threshold=None):
     """One process per GPU: pile this rank's shard, exchange, vote; rank 0 leaves the job's results in workdir."""
     import json
     import os
@@ -418,7 +429,7 @@ def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode:
         idx = shard_indices(batch, rank, world, plan)
         shard = select_reads(batch, idx)
         sc = ShardedConsensus(shard, dev, mode=mode)
-        calls = sc.step(min_depth)
+        calls = sc.step(min_depth, iupac_threshold=iupac_threshold)
         # data errors: the reference raises at the FIRST offending record in iteration order -- every rank
         # reports its first one (global read number), the parent re-raises the smallest
         err = None
@@ -456,12 +467,14 @@ def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode:
         dist.destroy_process_group()
 
 
-def run_sharded(batch: bamio.ReadBatch, devices: int, min_depth=1, mode: str = "fused", plan: str = None):
+def run_sharded(batch: bamio.ReadBatch, devices: int, min_depth=1, mode: str = "fused", plan: str = None,
+                iupac_threshold=None):
     """Pileup + vote of `batch` over `devices` GPUs of this node: one process per GPU (torch.distributed, NCCL for
     the plumbing, the fused peer-memory exchange on the data path), whole contigs per rank when there are enough
     of them, else contiguous blocks of every contig's sorted reads.  Returns (calls uint8[n_slots], counts
     int32[19, n_slots], derived int32[5, n_slots], events int32[n_events, 4]) in host memory -- bit-identical to
-    one GPU -- or raises the reference's IndexError / KeyError."""
+    one GPU -- or raises the reference's IndexError / KeyError.  iupac_threshold (extension): the IUPAC vote, see
+    kindel.bam_to_consensus."""
     import json
     import shutil
     import tempfile
@@ -471,6 +484,9 @@ def run_sharded(batch: bamio.ReadBatch, devices: int, min_depth=1, mode: str = "
 
     from . import engine
 
+    iupac_threshold = engine.check_iupac_threshold(iupac_threshold)
+    if iupac_threshold is not None and mode == "peer":
+        raise ValueError("iupac_threshold needs exchange mode 'fused' or 'allreduce', not 'peer'")
     engine.require_cuda()
     n_gpu = torch.cuda.device_count()
     if devices < 1 or devices > n_gpu:
@@ -481,7 +497,8 @@ def run_sharded(batch: bamio.ReadBatch, devices: int, min_depth=1, mode: str = "
     try:
         bamio.save_batch(os.path.join(workdir, "batch"), batch)
         try:
-            mp.spawn(_api_worker, args=(devices, workdir, _free_port(), min_depth, mode, plan), nprocs=devices, join=True)
+            mp.spawn(_api_worker, args=(devices, workdir, _free_port(), min_depth, mode, plan, iupac_threshold),
+                     nprocs=devices, join=True)
         except Exception as exc:
             notes = []
             for r in range(devices):

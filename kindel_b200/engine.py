@@ -7,7 +7,7 @@ implementation behind these functions: without a CUDA device they raise.
 
     upload(batch)              ReadBatch (host numpy) -> DeviceBatch (device tensors + kdl_batch [+ kdl_qmask])
     pileup(dbatch)             K1 (+ K1q for masked bases): count table [19, n_slots] int32 + insertion events
-    vote(counts, min_depth)    K2: call byte per slot
+    vote(counts, min_depth)    K2: call byte per slot (iupac_threshold=t: the IUPAC vote)
     derive(counts)             derived depth columns [5, n_slots]
 """
 from __future__ import annotations
@@ -223,16 +223,34 @@ def diagnose_and_raise(dbatch: DeviceBatch):
     raise RuntimeError("pileup raised its error flag but no offending read was found")
 
 
-def vote(counts: torch.Tensor, min_depth=1, out: torch.Tensor = None) -> torch.Tensor:
-    """K2.  counts int32[>=7, n_slots] (contiguous) -> calls uint8[n_slots] (`out` reuses a buffer)."""
+def check_iupac_threshold(t):
+    """None (off) or a float in [0, 1]; anything else (NaN included) raises ValueError."""
+    if t is None:
+        return None
+    t = float(t)
+    if not 0.0 <= t <= 1.0:
+        raise ValueError("iupac_threshold must lie in [0, 1], got %r" % t)
+    return t
+
+
+def vote(counts: torch.Tensor, min_depth=1, out: torch.Tensor = None, iupac_threshold=None) -> torch.Tensor:
+    """K2.  counts int32[>=7, n_slots] (contiguous) -> calls uint8[n_slots] (`out` reuses a buffer).
+    iupac_threshold (extension, default None = off): the IUPAC vote of kdl_vote_iupac, multi-base calls as IUPAC
+    codes (bit 7 of the call byte)."""
+    t = check_iupac_threshold(iupac_threshold)
     lib = _ffi.load()
     dev = counts.device
     n_slots = counts.shape[1]
     with torch.cuda.device(dev):
         calls = out if out is not None else torch.empty(n_slots, dtype=torch.uint8, device=dev)
-        rc = lib.kdl_vote(counts.data_ptr(), n_slots, int(math.ceil(min_depth)), calls.data_ptr(),
-                          _stream_ptr(dev))
-        _ffi.check(rc, "kdl_vote")
+        if t is None:
+            rc = lib.kdl_vote(counts.data_ptr(), n_slots, int(math.ceil(min_depth)), calls.data_ptr(),
+                              _stream_ptr(dev))
+            _ffi.check(rc, "kdl_vote")
+        else:
+            rc = lib.kdl_vote_iupac(counts.data_ptr(), n_slots, int(math.ceil(min_depth)), t, calls.data_ptr(),
+                                    _stream_ptr(dev))
+            _ffi.check(rc, "kdl_vote_iupac")
     return calls
 
 

@@ -29,6 +29,10 @@ result = namedtuple("result", ["consensuses", "refs_changes", "refs_reports"])
 
 _BASE_CHARS = np.frombuffer(b"ACGTN", dtype=np.uint8)
 _CHANGE_LUT = (None, "D", "N", "I")
+# letter of every call byte: bits 0-2 = base code (0..4 = A,C,G,T,N), or with bit 7 set (the IUPAC vote's multi-base
+# calls) bits 0-3 = the base set as a BAM nibble, A=1 C=2 G=4 T=8
+_CALL_LETTERS = np.array([ord("=ACMGRSVTWYHKDBN"[c & 15]) if c & 0x80 else ord("ACGTN"[min(c & 7, 4)])
+                          for c in range(256)], dtype=np.uint8)
 
 try:  # the reference wraps consensus sequences in dnaio.Sequence (kindel.py:433-434)
     from dnaio import Sequence as _Sequence
@@ -68,9 +72,10 @@ class PileupRun:
         run._ins = InsertionTable(batch, events)
         return run
 
-    def vote(self, min_depth=1) -> np.ndarray:
-        """K2 over the whole table -> call bytes on the host (the device copy is kept for K5)."""
-        self.calls_device = engine.vote(self.counts, min_depth)
+    def vote(self, min_depth=1, iupac_threshold=None) -> np.ndarray:
+        """K2 over the whole table -> call bytes on the host (the device copy is kept for K5).  iupac_threshold:
+        extension, see bam_to_consensus."""
+        self.calls_device = engine.vote(self.counts, min_depth, iupac_threshold=iupac_threshold)
         return self.calls_device.cpu().numpy()
 
     @property
@@ -146,12 +151,15 @@ def _default_devices(devices):
     return max(1, int(devices))
 
 
-def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq=0, exclude_flags=0):
+def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq=0, exclude_flags=0,
+               iupac_threshold=None):
     """(PileupRun, calls) of an alignment file on `devices` GPUs.  devices > 1: one process per GPU, reads (or whole
     contigs) sharded, counts exchanged over NVLink in front of the vote (distributed.run_sharded); the result is
     bit-identical to one GPU.  min_base_quality / min_mapq / exclude_flags (extension, all off by default): a record
     with MAPQ < min_mapq or FLAG & exclude_flags is treated as unmapped; a base with Phred quality < min_base_quality
-    is read as N and not counted (kindel_b200/bamio.py)."""
+    is read as N and not counted (kindel_b200/bamio.py).  iupac_threshold: the vote of the sharded job (extension,
+    see bam_to_consensus); calls is None for one GPU, where the caller votes."""
+    iupac_threshold = check_iupac_threshold(iupac_threshold)
     batch = bamio.read_alignment(bam_path, min_mapq=min_mapq, exclude_flags=exclude_flags,
                                  min_base_quality=min_base_quality)
     devices = _default_devices(devices)
@@ -160,7 +168,7 @@ def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq
         return run, None
     from . import distributed
 
-    calls, counts, derived, events = distributed.run_sharded(batch, devices, min_depth)
+    calls, counts, derived, events = distributed.run_sharded(batch, devices, min_depth, iupac_threshold=iupac_threshold)
     return PileupRun.from_host_tables(batch, counts, derived, events), calls
 
 
@@ -206,7 +214,12 @@ def _vote_columns(weights, insertions, deletions):
     return cols
 
 
-def _device_vote(cols: np.ndarray, min_depth) -> np.ndarray:
+def check_iupac_threshold(t):
+    """The one check of the iupac_threshold option: None (off) or a number in [0, 1], else ValueError."""
+    return engine.check_iupac_threshold(t)
+
+
+def _device_vote(cols: np.ndarray, min_depth, iupac_threshold=None) -> np.ndarray:
     import torch
 
     dev = engine.require_cuda()
@@ -214,18 +227,22 @@ def _device_vote(cols: np.ndarray, min_depth) -> np.ndarray:
     n_pad = (n + 3) // 4 * 4
     t = torch.zeros((7, n_pad), dtype=torch.int32, device=dev)
     t[:, :n] = torch.from_numpy(np.ascontiguousarray(cols)).to(dev)
-    return engine.vote(t, min_depth).cpu().numpy()[:n]
+    return engine.vote(t, min_depth, iupac_threshold=iupac_threshold).cpu().numpy()[:n]
 
 
 def _emit_range(calls, lo, hi, ins_lookup, out, changes):
-    """Append the consensus text of positions [lo, hi) to `out` (kindel.py:413-424)."""
+    """Append the consensus text of positions [lo, hi) to `out` (kindel.py:413-424).  A bit-7 call (IUPAC vote)
+    emits its ambiguity code; when `changes` keeps an `iupac` list, its 1-based position is added there."""
     if hi <= lo:
         return
     seg = calls[lo:hi]
     change = (seg >> 4) & 3
-    chars = _BASE_CHARS[seg & 7]
+    chars = _CALL_LETTERS[seg]
     for k in np.flatnonzero(change).tolist():
         changes[lo + k] = _CHANGE_LUT[change[k]]
+    iupac = getattr(changes, "iupac", None)
+    if iupac is not None:
+        iupac.extend(str(lo + k + 1) for k in np.flatnonzero(seg & 0x80).tolist())
     ins_pos = np.flatnonzero(change == 3)
     keep = change != 1
     if ins_pos.size == 0:
@@ -248,7 +265,8 @@ def assemble_consensus(calls, ins_lookup, cdr_patches=None, trim_ends=False, upp
     their lower-cased sequence and skip `end - start - 1` further positions without looking at them.
     """
     L = calls.shape[0]
-    changes = [None] * L
+    changes = _Changes([None] * L)
+    changes.iupac = []  # positions of multi-base IUPAC calls that were emitted
     out = []
     starts = sorted({r.start for r in cdr_patches if r.seq and 0 <= r.start < L}) if cdr_patches else []
     pos = 0
@@ -272,10 +290,13 @@ def assemble_consensus(calls, ins_lookup, cdr_patches=None, trim_ends=False, upp
     return seq, changes
 
 
-def consensus_sequence(weights, insertions, deletions, cdr_patches, trim_ends, min_depth, uppercase):
+def consensus_sequence(weights, insertions, deletions, cdr_patches, trim_ends, min_depth, uppercase,
+                       iupac_threshold=None):
     """Per-position vote -> (consensus string, changes) (reference kindel/kindel.py:384-430).
-    The vote itself runs on the GPU (K2); strings are assembled here."""
-    calls = _device_vote(_vote_columns(weights, insertions, deletions), min_depth)[: len(weights)]
+    The vote itself runs on the GPU (K2); strings are assembled here.  iupac_threshold: extension, see
+    bam_to_consensus."""
+    iupac_threshold = check_iupac_threshold(iupac_threshold)
+    calls = _device_vote(_vote_columns(weights, insertions, deletions), min_depth, iupac_threshold)[: len(weights)]
     return assemble_consensus(calls, lambda p: dict_consensus(insertions[p]), cdr_patches, trim_ends, uppercase)
 
 
@@ -447,9 +468,12 @@ DepthRange = namedtuple("DepthRange", ["dmin", "dmax"])  # min / max ACGT depth 
 
 
 def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_depth, min_overlap,
-                 clip_decay_threshold, trim_ends, uppercase, filters=None):
+                 clip_decay_threshold, trim_ends, uppercase, filters=None, iupac_threshold=None):
     """REPORT text block (reference kindel/kindel.py:437-485).  filters (extension): (min_base_quality, min_mapq,
-    exclude_flags); when any is set, three option lines follow `- uppercase:`, otherwise the text is the reference's."""
+    exclude_flags); when any is set, three option lines follow `- uppercase:`, otherwise the text is the reference's.
+    iupac_threshold (extension): when set, `- iupac_threshold:` follows the option lines and `- iupac sites:` (the
+    positions of multi-base calls, from the `iupac` list of a changes list this module built) follows
+    `- ambiguous sites:`."""
     if isinstance(weights, DepthRange):  # already reduced on the device: no table copy needed
         dmin, dmax = weights.dmin, weights.dmax
     elif isinstance(weights, BaseCounts):
@@ -480,10 +504,16 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
     if filters is not None and any(filters):
         lines += ["- min_base_quality: {}".format(filters[0]), "- min_mapq: {}".format(filters[1]),
                   "- exclude_flags: {:#x}".format(filters[2])]
+    if iupac_threshold is not None:
+        lines.append("- iupac_threshold: {}".format(iupac_threshold))
     lines += [
         "observations:",
         "- min, max observed depth: {}, {}".format(dmin, dmax),
         "- ambiguous sites: {}".format(", ".join(sites["N"])),
+    ]
+    if iupac_threshold is not None:
+        lines.append("- iupac sites: {}".format(", ".join(getattr(changes, "iupac", None) or [])))
+    lines += [
         "- insertion sites: {}".format(", ".join(sites["I"])),
         "- deletion sites: {}".format(", ".join(sites["D"])),
         "- clip-dominant regions: {}".format(", ".join(patches)),
@@ -494,26 +524,34 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
 # --------------------------------------------------------------------------------- public API
 def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_decay_threshold=0.1,
                      mask_ends=50, trim_ends=False, uppercase=False, devices=None, min_base_quality=0, min_mapq=0,
-                     exclude_flags=0):
+                     exclude_flags=0, iupac_threshold=None):
     """Consensus sequence(s) of an alignment file (reference kindel/kindel.py:488-555).
 
     Device work per file: one pileup (K1) and one vote (K2) over all contigs at once; only the
     call bytes, the insertion events and -- for --realign and the report -- count columns come
     back to the host.  `devices` (extension; default $KINDEL_GPUS or 1) shards the pileup over that many GPUs of
-    the node.  min_base_quality / min_mapq / exclude_flags: extension, see pileup_run."""
+    the node.  min_base_quality / min_mapq / exclude_flags: extension, see pileup_run.
+
+    iupac_threshold (extension; default None = off, the reference's vote): t in [0, 1].  Where a base is emitted,
+    the call is the smallest set of the most frequent bases (A, C, G, T; N is not an allele) that holds at least
+    t * depth of the reads, tied bases entering together, written as its IUPAC code (R = A/G, Y = C/T, ...,
+    N = all four).  The D / N / I changes and the inserted strings are those of the reference's vote."""
+    iupac_threshold = check_iupac_threshold(iupac_threshold)
     filters = (min_base_quality, min_mapq, exclude_flags)
-    run, calls = pileup_run(bam_path, devices, min_depth, *filters)
+    run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold)
     if calls is None:
-        calls = run.vote(min_depth)
+        calls = run.vote(min_depth, iupac_threshold)
     return consensus_from_run(run, calls, bam_path, realign, min_depth, min_overlap,
-                              clip_decay_threshold, mask_ends, trim_ends, uppercase, filters=filters)
+                              clip_decay_threshold, mask_ends, trim_ends, uppercase, filters=filters,
+                              iupac_threshold=iupac_threshold)
 
 
 class _Changes(list):
     """The reference's `changes` list (None / 'D' / 'N' / 'I' per position) that also remembers where its few
-    non-None entries are, so the report needs no pass over millions of Nones."""
+    non-None entries are, so the report needs no pass over millions of Nones, and (`iupac`) the 1-based positions
+    of multi-base IUPAC calls, which the list itself cannot show."""
 
-    __slots__ = ("sites",)
+    __slots__ = ("sites", "iupac")
 
 
 def _changes_list(calls):
@@ -526,6 +564,7 @@ def _changes_list(calls):
         name = _CHANGE_LUT[code]
         out[k] = name
         out.sites[name].append(str(k + 1))
+    out.iupac = [str(k + 1) for k in np.flatnonzero(calls & 0x80).tolist()]
     return out
 
 
@@ -546,8 +585,10 @@ def _device_texts(run, calls_all):
 
 
 def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min_overlap=9,
-                       clip_decay_threshold=0.1, mask_ends=50, trim_ends=False, uppercase=False, filters=None):
-    """Host half of bam_to_consensus: per contig, optional CDR patches, string assembly, report."""
+                       clip_decay_threshold=0.1, mask_ends=50, trim_ends=False, uppercase=False, filters=None,
+                       iupac_threshold=None):
+    """Host half of bam_to_consensus: per contig, optional CDR patches, string assembly, report.  The call bytes
+    already carry the vote; iupac_threshold (extension) only adds its lines to the report."""
     ins_table = run.ins_table
     consensuses, refs_changes, refs_reports = [], {}, {}
     on_device = run.counts is not None
@@ -581,7 +622,7 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
             cons, changes = assemble_consensus(calls_all[s:e - 1], lambda p, s=s: ins_table.consensus_at(s + p),
                                                cdr_patches, trim_ends, uppercase)
         report = build_report(ref_id, report_weights, changes, cdr_patches, bam_path, realign, min_depth,
-                              min_overlap, clip_decay_threshold, trim_ends, uppercase, filters)
+                              min_overlap, clip_decay_threshold, trim_ends, uppercase, filters, iupac_threshold)
         consensuses.append(consensus_seqrecord(cons, ref_id))
         refs_reports[ref_id] = report
         refs_changes[ref_id] = changes

@@ -36,12 +36,14 @@ def row(path: str, d: dict) -> str:
                 f"{fmt(d.get('value'))} | — | — | — | — |")
     cfg = d.get("config", {})
     roof = d.get("roofline", {})
-    e2e = d.get("e2e", {})
+    e2e = d.get("e2e") or {}  # (null on an --iupac-threshold line: the host-buffer call has no IUPAC vote)
     km = d.get("kernels_ms", {})
     work = cfg.get("workload", "?")
     cx = cfg.get("complex_reads_per_rank")
     if cx:
         work += f" ({cx} complex reads/GPU)"
+    if d.get("iupac_threshold") is not None:
+        work += f", IUPAC vote at {d['iupac_threshold']}"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
            f"{fmt(km.get('k0_k1_pileup'), '.4f')} | {fmt(roof.get('frac'), '.3f')} | {fmt(e2e.get('value'))} | "
            f"{d.get('parity')} |")
