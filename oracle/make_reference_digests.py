@@ -10,6 +10,10 @@ so they need nothing outside the repository.  It holds, as truncated sha256 dige
   host_api      per clip-heavy / generic case and its option set (`options`): what `bam_to_consensus` returns
                 or raises, the CDR helpers on every contig, and the `weights` / `features` frames
   suite_fasta   the FASTA files of the reference's own test suite, per fixture and mode (plain / realign)
+  limit_cases   per group of tests/limit_cases.py: per contig its table, insertion dicts and `changes`, and the
+                FASTA of `bam_to_consensus` with the default options
+
+`python -m oracle.make_reference_digests limit_cases` recomputes only the named sections of an existing file.
 """
 from __future__ import annotations
 
@@ -99,7 +103,6 @@ def fasta_digest(records):
 
 
 def _fuzz_pileup(k, tmp):
-    import helpers
     from fuzz_cases import random_case
 
     out = []
@@ -107,21 +110,25 @@ def _fuzz_pileup(k, tmp):
         path = os.path.join(tmp, "fuzz%d.sam" % seed)
         with open(path, "w") as fh:
             fh.write(random_case(seed))
-        try:
-            alns = k.parse_bam(path)
-        except IndexError:
-            out.append({"raises": ["IndexError"]})
-            continue
-        except KeyError as exc:
-            out.append({"raises": ["KeyError", exc.args[0]]})
-            continue
-        contigs = []
-        for aln in alns.values():
-            t, ins = helpers.reference_alignment_to_table(aln)
-            _, changes = k.consensus_sequence(aln.weights, aln.insertions, aln.deletions, None, False, 1, False)
-            contigs.append(table_digest(t, ins, changes))
-        out.append({"raises": None, "contigs": list(alns), "digests": contigs})
+        out.append(_fuzz_pileup_one(k, path))
     return out
+
+
+def _fuzz_pileup_one(k, path):
+    import helpers
+
+    try:
+        alns = k.parse_bam(path)
+    except IndexError:
+        return {"raises": ["IndexError"]}
+    except KeyError as exc:
+        return {"raises": ["KeyError", exc.args[0]]}
+    contigs = []
+    for aln in alns.values():
+        t, ins = helpers.reference_alignment_to_table(aln)
+        _, changes = k.consensus_sequence(aln.weights, aln.insertions, aln.deletions, None, False, 1, False)
+        contigs.append(table_digest(t, ins, changes))
+    return {"raises": None, "contigs": list(alns), "digests": contigs}
 
 
 def _host_api(k, tmp, kind):
@@ -149,6 +156,21 @@ def _host_api(k, tmp, kind):
             except IndexError:
                 entry["features"] = "IndexError"
         out.append(entry)
+    return out
+
+
+def _limit_cases(k, tmp):
+    import limit_cases
+
+    out = {}
+    for name in limit_cases.GROUPS:
+        path = os.path.join(tmp, name + ".sam")
+        with open(path, "w") as fh:
+            fh.write(limit_cases.sam_text(name))
+        entry = _fuzz_pileup_one(k, path)
+        res = k.bam_to_consensus(path)
+        entry["fasta"] = fasta_digest([(r.name, r.sequence) for r in res.consensuses])
+        out[name] = entry
     return out
 
 
@@ -180,11 +202,21 @@ def main():
     if not refload.available() or not os.path.isdir(os.path.join(refload.REFERENCE_ROOT, "tests")):
         raise SystemExit("the reference tree (with its tests/) is not present")
     k = refload.load_reference()
+    sections = {"fuzz_pileup": lambda tmp: _fuzz_pileup(k, tmp),
+                "host_api": lambda tmp: {"clip": _host_api(k, tmp, "clip"), "gen": _host_api(k, tmp, "gen")},
+                "suite_fasta": lambda tmp: _suite_fasta(refload.REFERENCE_ROOT),
+                "limit_cases": lambda tmp: _limit_cases(k, tmp)}
+    only = sys.argv[1:]
+    if any(s not in sections for s in only):
+        raise SystemExit("sections: " + ", ".join(sections))
+    doc = {"reference": "bede/kindel v1.2.1 @ 14d727b", "generator": "oracle/make_reference_digests.py"}
+    if only:
+        with open(OUT) as fh:
+            doc = json.load(fh)
     with tempfile.TemporaryDirectory() as tmp:
-        doc = {"reference": "bede/kindel v1.2.1 @ 14d727b", "generator": "oracle/make_reference_digests.py",
-               "fuzz_pileup": _fuzz_pileup(k, tmp),
-               "host_api": {"clip": _host_api(k, tmp, "clip"), "gen": _host_api(k, tmp, "gen")},
-               "suite_fasta": _suite_fasta(refload.REFERENCE_ROOT)}
+        for name, make in sections.items():
+            if not only or name in only:
+                doc[name] = make(tmp)
     with open(OUT, "w") as fh:
         json.dump(doc, fh, separators=(",", ":"), sort_keys=True)
     print("wrote", OUT, os.path.getsize(OUT), "bytes")

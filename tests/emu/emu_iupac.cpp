@@ -1,4 +1,4 @@
-// emu_iupac.cpp -- TEST INFRASTRUCTURE: the IUPAC vote (K2 and K2x with IupacVote, kindel_b200/csrc/vote.cu) and K5
+// emu_iupac.cpp -- TEST INFRASTRUCTURE: the IUPAC vote (K2 and K2x with IupacVote, kindel_b200/csrc/vote.cu), K4 and K5
 // (assemble.cu) compiled for the host and run under tests/emu/cuda_emu.h, as emu_pileup.cpp does for the other
 // kernels.  The kernel sources are included as they are; nothing here is part of the product.
 #define KDL_HOST_EMU 1
@@ -75,6 +75,15 @@ int emu_exchange_epoch_iupac(const kdl_exchange* xs, int n_ranks, long long n_sl
             if (e_) { snprintf(g_error, sizeof g_error, "%s", e_); return 1; }
         }
     }
+    return 0;
+}
+
+// K4 as kdl_cdr_flags launches it: flags and bases of slots [slot_lo, slot_hi).  HOST pointers.
+int emu_cdr_flags(const int32_t* counts, long long n_slots, long long slot_lo, long long slot_hi, double decay,
+                  uint8_t* flags, uint8_t* bases) {
+    g_error[0] = 0;
+    if (slot_hi <= slot_lo) return 0;
+    EMU_RUN((slot_hi - slot_lo + 255) / 256, 256, kdl::cdr_flags_kernel(counts, n_slots, slot_lo, slot_hi, decay, flags, bases));
     return 0;
 }
 

@@ -2,7 +2,7 @@
 
 The sources of kindel_b200/csrc/vote.cu and assemble.cu are compiled for the host on top of tests/emu/cuda_emu.h, as
 tests/emu_harness.py does for the other kernels, into a library of its own.  `vote_iupac` is K2 with the IUPAC vote,
-`exchange_epoch` one epoch of K2x (IUPAC) + K2g for every rank, `assemble` the consensus text K5 writes."""
+`exchange_epoch` one epoch of K2x (IUPAC) + K2g for every rank, `assemble` the consensus text K5 writes, `cdr_flags` the --realign predicates of K4."""
 from __future__ import annotations
 
 import ctypes as C
@@ -49,6 +49,7 @@ def load():
     lib.emu_exchange_epoch_iupac.argtypes = [C.POINTER(_ffi.KdlExchange), C.c_int, C.c_longlong, C.c_longlong,
                                              C.c_double, C.c_int, C.c_int]
     lib.emu_assemble.argtypes = [vp, C.c_longlong, vp, vp, C.c_int, vp, vp, vp, C.c_longlong, vp, vp, vp]
+    lib.emu_cdr_flags.argtypes = [vp, C.c_longlong, C.c_longlong, C.c_longlong, C.c_double, vp, vp]
     _lib = lib
     return lib
 
@@ -113,6 +114,21 @@ def assemble(calls: np.ndarray, batch, ins_slots, ins_strings):
                             offsets.ctypes.data, out.ctypes.data))
     text = out[: int(offsets[n_slots])].tobytes()
     return [text[int(offsets[s]):int(offsets[s + L])].decode("ascii") for s, L in zip(c_slot.tolist(), c_len.tolist())]
+
+
+def cdr_flags(counts: np.ndarray, slot_lo: int, slot_hi: int, decay: float):
+    """K4 (kdl_cdr_flags) over a host table: (flags, bases) uint8 of slots [slot_lo, slot_hi), like engine.cdr_flags.
+    Slots outside the range keep the canary 0xEE, which is checked."""
+    lib = load()
+    counts = np.ascontiguousarray(counts, dtype=np.int32)
+    n = counts.shape[1]
+    flags = np.full(n, 0xEE, dtype=np.uint8)
+    bases = np.full(n, 0xEE, dtype=np.uint8)
+    _check(lib.emu_cdr_flags(counts.ctypes.data, n, int(slot_lo), int(slot_hi), float(decay), flags.ctypes.data,
+                             bases.ctypes.data))
+    assert (flags[:slot_lo] == 0xEE).all() and (flags[slot_hi:] == 0xEE).all(), "K4 wrote outside its slot range"
+    assert (bases[:slot_lo] == 0xEE).all() and (bases[slot_hi:] == 0xEE).all(), "K4 wrote outside its slot range"
+    return flags[slot_lo:slot_hi].copy(), bases[slot_lo:slot_hi].copy()
 
 
 def set_schedule(mode: str = "forward", seed: int = 1):
