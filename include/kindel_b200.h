@@ -241,6 +241,22 @@ int kdl_assemble(const uint8_t* calls, int64_t n_slots, const int64_t* contig_sl
                  int32_t n_contigs, const int64_t* ins_slot, const uint32_t* ins_off, const uint8_t* ins_bytes,
                  int64_t n_ins, uint32_t* block_sums, uint32_t* offsets, uint8_t* out, void* stream);
 
+/* K2q -- per-base consensus qualities (extension; the reference has no such output), after any vote of the same
+ * table (kdl_vote, kdl_vote_iupac, or the exchange's reduced table and gathered calls).  n_slots % 4 == 0; only
+ * columns 0-3 of counts are read.  qual[s] = Q in 0..60 of the base slot s emits: with D = A + C + G + T and k = the
+ * call's support -- the count of the called base, the summed counts of a multi-base IUPAC set, 0 for every call that
+ * emits N (min depth, tie, zero depth, N winning, the IUPAC set of all four bases) and for a 'D' call -- Q = 0 when
+ * k = 0, else the largest q <= 60 with (double)(D - k + 1) * TEN[q] <= (double)(D + 2), TEN[q] the correctly rounded
+ * double of 10^(q/10) (kindel_b200/csrc/assemble.cu). */
+int kdl_consensus_qual(const int32_t* counts, const uint8_t* calls, int64_t n_slots, uint8_t* qual, void* stream);
+
+/* K5q -- the quality text beside kdl_assemble's text, on the same stream after it: `offsets` is what kdl_assemble
+ * wrote.  Slot s owns out[offsets[s] .. offsets[s + 1]): every byte of an inserted string gets '!' + ins_qual[k] of
+ * its slot (ins_slot ascending, as given to kdl_assemble), the slot's last byte '!' + qual[s].  out: device bytes, as
+ * many as kdl_assemble's text.  All pointers are device pointers. */
+int kdl_assemble_qual(const uint32_t* offsets, const uint8_t* qual, int64_t n_slots, const int64_t* ins_slot,
+                      const uint8_t* ins_qual, int64_t n_ins, uint8_t* out, void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced

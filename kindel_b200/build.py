@@ -6,6 +6,8 @@
         -> kindel_b200/_lib/libkindel_b200.so          nvcc, -gencode arch=compute_90a,code=sm_90a
     oracle/kindel_oracle.c -> oracle/_build/libkindel_oracle.so   gcc (test infrastructure)
     oracle/kindel_qoracle.c -> oracle/_build/libkindel_qoracle.so gcc (test infrastructure: the base-quality filter)
+    oracle/kindel_ioracle.c, kindel_fqoracle.c -> oracle/_build/  gcc (test infrastructure: the IUPAC vote, the
+                                                                  per-base consensus qualities)
 
 Both artefacts are git-ignored.  A rebuild is skipped when the artefact is newer than every source and than
 this file (which holds the compiler flags).
@@ -28,6 +30,8 @@ QORACLE_SRC = os.path.join(ROOT, "oracle", "kindel_qoracle.c")
 QORACLE_LIB = os.path.join(ORACLE_DIR, "libkindel_qoracle.so")
 IORACLE_SRC = os.path.join(ROOT, "oracle", "kindel_ioracle.c")
 IORACLE_LIB = os.path.join(ORACLE_DIR, "libkindel_ioracle.so")
+FQORACLE_SRC = os.path.join(ROOT, "oracle", "kindel_fqoracle.c")
+FQORACLE_LIB = os.path.join(ORACLE_DIR, "libkindel_fqoracle.so")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -72,9 +76,10 @@ def build_engine(force: bool = False, verbose: bool = False) -> str:
 
 
 def build_oracle(force: bool = False) -> str:
-    """The C checkers (the pileup restatement, its base-quality-masking variant and the IUPAC vote); returns the
-    first's path."""
-    for src, lib in ((ORACLE_SRC, ORACLE_LIB), (QORACLE_SRC, QORACLE_LIB), (IORACLE_SRC, IORACLE_LIB)):
+    """The C checkers (the pileup restatement, its base-quality-masking variant, the IUPAC vote and the consensus
+    qualities); returns the first's path."""
+    for src, lib in ((ORACLE_SRC, ORACLE_LIB), (QORACLE_SRC, QORACLE_LIB), (IORACLE_SRC, IORACLE_LIB),
+                     (FQORACLE_SRC, FQORACLE_LIB)):
         if not force and _newer(lib, [src, os.path.abspath(__file__)]):
             continue
         os.makedirs(ORACLE_DIR, exist_ok=True)

@@ -1,7 +1,8 @@
 """`kindel` command line on the H100 engine (restates the argh CLI of reference kindel/cli.py:9-66).
 
 Sub-commands, flags, defaults and output streams follow the reference: `consensus` prints the
-REPORT blocks to stderr and one `>name` / sequence pair per contig to stdout (cli.py:30-33),
+REPORT blocks to stderr and one `>name` / sequence pair per contig to stdout (cli.py:30-33; with the `--fastq`
+extension one FASTQ record per contig instead),
 `weights` / `features` write TSV to stdout (cli.py:44,50), `version` prints `kindel <version>`;
 `variants` (in the reference's README only) is an extension, see kindel.variants.
 argh derived the flags from the function signatures (first letter as short option unless two
@@ -17,16 +18,20 @@ from . import __version__
 
 
 def consensus(bam_path, realign=False, min_depth=1, min_overlap=7, clip_decay_threshold=0.1, mask_ends=50,
-              trim_ends=False, uppercase=False, gpus=None, iupac_threshold=None, **filters):
+              trim_ends=False, uppercase=False, gpus=None, iupac_threshold=None, fastq=False, **filters):
     """Infer consensus sequence(s) from alignment in SAM/BAM format"""
     from . import kindel
 
     res = kindel.bam_to_consensus(bam_path, realign, min_depth, min_overlap, clip_decay_threshold, mask_ends,
-                                  trim_ends, uppercase, devices=gpus, iupac_threshold=iupac_threshold, **filters)
+                                  trim_ends, uppercase, devices=gpus, iupac_threshold=iupac_threshold,
+                                  qualities=fastq, **filters)
     print("\n".join(res.refs_reports.values()), file=sys.stderr)
     for record in res.consensuses:
-        print(f">{record.name}")
-        print(record.sequence)
+        if fastq:  # extension: @name, sequence, +, Phred+33 qualities
+            print(f"@{record.name}\n{record.sequence}\n+\n{record.qualities}")
+        else:
+            print(f">{record.name}")
+            print(record.sequence)
 
 
 def weights(bam_path, relative=False, confidence=True, confidence_alpha=0.01, gpus=None, **filters):
@@ -117,9 +122,12 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--iupac-threshold", type=_iupac_threshold, default=None, metavar="F",
                    help="emit the IUPAC code of the fewest most frequent bases that reach this fraction (0-1) of "
                         "the depth instead of the majority base")
+    # extension (not in the reference's CLI): per-base qualities, off by default
+    p.add_argument("--fastq", action="store_true",
+                   help="write FASTQ with a Phred quality per consensus base instead of FASTA")
     p.set_defaults(func=lambda a: consensus(a.bam_path, a.realign, a.min_depth, a.min_overlap,
                                             a.clip_decay_threshold, a.mask_ends, a.trim_ends, a.uppercase, a.gpus,
-                                            a.iupac_threshold, **_filters(a)))
+                                            a.iupac_threshold, a.fastq, **_filters(a)))
 
     p = sub.add_parser("weights", help=weights.__doc__, description=weights.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")

@@ -378,6 +378,23 @@ int kdl_assemble(const uint8_t* calls, int64_t n_slots, const int64_t* contig_sl
     return check_launch();
 }
 
+int kdl_consensus_qual(const int32_t* counts, const uint8_t* calls, int64_t n_slots, uint8_t* qual, void* stream) {
+    if (!counts || !calls || !qual || n_slots <= 0 || (n_slots & 3)) return KDL_ERR_INVALID_ARG;
+    const long long grid = (n_slots / 4 + 255) / 256;
+    kdl::consensus_qual_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(counts, calls, n_slots, qual);
+    return check_launch();
+}
+
+int kdl_assemble_qual(const uint32_t* offsets, const uint8_t* qual, int64_t n_slots, const int64_t* ins_slot,
+                      const uint8_t* ins_qual, int64_t n_ins, uint8_t* out, void* stream) {
+    if (!offsets || !qual || !out || n_slots <= 0 || n_ins < 0 || (n_ins > 0 && (!ins_slot || !ins_qual)))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
+    kdl::assemble_qual_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
+        offsets, qual, n_slots, ins_slot, ins_qual, n_ins, out);
+    return check_launch();
+}
+
 int kdl_table_alloc(int64_t bytes, void** dev_ptr) {
     if (!dev_ptr || bytes <= 0) return KDL_ERR_INVALID_ARG;
     *dev_ptr = nullptr;

@@ -9,6 +9,8 @@ implementation behind these functions: without a CUDA device they raise.
     pileup(dbatch)             K1 (+ K1q for masked bases): count table [19, n_slots] int32 + insertion events
     vote(counts, min_depth)    K2: call byte per slot (iupac_threshold=t: the IUPAC vote)
     derive(counts)             derived depth columns [5, n_slots]
+    consensus_qual(counts, calls)  K2q: Phred quality of the base each slot emits (extension)
+    assemble(calls, ...)       K5 (+ K5q): consensus text (and its quality text) of every contig
 """
 from __future__ import annotations
 
@@ -282,9 +284,27 @@ def cdr_flags(counts: torch.Tensor, slot_lo: int, slot_hi: int, clip_decay_thres
     return flags[slot_lo:slot_hi].cpu().numpy(), bases[slot_lo:slot_hi].cpu().numpy()
 
 
-def assemble(calls: torch.Tensor, host: ReadBatch, ins_slots: np.ndarray, ins_strings):
+def consensus_qual(counts: torch.Tensor, calls: torch.Tensor) -> torch.Tensor:
+    """K2q (extension): the Phred quality 0..60 of the base every slot emits, uint8[n_slots] on the device, from the
+    call bytes of any vote over `counts` (int32[>= 4, n_slots], contiguous; n_slots % 4 == 0).  The rule:
+    kindel_b200/quality.py."""
+    lib = _ffi.load()
+    dev = counts.device
+    n_slots = counts.shape[1]
+    with torch.cuda.device(dev):
+        qual = torch.empty(n_slots, dtype=torch.uint8, device=dev)
+        rc = lib.kdl_consensus_qual(counts.data_ptr(), calls.data_ptr(), n_slots, qual.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_consensus_qual")
+    return qual
+
+
+def assemble(calls: torch.Tensor, host: ReadBatch, ins_slots: np.ndarray, ins_strings, qual: torch.Tensor = None,
+             ins_qual=None):
     """K5: consensus text of every contig from the device call bytes.  ins_slots (ascending) / ins_strings: the
-    chosen insertion string of every slot whose call carries change 'I'.  Returns a list of str, one per contig."""
+    chosen insertion string of every slot whose call carries change 'I'.  Returns a list of str, one per contig.
+    qual (extension): K2q's per-slot qualities on the device, ins_qual the Q of each inserted string (host ints, one
+    per ins_slots entry); K5q then writes the Phred+33 quality text beside the consensus text and the call returns
+    (texts, quality texts)."""
     lib = _ffi.load()
     dev = calls.device
     n_slots = int(calls.shape[0])
@@ -310,13 +330,23 @@ def assemble(calls: torch.Tensor, host: ReadBatch, ins_slots: np.ndarray, ins_st
                               t_is.data_ptr(), t_io.data_ptr(), t_ib.data_ptr(), len(enc), sums.data_ptr(),
                               offsets.data_ptr(), out.data_ptr(), _stream_ptr(dev))
         _ffi.check(rc, "kdl_assemble")
+        if qual is not None:
+            t_iq = put(np.asarray(ins_qual, dtype=np.uint8) if len(enc) else np.zeros(1, dtype=np.uint8))
+            qout = torch.empty_like(out)
+            rc = lib.kdl_assemble_qual(offsets.data_ptr(), qual.data_ptr(), n_slots, t_is.data_ptr(), t_iq.data_ptr(),
+                                       len(enc), qout.data_ptr(), _stream_ptr(dev))
+            _ffi.check(rc, "kdl_assemble_qual")
         starts = torch.from_numpy(np.asarray(host.contig_slot, dtype=np.int64)).to(dev)
         ends = starts + torch.from_numpy(np.asarray(host.contig_len, dtype=np.int64)).to(dev)
         lo = offsets[starts].cpu().numpy().astype(np.int64) & 0xFFFFFFFF
         hi = offsets[ends].cpu().numpy().astype(np.int64) & 0xFFFFFFFF
         total = int(offsets[n_slots].item()) & 0xFFFFFFFF
         text = out[:total].cpu().numpy().tobytes()
-    return [text[a:b].decode("ascii") for a, b in zip(lo.tolist(), hi.tolist())]
+        texts = [text[a:b].decode("ascii") for a, b in zip(lo.tolist(), hi.tolist())]
+        if qual is None:
+            return texts
+        qtext = qout[:total].cpu().numpy().tobytes()
+    return texts, [qtext[a:b].decode("ascii") for a, b in zip(lo.tolist(), hi.tolist())]
 
 
 class HostContext:

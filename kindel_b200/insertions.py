@@ -67,6 +67,13 @@ class InsertionTable:
         """(string, tie) = consensus(insertions[pos])[0], [3]  (kindel.py:369-381)."""
         return dict_consensus(self.dict_at(slot))
 
+    def consensus_count_at(self, slot: int):
+        """(string, tie, count): consensus_at and the chosen string's count in the slot's dict (0 when it is empty),
+        the support of its quality (kindel_b200/quality.py)."""
+        d = self.dict_at(slot)
+        text, tie = dict_consensus(d)
+        return text, tie, int(d.get(text, 0))
+
 
 def dict_consensus(d: dict):
     if not d or not sum(d.values()):

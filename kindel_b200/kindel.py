@@ -20,7 +20,7 @@ from collections import OrderedDict, namedtuple
 
 import numpy as np
 
-from . import bamio, engine
+from . import bamio, engine, quality
 from .insertions import InsertionTable, dict_consensus
 from .views import Alignment, BaseCounts, Insertions
 
@@ -230,14 +230,17 @@ def _device_vote(cols: np.ndarray, min_depth, iupac_threshold=None) -> np.ndarra
     return engine.vote(t, min_depth, iupac_threshold=iupac_threshold).cpu().numpy()[:n]
 
 
-def _emit_range(calls, lo, hi, ins_lookup, out, changes):
+def _emit_range(calls, lo, hi, ins_lookup, out, changes, qual=None, ins_qual=None, qout=None):
     """Append the consensus text of positions [lo, hi) to `out` (kindel.py:413-424).  A bit-7 call (IUPAC vote)
-    emits its ambiguity code; when `changes` keeps an `iupac` list, its 1-based position is added there."""
+    emits its ambiguity code; when `changes` keeps an `iupac` list, its 1-based position is added there.
+    qual (extension): per-position Q (uint8 array like calls); then the Phred+33 text of every emitted character goes
+    to `qout`, an inserted string's from ins_qual(position)."""
     if hi <= lo:
         return
     seg = calls[lo:hi]
     change = (seg >> 4) & 3
     chars = _CALL_LETTERS[seg]
+    qchars = (np.asarray(qual[lo:hi], dtype=np.uint8) + 33).astype(np.uint8) if qual is not None else None
     for k in np.flatnonzero(change).tolist():
         changes[lo + k] = _CHANGE_LUT[change[k]]
     iupac = getattr(changes, "iupac", None)
@@ -245,49 +248,75 @@ def _emit_range(calls, lo, hi, ins_lookup, out, changes):
         iupac.extend(str(lo + k + 1) for k in np.flatnonzero(seg & 0x80).tolist())
     ins_pos = np.flatnonzero(change == 3)
     keep = change != 1
+
+    def emit(a, b):
+        out.append(chars[a:b][keep[a:b]].tobytes().decode("ascii"))
+        if qchars is not None:
+            qout.append(qchars[a:b][keep[a:b]].tobytes().decode("ascii"))
+
     if ins_pos.size == 0:
-        out.append(chars[keep].tobytes().decode("ascii"))
+        emit(0, hi - lo)
         return
     prev = 0
     for k in ins_pos.tolist():
-        out.append(chars[prev:k][keep[prev:k]].tobytes().decode("ascii"))
+        emit(prev, k)
         s, tie = ins_lookup(lo + k)
-        out.append("N" if tie else s.lower())
+        text = "N" if tie else s.lower()
+        out.append(text)
+        if qchars is not None:
+            qout.append(chr(33 + ins_qual(lo + k)) * len(text))
         prev = k
-    out.append(chars[prev:][keep[prev:]].tobytes().decode("ascii"))
+    emit(prev, hi - lo)
 
 
-def assemble_consensus(calls, ins_lookup, cdr_patches=None, trim_ends=False, uppercase=False):
+def assemble_consensus(calls, ins_lookup, cdr_patches=None, trim_ends=False, uppercase=False, qual=None,
+                       ins_qual=None):
     """Call bytes of one contig (length L) -> (consensus string, changes list).
 
     Restates the sequential part of consensus_sequence (kindel.py:387-401, 425-430): CDR patches
     (first Region whose start == pos, provided some Region starting there has a truthy seq) emit
     their lower-cased sequence and skip `end - start - 1` further positions without looking at them.
+    qual / ins_qual (extension): per-position Q (uint8[L]) and the Q of the inserted string at a position; the call
+    then returns (string, changes, quality string), a patch's characters at Q0 and trim_ends cutting both alike.
     """
     L = calls.shape[0]
     changes = _Changes([None] * L)
     changes.iupac = []  # positions of multi-base IUPAC calls that were emitted
     out = []
+    qout = [] if qual is not None else None
     starts = sorted({r.start for r in cdr_patches if r.seq and 0 <= r.start < L}) if cdr_patches else []
     pos = 0
     for st in starts:
         if st < pos:
             continue  # lies inside a span that is being skipped
-        _emit_range(calls, pos, st, ins_lookup, out, changes)
+        _emit_range(calls, pos, st, ins_lookup, out, changes, qual, ins_qual, qout)
         patch = next(r for r in cdr_patches if r.start == st)
         out.append(patch.seq.lower())
+        if qout is not None:
+            qout.append("!" * len(patch.seq))  # no aligned read supports a patch: Q0
         skip = (patch.end - patch.start) - 1
         if skip < 0:  # the reference's counter goes negative and never recovers: nothing more is emitted
             pos = L
             break
         pos = st + 1 + skip
-    _emit_range(calls, pos, L, ins_lookup, out, changes)
+    _emit_range(calls, pos, L, ins_lookup, out, changes, qual, ins_qual, qout)
     seq = "".join(out)
+    quals = "".join(qout) if qout is not None else None
     if trim_ends:
-        seq = seq.strip("N")
+        seq, quals = _trim_n(seq, quals)
     if uppercase:
         seq = seq.upper()
-    return seq, changes
+    return (seq, changes) if qual is None else (seq, changes, quals)
+
+
+def _trim_n(seq, quals=None):
+    """seq.strip("N") (trim_ends), and the quality characters at exactly the stripped positions removed."""
+    left = seq.lstrip("N")
+    out = left.rstrip("N")
+    if quals is None:
+        return out, None
+    a = len(seq) - len(left)
+    return out, quals[a:a + len(out)]
 
 
 def consensus_sequence(weights, insertions, deletions, cdr_patches, trim_ends, min_depth, uppercase,
@@ -300,8 +329,9 @@ def consensus_sequence(weights, insertions, deletions, cdr_patches, trim_ends, m
     return assemble_consensus(calls, lambda p: dict_consensus(insertions[p]), cdr_patches, trim_ends, uppercase)
 
 
-def consensus_seqrecord(consensus, ref_id):
-    return _Sequence(name=f"{ref_id}_cns", sequence=consensus, qualities=None)
+def consensus_seqrecord(consensus, ref_id, qualities=None):
+    """The record of one contig; qualities (extension): its Phred+33 quality string, None when not asked for."""
+    return _Sequence(name=f"{ref_id}_cns", sequence=consensus, qualities=qualities)
 
 
 # ---------------------------------------------------------------- realign (host, kindel.py:156-366)
@@ -524,7 +554,7 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
 # --------------------------------------------------------------------------------- public API
 def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_decay_threshold=0.1,
                      mask_ends=50, trim_ends=False, uppercase=False, devices=None, min_base_quality=0, min_mapq=0,
-                     exclude_flags=0, iupac_threshold=None):
+                     exclude_flags=0, iupac_threshold=None, qualities=False):
     """Consensus sequence(s) of an alignment file (reference kindel/kindel.py:488-555).
 
     Device work per file: one pileup (K1) and one vote (K2) over all contigs at once; only the
@@ -535,7 +565,11 @@ def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_d
     iupac_threshold (extension; default None = off, the reference's vote): t in [0, 1].  Where a base is emitted,
     the call is the smallest set of the most frequent bases (A, C, G, T; N is not an allele) that holds at least
     t * depth of the reads, tied bases entering together, written as its IUPAC code (R = A/G, Y = C/T, ...,
-    N = all four).  The D / N / I changes and the inserted strings are those of the reference's vote."""
+    N = all four).  The D / N / I changes and the inserted strings are those of the reference's vote.
+
+    qualities (extension; default False): every record's `.qualities` is then a Phred+33 string, one character per
+    character of `.sequence` (kindel_b200/quality.py has the rule); the sequence, changes and reports are those of
+    qualities=False.  Off, `.qualities` is None and nothing else runs."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
     filters = (min_base_quality, min_mapq, exclude_flags)
     run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold)
@@ -543,7 +577,7 @@ def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_d
         calls = run.vote(min_depth, iupac_threshold)
     return consensus_from_run(run, calls, bam_path, realign, min_depth, min_overlap,
                               clip_decay_threshold, mask_ends, trim_ends, uppercase, filters=filters,
-                              iupac_threshold=iupac_threshold)
+                              iupac_threshold=iupac_threshold, qualities=qualities)
 
 
 class _Changes(list):
@@ -568,31 +602,97 @@ def _changes_list(calls):
     return out
 
 
-def _device_texts(run, calls_all):
-    """K5: the consensus text of every contig assembled on the device (emitted-length scan + scatter); only the
-    insertion strings of the 'I' sites are resolved on the host (from the event list) and handed over."""
-    batch = run.batch
-    is_ins = ((calls_all >> 4) & 3) == 3
-    slots = np.flatnonzero(is_ins)
-    if slots.size:  # positions only: the extra slot behind a contig never emits (kindel.py:390 loops over weights)
+def _insertion_slots(batch, calls_all):
+    """Ascending slots whose call carries change 'I', positions only: the extra slot behind a contig never emits
+    (kindel.py:390 loops over weights)."""
+    slots = np.flatnonzero(((calls_all >> 4) & 3) == 3)
+    if slots.size:
         c = np.searchsorted(batch.contig_slot, slots, side="right") - 1
         slots = slots[slots < batch.contig_slot[c] + batch.contig_len[c].astype(np.int64)]
+    return slots
+
+
+def _acgt_depth(run, slots):
+    """A + C + G + T at the given slots, from the device table (a gather, not a copy of it) or the host one."""
+    if run.counts is not None:
+        import torch
+
+        idx = torch.from_numpy(np.asarray(slots, dtype=np.int64)).to(run.counts.device)
+        return run.counts[0:4].index_select(1, idx).sum(dim=0, dtype=torch.int64).cpu().numpy()
+    return run.host_counts[0:4, slots].astype(np.int64).sum(axis=0)
+
+
+def _insertion_qualities(run, slots):
+    """{slot: Q of its inserted string} (kindel_b200/quality.py): D = max(min(depth, depth_next), count of the chosen
+    string), the two depths the vote's 'I' rule compares; depth_next at a contig's last position is the empty slot
+    behind it (kindel.py:405-412: 0)."""
+    if len(slots) == 0:
+        return {}
+    slots = np.asarray(slots, dtype=np.int64)
+    depth, depth_next = _acgt_depth(run, slots), _acgt_depth(run, slots + 1)
+    out = {}
+    for sl, d, dn in zip(slots.tolist(), depth.tolist(), depth_next.tolist()):
+        _, tie, k = run.ins_table.consensus_count_at(sl)
+        out[sl] = quality.insertion_phred(d, dn, k, tie)
+    return out
+
+
+def _slot_qualities(run, calls_all):
+    """K2q over the run's table and calls: the device tensor when the table is on the device, else (host tables, e.g.
+    a multi-GPU result) the four base columns and the calls go up to the current device and 1 B per slot comes back."""
+    if run.counts is not None and run.calls_device is not None:
+        return engine.consensus_qual(run.counts, run.calls_device)
+    import torch
+
+    dev = engine.require_cuda()
+    n = calls_all.shape[0]
+    n_pad = (n + 3) // 4 * 4
+    cols = torch.zeros((4, n_pad), dtype=torch.int32, device=dev)
+    calls = torch.zeros(n_pad, dtype=torch.uint8, device=dev)
+    src = run.counts[0:4] if run.counts is not None else torch.from_numpy(np.ascontiguousarray(run.host_counts[0:4]))
+    cols[:, :n] = src.to(dev)
+    calls[:n] = torch.from_numpy(np.ascontiguousarray(calls_all, dtype=np.uint8)).to(dev)
+    return engine.consensus_qual(cols, calls)[:n]
+
+
+def _device_texts(run, calls_all, qual=None, ins_q=None):
+    """K5: the consensus text of every contig assembled on the device (emitted-length scan + scatter); only the
+    insertion strings of the 'I' sites are resolved on the host (from the event list) and handed over.  qual
+    (extension): K2q's device qualities; K5q then adds the quality texts and the call returns (texts, quality
+    texts)."""
+    batch = run.batch
+    slots = _insertion_slots(batch, calls_all)
     strings = []
     for sl in slots.tolist():
         text, tie = run.ins_table.consensus_at(sl)
         strings.append("N" if tie else text.lower())
-    return engine.assemble(run.calls_device, batch, slots, strings)
+    if qual is None:
+        return engine.assemble(run.calls_device, batch, slots, strings)
+    return engine.assemble(run.calls_device, batch, slots, strings, qual=qual,
+                           ins_qual=[ins_q[sl] for sl in slots.tolist()])
 
 
 def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min_overlap=9,
                        clip_decay_threshold=0.1, mask_ends=50, trim_ends=False, uppercase=False, filters=None,
-                       iupac_threshold=None):
+                       iupac_threshold=None, qualities=False):
     """Host half of bam_to_consensus: per contig, optional CDR patches, string assembly, report.  The call bytes
-    already carry the vote; iupac_threshold (extension) only adds its lines to the report."""
+    already carry the vote; iupac_threshold (extension) only adds its lines to the report.  qualities (extension):
+    see bam_to_consensus -- K2q (and, with the device text, K5q) on the device, the host assembly otherwise."""
     ins_table = run.ins_table
     consensuses, refs_changes, refs_reports = [], {}, {}
     on_device = run.counts is not None
-    texts = _device_texts(run, calls_all) if (on_device and not realign and run.calls_device is not None) else None
+    device_text = on_device and not realign and run.calls_device is not None
+    qual_all = ins_q = qtexts = None
+    if qualities:
+        qual_all = _slot_qualities(run, calls_all)
+        ins_q = _insertion_qualities(run, _insertion_slots(run.batch, calls_all))
+        if not device_text:
+            qual_all = qual_all.cpu().numpy()  # 1 B per slot for the host assembly
+    texts = None
+    if device_text:
+        texts = _device_texts(run, calls_all, qual_all, ins_q) if qualities else _device_texts(run, calls_all)
+        if qualities:
+            texts, qtexts = texts
     for c, ref_id in enumerate(run.batch.contig_names):
         s, e = run.contig_slice(c)
         if on_device:
@@ -612,18 +712,25 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
             cdr_patches = merge_cdrps(cdrps, min_overlap)
         else:
             cdr_patches = None
+        quals = None
         if texts is not None:
             cons, changes = texts[c], _changes_list(calls_all[s:e - 1])
+            if qtexts is not None:
+                quals = qtexts[c]
             if trim_ends:
-                cons = cons.strip("N")
+                cons, quals = _trim_n(cons, quals)
             if uppercase:
                 cons = cons.upper()
+        elif qualities:
+            cons, changes, quals = assemble_consensus(
+                calls_all[s:e - 1], lambda p, s=s: ins_table.consensus_at(s + p), cdr_patches, trim_ends, uppercase,
+                qual=qual_all[s:e - 1], ins_qual=lambda p, s=s: ins_q[s + p])
         else:
             cons, changes = assemble_consensus(calls_all[s:e - 1], lambda p, s=s: ins_table.consensus_at(s + p),
                                                cdr_patches, trim_ends, uppercase)
         report = build_report(ref_id, report_weights, changes, cdr_patches, bam_path, realign, min_depth,
                               min_overlap, clip_decay_threshold, trim_ends, uppercase, filters, iupac_threshold)
-        consensuses.append(consensus_seqrecord(cons, ref_id))
+        consensuses.append(consensus_seqrecord(cons, ref_id, quals))
         refs_reports[ref_id] = report
         refs_changes[ref_id] = changes
     return result(consensuses, refs_changes, refs_reports)
