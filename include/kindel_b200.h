@@ -257,6 +257,25 @@ int kdl_consensus_qual(const int32_t* counts, const uint8_t* calls, int64_t n_sl
 int kdl_assemble_qual(const uint32_t* offsets, const uint8_t* qual, int64_t n_slots, const int64_t* ins_slot,
                       const uint8_t* ins_qual, int64_t n_ins, uint8_t* out, void* stream);
 
+/* K6 -- the variant sites of `variants --only-variants` and of the VCF (extension), selected on the device.  At each
+ * position (slots [contig_slot[c], contig_slot[c] + contig_len[c]); never the extra slot behind a contig or the
+ * padding), with t = columns 0-5 of counts (A, C, G, T, N, deletions), depth = their sum and top = the first maximum,
+ * allele k is a variant when t[k] > abs_floor and (double)t[k] / (double)depth > rel_threshold (0 at depth 0) and
+ * k != top; a site is a position with a variant allele.  abs_floor: floor of the absolute threshold clamped to
+ * [-1, 2^31] (2^31 for NaN); rel_threshold: NaN selects nothing.  n_slots % 4 == 0, counts 16-byte aligned.
+ *
+ * kdl_variant_count runs the per-CTA counts and their scan; the number of sites is then block_sums[words - 1], with
+ * block_sums device scratch of words = kdl_variant_scratch_words(n_slots) uint32.  kdl_variant_scatter, on the same
+ * stream after it with the same arguments and n_sites = that number, writes the sites in ascending slot order:
+ * site_slot[i], site_counts[k * n_sites + i] (k = 0..5) and site_mask[i] (bit k: allele k is a variant).  All pointers
+ * are device pointers. */
+int64_t kdl_variant_scratch_words(int64_t n_slots);
+int kdl_variant_count(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                      int32_t n_contigs, int64_t abs_floor, double rel_threshold, uint32_t* block_sums, void* stream);
+int kdl_variant_scatter(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                        int32_t n_contigs, int64_t abs_floor, double rel_threshold, const uint32_t* block_sums,
+                        int64_t n_sites, int64_t* site_slot, int32_t* site_counts, uint8_t* site_mask, void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced

@@ -4,7 +4,8 @@ Sub-commands, flags, defaults and output streams follow the reference: `consensu
 REPORT blocks to stderr and one `>name` / sequence pair per contig to stdout (cli.py:30-33; with the `--fastq`
 extension one FASTQ record per contig instead),
 `weights` / `features` write TSV to stdout (cli.py:44,50), `version` prints `kindel <version>`;
-`variants` (in the reference's README only) is an extension, see kindel.variants.
+`variants` (in the reference's README only) is an extension, see kindel.variants; its `--vcf` writes a sites-only VCF
+(kindel.variants_vcf).
 argh derived the flags from the function signatures (first letter as short option unless two
 parameters share it); argparse spells the same set out.  Note the CLI default `--min-overlap 7`
 (cli.py:13) differs from the API default 9 (kindel.py:492), as in the reference.
@@ -49,11 +50,15 @@ def features(bam_path, gpus=None, **filters):
     kindel.features(bam_path, devices=gpus, **filters).to_csv(sys.stdout, sep="\t", index=False)
 
 
-def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False, absolute=False, **filters):
+def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False, absolute=False, gpus=None, vcf=False,
+             **filters):
     """Output variants exceeding specified absolute and relative frequency thresholds"""
     from . import kindel
 
-    kindel.variants(bam_path, abs_threshold, rel_threshold, only_variants, absolute, **filters).to_csv(
+    if vcf:  # extension: the sites of --only-variants as a sites-only VCF
+        sys.stdout.write(kindel.variants_vcf(bam_path, abs_threshold, rel_threshold, devices=gpus, **filters))
+        return
+    kindel.variants(bam_path, abs_threshold, rel_threshold, only_variants, absolute, devices=gpus, **filters).to_csv(
         sys.stdout, sep="\t", index=False)
 
 
@@ -154,9 +159,13 @@ def build_parser() -> argparse.ArgumentParser:
                    help="relative frequency (0.0-1.0) above which to call variants")
     p.add_argument("-o", "--only-variants", action="store_true", help="exclude invariant sites from output")
     p.add_argument("--absolute", action="store_true", help="report absolute variant frequencies")
+    _add_gpus(p)
     _add_filters(p)
+    # extension: the variant sites as VCF (REF = the sample's most frequent allele; see kindel.variants_vcf)
+    p.add_argument("--vcf", action="store_true",
+                   help="write the variant sites as a sites-only VCF 4.2 instead of the table")
     p.set_defaults(func=lambda a: variants(a.bam_path, a.abs_threshold, a.rel_threshold, a.only_variants, a.absolute,
-                                           **_filters(a)))
+                                           a.gpus, a.vcf, **_filters(a)))
 
     p = sub.add_parser("plot", help=plot.__doc__, description=plot.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")
@@ -167,9 +176,18 @@ def build_parser() -> argparse.ArgumentParser:
     return parser
 
 
+def _check_variants_args(parser, args):
+    # --absolute and --only-variants shape the table; the VCF always holds the variant sites alone
+    if getattr(args, "vcf", False):
+        for flag, on in (("--absolute", args.absolute), ("--only-variants", args.only_variants)):
+            if on:
+                parser.error("variants: --vcf cannot be combined with %s (a table option)" % flag)
+
+
 def main(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
+    _check_variants_args(parser, args)
     if not getattr(args, "func", None):
         parser.print_usage()
         return 1

@@ -12,6 +12,7 @@
 #include "pileup_mask.cu"
 #include "vote.cu"
 #include "assemble.cu"
+#include "variants.cu"
 
 namespace {
 
@@ -392,6 +393,51 @@ int kdl_assemble_qual(const uint32_t* offsets, const uint8_t* qual, int64_t n_sl
     const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
     kdl::assemble_qual_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
         offsets, qual, n_slots, ins_slot, ins_qual, n_ins, out);
+    return check_launch();
+}
+
+int64_t kdl_variant_scratch_words(int64_t n_slots) {
+    return n_slots < 0 ? 0 : (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK + 1;
+}
+
+static int variant_args(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                        int32_t n_contigs, int64_t abs_floor, double rel_threshold, kdl::VariantArgs* a) {
+    // the scan counts sites in uint32; abs_floor outside [-1, 2^31] is a caller that skipped the clamp
+    if (!counts || n_slots <= 0 || (n_slots & 3) || n_slots > (int64_t)UINT32_MAX || n_contigs < 0 ||
+        (n_contigs > 0 && (!contig_slot || !contig_len)) || abs_floor < -1 || abs_floor > (1LL << 31))
+        return KDL_ERR_INVALID_ARG;
+    *a = kdl::VariantArgs{};
+    a->counts = counts; a->n_slots = n_slots;
+    a->layout.contig_slot = contig_slot; a->layout.contig_len = contig_len; a->layout.n_contigs = n_contigs;
+    a->abs_floor = abs_floor; a->rel_threshold = rel_threshold;
+    return KDL_OK;
+}
+
+int kdl_variant_count(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                      int32_t n_contigs, int64_t abs_floor, double rel_threshold, uint32_t* block_sums, void* stream) {
+    kdl::VariantArgs a;
+    int rc = variant_args(counts, n_slots, contig_slot, contig_len, n_contigs, abs_floor, rel_threshold, &a);
+    if (rc != KDL_OK) return rc;
+    if (!block_sums) return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
+    cudaStream_t st = (cudaStream_t)stream;
+    kdl::variant_sums_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, st>>>(a, block_sums);
+    if ((rc = check_launch()) != KDL_OK) return rc;
+    kdl::assemble_scan_sums_kernel<<<1, kdl::A_THREADS, 0, st>>>(block_sums, n_blocks);
+    return check_launch();
+}
+
+int kdl_variant_scatter(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                        int32_t n_contigs, int64_t abs_floor, double rel_threshold, const uint32_t* block_sums,
+                        int64_t n_sites, int64_t* site_slot, int32_t* site_counts, uint8_t* site_mask, void* stream) {
+    kdl::VariantArgs a;
+    int rc = variant_args(counts, n_slots, contig_slot, contig_len, n_contigs, abs_floor, rel_threshold, &a);
+    if (rc != KDL_OK) return rc;
+    if (!block_sums || n_sites < 0 || n_sites > n_slots || (n_sites > 0 && (!site_slot || !site_counts || !site_mask)))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
+    kdl::variant_scatter_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
+        a, block_sums, n_sites, site_slot, site_counts, site_mask);
     return check_launch();
 }
 

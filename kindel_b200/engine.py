@@ -11,6 +11,7 @@ implementation behind these functions: without a CUDA device they raise.
     derive(counts)             derived depth columns [5, n_slots]
     consensus_qual(counts, calls)  K2q: Phred quality of the base each slot emits (extension)
     assemble(calls, ...)       K5 (+ K5q): consensus text (and its quality text) of every contig
+    variant_sites(counts, ...) K6: the variant sites of `variants --only-variants` and the VCF (extension)
 """
 from __future__ import annotations
 
@@ -347,6 +348,52 @@ def assemble(calls: torch.Tensor, host: ReadBatch, ins_slots: np.ndarray, ins_st
             return texts
         qtext = qout[:total].cpu().numpy().tobytes()
     return texts, [qtext[a:b].decode("ascii") for a, b in zip(lo.tolist(), hi.tolist())]
+
+
+def variant_abs_floor(abs_threshold) -> int:
+    """The absolute threshold as K6 takes it: for an integer count t, t > x is t > floor(x), and with counts in
+    [0, 2^31) floor(x) clamped to [-1, 2^31] selects the same counts; NaN selects nothing (2^31)."""
+    if isinstance(abs_threshold, (int, np.integer)):
+        x = int(abs_threshold)
+    else:
+        x = float(abs_threshold)
+        if math.isnan(x):
+            return 1 << 31
+        if math.isinf(x):
+            return 1 << 31 if x > 0 else -1
+        x = math.floor(x)
+    return max(-1, min(1 << 31, x))
+
+
+def variant_sites(counts: torch.Tensor, contig_slot, contig_len, abs_threshold, rel_threshold):
+    """K6 (extension): the variant sites of a device table (int32[>= 6, n_slots], contiguous, n_slots % 4 == 0) --
+    the positions where an allele other than the first most frequent one passes both thresholds (kindel.variant_alleles
+    is the rule).  Returns (slot int64[n], counts int32[6, n], mask uint8[n]) on the host, in ascending slot order;
+    bit k of mask: allele k (A, C, G, T, N, deletions) is a variant.  One 4-byte read-back sizes the result."""
+    lib = _ffi.load()
+    dev = counts.device
+    n_slots = int(counts.shape[1])
+    a, r = variant_abs_floor(abs_threshold), float(rel_threshold)
+    n_contigs = len(contig_len)
+    with torch.cuda.device(dev):
+        t_slot = torch.from_numpy(np.ascontiguousarray(contig_slot, dtype=np.int64) if n_contigs
+                                  else np.zeros(1, dtype=np.int64)).to(dev)
+        t_len = torch.from_numpy(np.ascontiguousarray(contig_len, dtype=np.int32) if n_contigs
+                                 else np.zeros(1, dtype=np.int32)).to(dev)
+        sums = torch.empty(int(lib.kdl_variant_scratch_words(n_slots)), dtype=torch.int32, device=dev)
+        args = (counts.data_ptr(), n_slots, t_slot.data_ptr(), t_len.data_ptr(), n_contigs, a, r, sums.data_ptr())
+        rc = lib.kdl_variant_count(*args, _stream_ptr(dev))
+        _ffi.check(rc, "kdl_variant_count")
+        n = int(sums[-1].item()) & 0xFFFFFFFF
+        site_slot = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+        site_counts = torch.empty((6, max(n, 1)), dtype=torch.int32, device=dev)
+        site_mask = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        rc = lib.kdl_variant_scatter(*args, n, site_slot.data_ptr(), site_counts.data_ptr(), site_mask.data_ptr(),
+                                     _stream_ptr(dev))
+        _ffi.check(rc, "kdl_variant_scatter")
+        if n == 0:
+            return np.zeros(0, dtype=np.int64), np.zeros((6, 0), dtype=np.int32), np.zeros(0, dtype=np.uint8)
+        return site_slot.cpu().numpy(), site_counts[:, :n].cpu().numpy(), site_mask.cpu().numpy()
 
 
 class HostContext:

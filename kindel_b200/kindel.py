@@ -803,42 +803,168 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
     """EXTENSION -- not in the reference snapshot.  The reference's README (README.md:106-107) lists a `variants`
     sub-command ("Output variants exceeding specified absolute and relative frequency thresholds") but its code
     (kindel/kindel.py, kindel/cli.py) has no such function, so there is nothing to be bit-exact with: parity
-    unpinned (SURVEY.md section 8c).  Defined here as a host-side filter over the same integer table `weights`
-    reports: per site, every allele (A, C, G, T, N, deletion) other than the site's most frequent one whose count
-    exceeds `abs_threshold` AND whose share of the depth (A+C+G+T+N+deletions, as in `weights`) exceeds
-    `rel_threshold`.  Columns: chrom, pos, depth, consensus (allele letter, `-` = deletion), then one column per
-    allele holding its relative (default) or absolute frequency where it is a variant and 0 elsewhere."""
+    unpinned (SURVEY.md section 8c).  Defined here as a filter over the same integer table `weights` reports: per
+    site, every allele (A, C, G, T, N, deletion) other than the site's most frequent one whose count exceeds
+    `abs_threshold` AND whose share of the depth (A+C+G+T+N+deletions, as in `weights`) exceeds `rel_threshold`
+    (variant_alleles).  Columns: chrom, pos, depth, consensus (allele letter, `-` = deletion), then one column per
+    allele holding its relative (default) or absolute frequency where it is a variant and 0 elsewhere.  With
+    only_variants the sites are selected on the device (K6, variant_sites) and only they are copied back."""
     run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags)[0]
     return variants_from_run(run, abs_threshold, rel_threshold, only_variants, absolute)
 
 
-def variants_from_run(run, abs_threshold=1, rel_threshold=0.01, only_variants=False, absolute=False):
-    """Host half of `variants` (extension; see there)."""
+_ALLELE_LETTERS = np.array(list("ACGTN-"))
+
+
+def variant_alleles(t, abs_threshold, rel_threshold):
+    """The rule of `variants` (extension) over count columns t (int64 [6, n]: A, C, G, T, N, deletions) ->
+    (depth, top, share, is_var): depth = the sum of the six, top = the first most frequent allele, share = each
+    count's true-division share of the depth (0 at depth 0), and is_var [6, n] = count > abs_threshold and
+    share > rel_threshold and not the top allele.  K6 (kindel_b200/csrc/variants.cu) evaluates the same rule on the
+    device."""
+    depth = t.sum(axis=0)
+    top = t.argmax(axis=0)                                        # first maximum in A,C,G,T,N,del order
+    with np.errstate(invalid="ignore", divide="ignore"):
+        share = np.where(depth > 0, t / np.maximum(depth, 1), 0.0)
+    is_var = (t > abs_threshold) & (share > rel_threshold) & (np.arange(6)[:, None] != top[None, :])
+    return depth, top, share, is_var
+
+
+def variant_sites(run, abs_threshold=1, rel_threshold=0.01):
+    """The sites of `variants --only-variants` (extension): (slot int64[n], counts int32[6, n], mask uint8[n]) in
+    ascending slot order, bit k of mask set where allele k (A, C, G, T, N, deletions) is a variant.  A device run
+    selects them with K6 and copies back only the sites; host tables (e.g. a multi-GPU result) go through
+    variant_alleles."""
+    batch = run.batch
+    if run.counts is not None:
+        return engine.variant_sites(run.counts, batch.contig_slot, batch.contig_len, abs_threshold, rel_threshold)
+    tab = run.host_counts
+    slots, counts, masks = [], [], []
+    for c in range(batch.n_contigs):
+        s, e = run.contig_slice(c)
+        t = tab[0:6, s:e - 1].astype(np.int64)
+        is_var = variant_alleles(t, abs_threshold, rel_threshold)[3]
+        at = np.flatnonzero(is_var.any(axis=0))
+        slots.append(s + at)
+        counts.append(tab[0:6, s + at])
+        masks.append((is_var[:, at].astype(np.uint8) << np.arange(6, dtype=np.uint8)[:, None]).sum(axis=0,
+                                                                                               dtype=np.uint8))
+    if not slots:
+        return np.zeros(0, dtype=np.int64), np.zeros((6, 0), dtype=np.int32), np.zeros(0, dtype=np.uint8)
+    return (np.concatenate(slots).astype(np.int64), np.concatenate(counts, axis=1).astype(np.int32),
+            np.concatenate(masks).astype(np.uint8))
+
+
+def _variants_frame(chrom, pos, t, abs_threshold, rel_threshold, absolute):
+    """The `variants` rows of positions pos (1-based) of one contig with count columns t, and their is_var."""
     import pandas as pd
 
-    tab = run.host_counts
+    depth, top, share, is_var = variant_alleles(t, abs_threshold, rel_threshold)
+    value = np.where(is_var, t if absolute else np.round(share, 4), 0)
+    df = pd.DataFrame({"chrom": [chrom] * pos.shape[0], "pos": pos, "depth": depth,
+                       "consensus": np.where(depth > 0, _ALLELE_LETTERS[top], "N")})
+    for k, a in enumerate(["A", "C", "G", "T", "N", "deletions"]):
+        df[a] = value[k]
+    return df, is_var
+
+
+def variants_from_run(run, abs_threshold=1, rel_threshold=0.01, only_variants=False, absolute=False):
+    """Host half of `variants` (extension; see there).  only_variants: the rows of variant_sites (K6 on a device run:
+    only the sites leave the device), else every position from the whole table."""
+    import pandas as pd
+
     alleles = ["A", "C", "G", "T", "N", "deletions"]
-    rows = [0, 1, 2, 3, 4, 5]
     frames = []
-    for c, chrom in enumerate(run.batch.contig_names):
-        s, e = run.contig_slice(c)
-        L = e - s - 1
-        t = tab[rows, s:s + L].astype(np.int64)                       # [6, L]
-        depth = t.sum(axis=0)
-        top = t.argmax(axis=0)                                        # first maximum in A,C,G,T,N,del order
-        with np.errstate(invalid="ignore", divide="ignore"):
-            share = np.where(depth > 0, t / np.maximum(depth, 1), 0.0)
-        is_var = (t > abs_threshold) & (share > rel_threshold) & (np.arange(6)[:, None] != top[None, :])
-        value = np.where(is_var, t if absolute else np.round(share, 4), 0)
-        df = pd.DataFrame({"chrom": [chrom] * L, "pos": np.arange(1, L + 1, dtype=np.int64), "depth": depth,
-                           "consensus": np.where(depth > 0, np.array(list("ACGTN-"))[top], "N")})
-        for k, a in enumerate(alleles):
-            df[a] = value[k]
-        if only_variants:
-            df = df[is_var.any(axis=0)]
-        frames.append(df)
+    if only_variants:
+        site_slot, site_counts, _ = variant_sites(run, abs_threshold, rel_threshold)
+        for c, chrom in enumerate(run.batch.contig_names):
+            s, e = run.contig_slice(c)
+            lo, hi = np.searchsorted(site_slot, [s, e - 1])
+            if e - 1 == s:  # an empty contig, as below
+                frames.append(_variants_frame(chrom, np.zeros(0, dtype=np.int64), np.zeros((6, 0), dtype=np.int64),
+                                              abs_threshold, rel_threshold, absolute)[0])
+                continue
+            # one more row (an all-zero column, sliced off again) so that pandas infers every column's dtype from a
+            # non-empty column even for a contig without sites, as it does for the per-position frame filtered below
+            pos = np.append(site_slot[lo:hi] - s + 1, 0).astype(np.int64)
+            t = np.zeros((6, hi - lo + 1), dtype=np.int64)
+            t[:, :hi - lo] = site_counts[:, lo:hi]
+            frames.append(_variants_frame(chrom, pos, t, abs_threshold, rel_threshold, absolute)[0].iloc[:hi - lo])
+    else:
+        tab = run.host_counts
+        for c, chrom in enumerate(run.batch.contig_names):
+            s, e = run.contig_slice(c)
+            L = e - s - 1
+            t = tab[0:6, s:s + L].astype(np.int64)                    # [6, L]
+            frames.append(_variants_frame(chrom, np.arange(1, L + 1, dtype=np.int64), t, abs_threshold,
+                                          rel_threshold, absolute)[0])
     cols = ["chrom", "pos", "depth", "consensus"] + alleles
     return pd.concat(frames, ignore_index=True) if frames else pd.DataFrame(columns=cols)
+
+
+# ------------------------------------------------------------------------------------------------ VCF
+_VCF_ALT = ((0, "A"), (1, "C"), (2, "G"), (3, "T"), (5, "*"))  # N (4) is not an allele
+
+
+def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
+                 exclude_flags=0) -> str:
+    """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
+
+    kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
+    file of the sample's minority variants, in the coordinates of the alignment's reference.  Per site: CHROM and the
+    1-based POS; REF the top allele's letter (N when the top allele is N or a deletion, or the depth is 0); ALT the
+    variant alleles among A, C, G, T and the deletion, in that order, the deletion written `*` (VCF 4.2: allele
+    missing due to an upstream deletion, which is what the per-position deletion count is); ID and QUAL `.`, FILTER
+    PASS; INFO DP (the depth A+C+G+T+N+deletions), AD (the REF count, then each ALT's) and AF (each ALT's share of the
+    depth, rounded to 4 decimals: the value `variants` prints).  A site whose only variant allele is N is not
+    written.  devices and the filters: extensions, see pileup_run."""
+    filters = (min_base_quality, min_mapq, exclude_flags)
+    run = pileup_run(bam_path, devices, 1, *filters)[0]
+    return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters)
+
+
+def _vcf_header(run, abs_threshold, rel_threshold, filters):
+    from . import __version__
+
+    mbq, mapq, flags = filters if filters is not None else (0, 0, 0)
+    lines = ["##fileformat=VCFv4.2", "##source=kindel {}".format(__version__),
+             "##kindelVariants=abs_threshold={};rel_threshold={};min_base_quality={};min_mapq={};exclude_flags={:#x}"
+             .format(abs_threshold, rel_threshold, mbq, mapq, flags)]
+    lines += ["##contig=<ID={},length={}>".format(name, int(L))
+              for name, L in zip(run.batch.contig_names, run.batch.contig_len)]
+    lines += ['##INFO=<ID=DP,Number=1,Type=Integer,Description="Depth: A + C + G + T + N + deletions">',
+              '##INFO=<ID=AD,Number=R,Type=Integer,Description="Count of REF (the most frequent allele) and of each '
+              'ALT allele">',
+              '##INFO=<ID=AF,Number=A,Type=Float,Description="Share of the depth of each ALT allele, rounded to 4 '
+              'decimals">',
+              "#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO"]
+    return lines
+
+
+def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None) -> str:
+    """Host half of variants_vcf (see there): the VCF text of a finished pileup.  filters: (min_base_quality,
+    min_mapq, exclude_flags) as the pileup applied them, for the header."""
+    lines = _vcf_header(run, abs_threshold, rel_threshold, filters)
+    site_slot, site_counts, site_mask = variant_sites(run, abs_threshold, rel_threshold)
+    batch = run.batch
+    contig_slot = np.asarray(batch.contig_slot, dtype=np.int64)
+    t = site_counts.astype(np.int64)
+    depth, top, share, _ = variant_alleles(t, abs_threshold, rel_threshold)
+    rounded = np.round(share, 4)
+    contig = np.searchsorted(contig_slot, site_slot, side="right") - 1
+    for i in range(site_slot.shape[0]):
+        m = int(site_mask[i])
+        alts = [(k, letter) for k, letter in _VCF_ALT if m >> k & 1]
+        if not alts:
+            continue  # N alone
+        c = int(contig[i])
+        tp = int(top[i])
+        ref = "ACGT"[tp] if tp < 4 and depth[i] > 0 else "N"
+        info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(str(int(t[k, i])) for k in [tp] + [k for k, _ in alts]),
+                                          ",".join(repr(float(rounded[k, i])) for k, _ in alts))
+        lines.append("\t".join((batch.contig_names[c], str(int(site_slot[i] - contig_slot[c]) + 1), ".", ref,
+                                ",".join(letter for _, letter in alts), ".", "PASS", info)))
+    return "\n".join(lines) + "\n"
 
 
 def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0):

@@ -46,6 +46,8 @@ def row(path: str, d: dict) -> str:
         work += f", IUPAC vote at {d['iupac_threshold']}"
     if d.get("qualities"):
         work += ", + per-base qualities"
+    if d.get("variants"):
+        work += ", + variant sites (K6)"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
            f"{fmt(km.get('k0_k1_pileup'), '.4f')} | {fmt(roof.get('frac'), '.3f')} | {fmt(e2e.get('value'))} | "
            f"{d.get('parity')} |")
