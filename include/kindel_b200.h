@@ -186,6 +186,21 @@ int kdl_pileup(const kdl_batch* batch, int32_t* counts, int64_t n_slots, int32_t
 int kdl_pileup_range(const kdl_batch* batch, int32_t* counts, int64_t n_slots, int64_t slot_lo,
                      int64_t slot_hi, int32_t flags, int32_t* ins_events, int32_t* err_flag, void* stream);
 
+/* kdl_pileup_range with the table's dirty-sector map, so that KDL_PILEUP_ZERO_REST zeroes only what an earlier pileup
+ * wrote instead of all of columns 5..18 (complex reads dirty a few per cent of their 32-byte sectors).
+ *   dirty_map  device uint32[4 * ceil(n_slots / 64)], 16-byte aligned, owned by the caller with the table: one
+ *              16-byte record per 64-slot window w; byte b (0..13) of the record is column 5 + b, bit s of that byte
+ *              covers slots [64 w + 8 s, 64 w + 8 s + 8).
+ *   invariant  a slot of columns 5..18 is non-zero only if its bit is set (a set bit over zeros is always allowed).
+ *              A new table's map is zero with the table; a caller that writes columns 5..18 by other means sets every
+ *              bit (0xFF bytes), and the next pileup with KDL_PILEUP_ZERO_REST zeroes everything.
+ * The pileup keeps the invariant: every kernel that writes columns 5..18 marks what it writes, and the zeroing clears
+ * the records of the windows it has zeroed whole.  A batch with complex reads as dense as 1 in 16 or more dirties nearly
+ * every sector: where the pileup zeroes, it then sets every record of [slot_lo, slot_hi) instead of marking op by op.
+ * NULL = kdl_pileup_range (zeroing of everything, no marking). */
+int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slots, int64_t slot_lo, int64_t slot_hi,
+                         int32_t flags, uint32_t* dirty_map, int32_t* ins_events, int32_t* err_flag, void* stream);
+
 /* K1q -- after kdl_pileup / kdl_pileup_range of the same batch on the same stream: subtracts 1 at the (column, slot)
  * where the pileup counted each masked base (column 4 for M/=/X, 18 for a left clip, 13 for a right clip; nothing for
  * an inserted base).  Launches nothing when qmask->n_reads == 0. */

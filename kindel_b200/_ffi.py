@@ -103,6 +103,8 @@ _PROTOTYPES = {
     "kdl_pileup": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_pileup_range": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                    C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_pileup_range_map": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_diagnose": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p]),
     "kdl_unmask": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_int64, C.c_void_p]),
     "kdl_vote": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),

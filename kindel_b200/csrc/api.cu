@@ -60,13 +60,13 @@ inline int ensure_tile_smem() {
 
 template <int kFlush, bool kCx>
 inline int launch_tile(const kdl_batch& b, int32_t* counts, long long n_slots, long long tile_lo, long long n_tiles,
-                       int split, int zero_rest, cudaStream_t st) {
+                       int split, int zero_rest, uint32_t* dirty_map, uint32_t map_after, cudaStream_t st) {
     int rc = ensure_tile_smem<kFlush, kCx>();
     if (rc != KDL_OK) return rc;
     const long long units = n_tiles * split, max_grid = (long long)sm_count() * 2;  // two CTAs per SM, persistent
     const long long grid = units < max_grid ? units : max_grid;
     kdl::pileup_tile_kernel<kFlush, kCx><<<(unsigned)grid, kdl::W_THREADS, sizeof(kdl::TileSmem<kdl::TileCfg<kCx>>), st>>>(
-        b, counts, n_slots, b.tile_index, tile_lo, n_tiles, split, zero_rest);
+        b, counts, n_slots, b.tile_index, tile_lo, n_tiles, split, zero_rest, dirty_map, map_after);
     return KDL_OK;
 }
 
@@ -113,9 +113,15 @@ int kdl_pileup(const kdl_batch* batch, int32_t* counts, int64_t n_slots, int32_t
 
 int kdl_pileup_range(const kdl_batch* batch, int32_t* counts, int64_t n_slots, int64_t slot_lo,
                      int64_t slot_hi, int32_t flags, int32_t* ins_events, int32_t* err_flag, void* stream) {
+    return kdl_pileup_range_map(batch, counts, n_slots, slot_lo, slot_hi, flags, nullptr, ins_events, err_flag, stream);
+}
+
+int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slots, int64_t slot_lo, int64_t slot_hi,
+                         int32_t flags, uint32_t* dirty_map, int32_t* ins_events, int32_t* err_flag, void* stream) {
     int rc = validate_batch(batch);
     if (rc != KDL_OK) return rc;
-    if (!counts || !err_flag || n_slots <= 0 || slot_lo < 0 || slot_hi > n_slots || slot_lo > slot_hi)
+    if (!counts || !err_flag || n_slots <= 0 || slot_lo < 0 || slot_hi > n_slots || slot_lo > slot_hi ||
+        (reinterpret_cast<uintptr_t>(dirty_map) & 15))
         return KDL_ERR_INVALID_ARG;
     const bool tileable = (n_slots % KDL_TILE) == 0 && (slot_lo % KDL_TILE) == 0 && (slot_hi % KDL_TILE) == 0;
     if ((slot_lo & 3) || (slot_hi & 3)) return KDL_ERR_INVALID_ARG;
@@ -142,14 +148,26 @@ int kdl_pileup_range(const kdl_batch* batch, int32_t* counts, int64_t n_slots, i
     bool cx_by_atomics = (batch->n_complex - batch->n_hard) * 16 < batch->n_reads;
     if (const char* ev = getenv("KDL_CX")) cx_by_atomics = !strcmp(ev, "atomics") ? true : (!strcmp(ev, "pieces") ? false : cx_by_atomics);
     // zeroing that the chosen kernels will not do themselves: the tile kernel overwrites the weight columns of a
-    // fresh table and, on request, zeroes columns 5..18 window by window in its flush
+    // fresh table and, on request, zeroes columns 5..18 window by window in its flush (only the sectors the map marks)
     const int zero_in_k1 = (tiled && split == 1 && fresh && n_tiles > 0 && (flags & KDL_PILEUP_ZERO_REST)) ? 1 : 0;
     const int zero_from = (fresh && !(tiled && split == 1)) ? 0 : 5;
     const int zero_to = ((flags & KDL_PILEUP_ZERO_REST) && !zero_in_k1) ? KDL_NCOL : 5;
-    if (zero_to > zero_from && slot_hi > slot_lo) {
-        kdl::zero_cols_kernel<<<sm_count() * 4, 256, 0, st>>>(counts, n_slots, zero_from, zero_to, slot_lo, slot_hi);
+    const bool zero_pass = zero_to > zero_from && slot_hi > slot_lo;
+    // The dirty-sector map.  Complex reads this dense (>= 1 in 16; a few per cent of sectors stay clean at 1 in 100)
+    // dirty nearly every sector: instead of K1e / K1g marking op by op, the kernel that zeroes -- K1's flush, or the
+    // zeroing pass -- leaves every record of the range set, and the next pileup zeroes all of it.  Where neither runs,
+    // the writers mark.
+    const bool k1_stores = tiled && split == 1 && fresh && n_tiles > 0;
+    const bool saturate = dirty_map && batch->n_complex > 0 && batch->n_complex * 16 >= batch->n_reads &&
+                          (k1_stores || zero_pass);
+    uint32_t* mark_map = saturate ? nullptr : dirty_map;
+    if (zero_pass) {
+        uint32_t* zmap = saturate || (zero_from <= 5 && zero_to == KDL_NCOL) ? dirty_map : nullptr;
+        kdl::zero_cols_kernel<<<sm_count() * 4, 256, 0, st>>>(counts, n_slots, zero_from, zero_to, slot_lo, slot_hi,
+                                                              zmap, saturate ? ~0u : 0u);
         if ((rc = check_launch()) != KDL_OK) return rc;
     }
+    const uint32_t map_after = saturate && k1_stores ? ~0u : 0u;
     if (batch->n_reads == 0) return KDL_OK;
     if (tiled) {
         if (n_tiles > 0) {
@@ -162,14 +180,16 @@ int kdl_pileup_range(const kdl_batch* batch, int32_t* counts, int64_t n_slots, i
             // runs and K1e counts their bases too, with REDs
             const bool cx = batch->n_complex > batch->n_hard && !cx_by_atomics;
             if (split > 1) {
-                rc = cx ? launch_tile<kdl::F_ATOMIC, true>(*batch, counts, n_slots, tile_lo, n_tiles, split, 0, st)
-                        : launch_tile<kdl::F_ATOMIC, false>(*batch, counts, n_slots, tile_lo, n_tiles, split, 0, st);
+                rc = cx ? launch_tile<kdl::F_ATOMIC, true>(*batch, counts, n_slots, tile_lo, n_tiles, split, 0, nullptr, 0, st)
+                        : launch_tile<kdl::F_ATOMIC, false>(*batch, counts, n_slots, tile_lo, n_tiles, split, 0, nullptr, 0, st);
             } else if (fresh) {
-                rc = cx ? launch_tile<kdl::F_STORE, true>(*batch, counts, n_slots, tile_lo, n_tiles, 1, zero_in_k1, st)
-                        : launch_tile<kdl::F_STORE, false>(*batch, counts, n_slots, tile_lo, n_tiles, 1, zero_in_k1, st);
+                rc = cx ? launch_tile<kdl::F_STORE, true>(*batch, counts, n_slots, tile_lo, n_tiles, 1, zero_in_k1, dirty_map,
+                                                          map_after, st)
+                        : launch_tile<kdl::F_STORE, false>(*batch, counts, n_slots, tile_lo, n_tiles, 1, zero_in_k1, dirty_map,
+                                                           map_after, st);
             } else {
-                rc = cx ? launch_tile<kdl::F_ADD, true>(*batch, counts, n_slots, tile_lo, n_tiles, 1, 0, st)
-                        : launch_tile<kdl::F_ADD, false>(*batch, counts, n_slots, tile_lo, n_tiles, 1, 0, st);
+                rc = cx ? launch_tile<kdl::F_ADD, true>(*batch, counts, n_slots, tile_lo, n_tiles, 1, 0, nullptr, 0, st)
+                        : launch_tile<kdl::F_ADD, false>(*batch, counts, n_slots, tile_lo, n_tiles, 1, 0, nullptr, 0, st);
             }
             if (rc != KDL_OK) return rc;
             if ((rc = check_launch()) != KDL_OK) return rc;
@@ -177,16 +197,16 @@ int kdl_pileup_range(const kdl_batch* batch, int32_t* counts, int64_t n_slots, i
         if (batch->n_complex > batch->n_hard) {  // K1e: insertions / deletions / clips of the tile-eligible complex reads
             if (cx_by_atomics)  // their bases too: 8 lanes per read
                 kdl::pileup_events_kernel<8><<<(unsigned)((batch->n_complex + 31) / 32), 256, 0, st>>>(
-                    *batch, counts, n_slots, ins_events, 1);
+                    *batch, counts, n_slots, ins_events, 1, mark_map);
             else                // a few scattered REDs per read: one thread per read
                 kdl::pileup_events_kernel<1><<<(unsigned)((batch->n_complex + 255) / 256), 256, 0, st>>>(
-                    *batch, counts, n_slots, ins_events, 0);
+                    *batch, counts, n_slots, ins_events, 0, mark_map);
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
         if (batch->n_hard > 0) {  // K1g: the reads that may wrap or raise, atomically, after the tile stores
             const int grid = grid_for(batch->n_hard, 8, cap);
             kdl::pileup_general_kernel<<<grid, 256, 0, st>>>(*batch, batch->hard_idx, batch->n_hard, counts, n_slots,
-                                                            ins_events, err_flag);
+                                                            ins_events, err_flag, mark_map);
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
     } else {
@@ -199,7 +219,7 @@ int kdl_pileup_range(const kdl_batch* batch, int32_t* counts, int64_t n_slots, i
         if (batch->n_complex > 0) {
             const int grid = grid_for(batch->n_reads, 8, cap);
             kdl::pileup_general_kernel<<<grid, 256, 0, st>>>(*batch, nullptr, batch->n_reads, counts, n_slots,
-                                                            ins_events, err_flag);
+                                                            ins_events, err_flag, mark_map);
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
     }

@@ -53,6 +53,40 @@ __device__ __forceinline__ int find_contig(const int64_t* __restrict__ off, int 
     return lo;
 }
 
+// ---- dirty-sector map of columns 5..18 (kdl_pileup_range_map, include/kindel_b200.h) --------------------------
+// uint32 map[4 * ceil(n_slots / 64)]: one 16-byte record per 64-slot window w; byte b (0..13) of the record is column
+// 5 + b, bit s of that byte stands for slots [64 w + 8 s, 64 w + 8 s + 8) -- one 32-byte sector of the column.  A slot
+// of columns 5..18 is non-zero only if its bit is set; a set bit over a zero sector is always allowed.
+// mark_dirty sets the bits of columns [col, col + n_col) over slots [s0, s1): one atomicOr per record word touched,
+// a handful per CIGAR op (the map is small enough to stay in L2).
+__device__ __forceinline__ void mark_dirty(uint32_t* __restrict__ map, int col, int n_col, long long s0, long long s1) {
+    if (s0 >= s1) return;
+    const uint32_t bytes = ((1u << n_col) - 1u) << (col - KDL_DEL);  // bytes of the record the columns own
+    uint32_t* rec = map + 4 * (s0 >> 6);
+    int lo = (int)(s0 & 63), left = (int)(s1 - s0);  // (one CIGAR op: fewer than 2^28 slots)
+    do {                                              // the windows [s0, s1) meets, from slot lo of the first
+        const int hi = left < 64 - lo ? lo + left : 64;
+        const uint32_t sec = ((2u << ((hi - 1) >> 3)) - 1u) & ~((1u << (lo >> 3)) - 1u);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint32_t nib = (bytes >> (4 * k)) & 0xFu;
+            const uint32_t v = sec * ((nib & 1u) | ((nib & 2u) << 7) | ((nib & 4u) << 14) | ((nib & 8u) << 21));
+            if (v) atomicOr(rec + k, v);
+        }
+        left -= hi - lo;
+        lo = 0;
+        rec += 4;
+    } while (left > 0);
+}
+
+// mark_dirty of the slots base + pyindex(i, n) for i in [lo, hi) that exist: the negative part wraps by n
+__device__ __forceinline__ void mark_dirty_py(uint32_t* __restrict__ map, int col, int n_col, long long base,
+                                              long long lo, long long hi, long long n) {
+    const long long a = lo > -n ? lo : -n, e = hi < 0 ? hi : 0;
+    if (a < e) mark_dirty(map, col, n_col, base + a + n, base + e + n);
+    mark_dirty(map, col, n_col, base + (lo > 0 ? lo : 0), base + (hi < n ? hi : n));
+}
+
 // consensus() over the five base counts (kindel/kindel.py:369-381): first maximum in dict order
 // A,T,G,C,N; all-zero -> N with no tie; tie = another key holds the same non-zero maximum.
 // Returns the emitted code (tie -> 4 = N) and the consensus key's count through *freq.

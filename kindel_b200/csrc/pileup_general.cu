@@ -21,8 +21,10 @@ namespace kdl {
 
 __global__ void __launch_bounds__(256)
 pileup_general_kernel(kdl_batch b, const uint32_t* __restrict__ list, long long n_list, int32_t* __restrict__ counts,
-                      long long n_slots, int32_t* __restrict__ ins_events, int32_t* __restrict__ err_flag) {
+                      long long n_slots, int32_t* __restrict__ ins_events, int32_t* __restrict__ err_flag,
+                      uint32_t* __restrict__ dirty_map = nullptr) {
     const int lane = threadIdx.x & 31;
+    const bool marks = dirty_map != nullptr && lane == 0;  // (the ops are warp-uniform: lane 0 marks their sectors)
     const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
     bool bad = false;
@@ -59,6 +61,7 @@ pileup_general_kernel(kdl_batch b, const uint32_t* __restrict__ list, long long 
                 r_pos += len;
                 q_pos += len;
             } else if (op == 1) {  // I
+                if (marks) mark_dirty_py(dirty_map, KDL_INS, 1, base, r_pos, r_pos + 1, L + 1);
                 if (lane == 0) {
                     const long long idx = pyindex(r_pos, L + 1);
                     if (idx < 0) {
@@ -74,6 +77,7 @@ pileup_general_kernel(kdl_batch b, const uint32_t* __restrict__ list, long long 
                 evt += 1;
                 q_pos += len;
             } else if (op == 2) {  // D
+                if (marks) mark_dirty_py(dirty_map, KDL_DEL, 1, base, r_pos, r_pos + len, L + 1);
                 for (long long k = lane; k < len; k += 32) {
                     const long long idx = pyindex(r_pos + k, L + 1);
                     if (idx < 0) { bad = true; continue; }
@@ -82,6 +86,11 @@ pileup_general_kernel(kdl_batch b, const uint32_t* __restrict__ list, long long 
                 r_pos += len;
             } else if (op == 4) {  // S
                 if (i == c0) {     // left clip: only when it is op #0 (kindel.py:64)
+                    if (marks) {
+                        mark_dirty_py(dirty_map, KDL_CLIP_ENDS, 1, base, r_pos, r_pos + 1, L + 1);
+                        mark_dirty(dirty_map, KDL_CEW_A, 5, base + (r_pos - len > 0 ? r_pos - len : 0),
+                                   base + (r_pos < L ? r_pos : L));  // (bases left of the contig are skipped, not wrapped)
+                    }
                     if (lane == 0) {
                         const long long idx = pyindex(r_pos, L + 1);
                         if (idx < 0) bad = true;
@@ -106,6 +115,10 @@ pileup_general_kernel(kdl_batch b, const uint32_t* __restrict__ list, long long 
                     // iterations that advance: while r_pos < L (kindel.py:78-81)
                     long long n_adv = L - r_pos;
                     n_adv = n_adv < 0 ? 0 : (n_adv > len ? len : n_adv);
+                    if (marks) {
+                        mark_dirty_py(dirty_map, KDL_CLIP_STARTS, 1, base, r_pos - 1, r_pos, L + 1);
+                        mark_dirty_py(dirty_map, KDL_CSW_A, 5, base, r_pos, r_pos + n_adv, L);
+                    }
                     for (long long k = lane; k < n_adv; k += 32) {
                         const long long q = q_pos + k;
                         const long long idx = pyindex(r_pos + k, L);
@@ -132,6 +145,7 @@ pileup_general_kernel(kdl_batch b, const uint32_t* __restrict__ list, long long 
 // increments per read, done here once per read with REDs.  By the flatten contract such a read cannot wrap an index
 // or raise: no checks.  Insertion events go to their deterministic rows.
 //
+// dirty_map (may be NULL): the sectors of columns 5..18 these updates touch are marked there, once per op range.
 // with_m: also count the reads' M/=/X bases here, with REDs into the weight columns -- what kdl_pileup_range asks
 // for when tile-eligible complex reads are RARE (a few per cent of a short-read BAM): the tile kernel then runs its
 // lean instantiation and treats them as inert, and their ~130 bases each cost less as atomics than the piece
@@ -143,7 +157,7 @@ pileup_general_kernel(kdl_batch b, const uint32_t* __restrict__ list, long long 
 template <int kLanes>
 __global__ void __launch_bounds__(256)
 pileup_events_kernel(kdl_batch b, int32_t* __restrict__ counts, long long n_slots, int32_t* __restrict__ ins_events,
-                     int with_m) {
+                     int with_m, uint32_t* __restrict__ dirty_map = nullptr) {
     const int lane = (int)(threadIdx.x % kLanes);
     constexpr int kStep = kLanes;
     const long long gtid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -162,6 +176,7 @@ pileup_events_kernel(kdl_batch b, int32_t* __restrict__ counts, long long n_slot
     const uint32_t* __restrict__ ops = blk + 2;
     long long r_pos = b.ref_start[r];
     int q_pos = 0;
+    const bool marks = dirty_map != nullptr && lane == 0;
     for (int o = 0; o < n_ops; ++o) {
         const uint32_t cg = ops[o];
         const int len = (int)(cg >> 4);
@@ -174,6 +189,7 @@ pileup_events_kernel(kdl_batch b, int32_t* __restrict__ counts, long long n_slot
             q_pos += len;
         } else if (op == 1) {  // I
             if (lane == 0) {
+                if (marks) mark_dirty(dirty_map, KDL_INS, 1, slot0 + r_pos, slot0 + r_pos + 1);
                 atomicAdd(tab + (long long)KDL_INS * n_slots + r_pos, 1);
                 if (ins_events)
                     reinterpret_cast<int4*>(ins_events)[evt] = make_int4((int)(slot0 + r_pos), (int)r, q_pos, len);
@@ -181,10 +197,15 @@ pileup_events_kernel(kdl_batch b, int32_t* __restrict__ counts, long long n_slot
             evt += 1;
             q_pos += len;
         } else if (op == 2) {  // D
+            if (marks) mark_dirty(dirty_map, KDL_DEL, 1, slot0 + r_pos, slot0 + r_pos + len);
             for (int d = lane; d < len; d += kStep) atomicAdd(tab + (long long)KDL_DEL * n_slots + r_pos + d, 1);
             r_pos += len;
         } else if (op == 4) {  // S
             if (o == 0) {      // left clip: its bases end where the read starts
+                if (marks) {
+                    mark_dirty(dirty_map, KDL_CLIP_ENDS, 1, slot0 + r_pos, slot0 + r_pos + 1);
+                    mark_dirty(dirty_map, KDL_CEW_A, 5, slot0 + (r_pos - len > 0 ? r_pos - len : 0), slot0 + r_pos);
+                }
                 if (lane == 0) atomicAdd(tab + (long long)KDL_CLIP_ENDS * n_slots + r_pos, 1);
                 for (int g = lane; g < len; g += kStep) {
                     const long long rel = r_pos - len + g;
@@ -192,6 +213,10 @@ pileup_events_kernel(kdl_batch b, int32_t* __restrict__ counts, long long n_slot
                 }
                 q_pos += len;
             } else {           // right clip (never reaches the contig end for these reads)
+                if (marks) {
+                    mark_dirty(dirty_map, KDL_CLIP_STARTS, 1, slot0 + r_pos - 1, slot0 + r_pos);
+                    mark_dirty(dirty_map, KDL_CSW_A, 5, slot0 + r_pos, slot0 + r_pos + len);
+                }
                 if (lane == 0) atomicAdd(tab + (long long)KDL_CLIP_STARTS * n_slots + r_pos - 1, 1);
                 for (int d = lane; d < len; d += kStep)
                     atomicAdd(tab + (long long)(KDL_CSW_A + nib2col(nibble_at(seq, q_pos + d))) * n_slots + r_pos + d, 1);

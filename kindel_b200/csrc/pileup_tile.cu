@@ -136,11 +136,16 @@ static_assert(TileCfg<true>::kPcap >= KDL_TILE_MAXOPS && TileCfg<true>::kPcap < 
 
 // kFlush: F_STORE = the weight columns hold stale data (first flush of a window stores, untouched tiles are stored
 // as zeros); F_ADD = add to what is there; F_ATOMIC = `split` CTAs share a tile, the table was zeroed, flush with REDs.
+// zero_rest (F_STORE): columns 5..18 hold an earlier pileup's sparse counts; the final flush of a window zeroes them --
+// all of them, or, given the dirty-sector map (kdl_common.cuh), only the sectors it marks.  map_after (F_STORE, with
+// the map): what the window's record holds after the flush -- 0 when K1e / K1g will mark what they write, all ones when
+// they will not (complex reads so dense that nearly every sector is dirty anyway).  Without them (the defaults) no map is read
+// or written.
 template <int kFlush, bool kCx>
 __global__ void __launch_bounds__(W_THREADS, 2)
 pileup_tile_kernel(kdl_batch b, int32_t* __restrict__ counts, long long n_slots,
                    const uint32_t* __restrict__ tile_index, long long tile_lo, long long n_tiles, int split,
-                   int zero_rest) {
+                   int zero_rest, uint32_t* __restrict__ dirty_map = nullptr, uint32_t map_after = 0u) {
     KDL_DYNAMIC_SMEM(smem_raw);
     using C = TileCfg<kCx>;
     using Smem = TileSmem<C>;
@@ -704,15 +709,32 @@ pileup_tile_kernel(kdl_batch b, int32_t* __restrict__ counts, long long n_slots,
             }
             if (kFresh && !stored) flush_window<F_STORE, true>(acc, rawacc, covacc, counts, n_slots, tile_slot + wlo, lane);
             else flush_window<kAdd, true>(acc, rawacc, covacc, counts, n_slots, tile_slot + wlo, lane);
+            uint4* mrec = kFresh && dirty_map ? reinterpret_cast<uint4*>(dirty_map) + ((tile_slot + wlo) >> 6) : nullptr;
+            uint4 rec = make_uint4(~0u, ~0u, ~0u, ~0u);
             if (kFresh && zero_rest) {
                 // columns 5..18 of the window hold an earlier pileup's sparse counts: zero them here, under the
-                // counting, instead of in a pass of their own (K1e / K1g add to them after this kernel)
+                // counting, instead of in a pass of their own (K1e / K1g add to them after this kernel).  Lane
+                // lane & 7 owns sector lane & 7 of each column; quarter q takes columns 5 + q + 4 k, which are byte q
+                // of word k of the window's map record.
                 int32_t* z = counts + tile_slot + wlo + 8 * (lane & 7);
-                for (int col = 5 + quarter; col < KDL_NCOL; col += 4) {
-                    int4* zp = reinterpret_cast<int4*>(z + (long long)col * n_slots);
-                    zp[0] = make_int4(0, 0, 0, 0);
-                    zp[1] = make_int4(0, 0, 0, 0);
+                if (mrec) rec = *mrec;
+                const int sh = 8 * quarter + (lane & 7);
+                const uint32_t mine = ((rec.x >> sh) & 1u) | (((rec.y >> sh) & 1u) << 1) | (((rec.z >> sh) & 1u) << 2) |
+                                      (((rec.w >> sh) & 1u) << 3);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const int col = 5 + quarter + 4 * k;
+                    if (col < KDL_NCOL && ((mine >> k) & 1u)) {
+                        int4* zp = reinterpret_cast<int4*>(z + (long long)col * n_slots);
+                        zp[0] = make_int4(0, 0, 0, 0);
+                        zp[1] = make_int4(0, 0, 0, 0);
+                    }
                 }
+                __syncwarp();  // every lane has read the record
+            }
+            if (mrec && lane == 0) {  // (without zero_rest the record is only replaced by all ones)
+                const bool differs = rec.x != map_after || rec.y != map_after || rec.z != map_after || rec.w != map_after;
+                if (zero_rest ? differs : map_after != 0u) *mrec = make_uint4(map_after, map_after, map_after, map_after);
             }
             blocks_since_flush = 0;
         }

@@ -408,16 +408,25 @@ __device__ __forceinline__ void flush_window(Planes& acc, int (&rawacc)[8], cons
     }
 }
 
-// zero columns [col_lo, col_hi) of slots [slot_lo, slot_hi) (multiples of 4), 128-bit stores
+// zero columns [col_lo, col_hi) of slots [slot_lo, slot_hi) (multiples of 4), 128-bit stores.  dirty_map (may be NULL):
+// map_fill = 0 (given only when the columns include all of 5..18) clears the records of the 64-slot windows wholly
+// inside the range; all ones sets the records of every window the range meets (K1e / K1g will not mark).
 __global__ void __launch_bounds__(256)
 zero_cols_kernel(int32_t* __restrict__ counts, long long n_slots, int col_lo, int col_hi, long long slot_lo,
-                 long long slot_hi) {
+                 long long slot_hi, uint32_t* __restrict__ dirty_map = nullptr, uint32_t map_fill = 0u) {
     const long long per_col = (slot_hi - slot_lo) >> 2;
     const long long total = per_col * (col_hi - col_lo);
-    for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < total;
-         v += (long long)gridDim.x * blockDim.x) {
+    const long long gtid = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
+    for (long long v = gtid; v < total; v += stride) {
         const long long col = col_lo + v / per_col, off = v % per_col;
         reinterpret_cast<int4*>(counts + col * n_slots + slot_lo)[off] = make_int4(0, 0, 0, 0);
+    }
+    if (dirty_map) {
+        const bool whole = map_fill == 0 && slot_hi != n_slots;  // (the last window of the table may be short)
+        const long long w_lo = map_fill ? slot_lo >> 6 : (slot_lo + 63) >> 6;
+        const long long w_hi = whole ? slot_hi >> 6 : (slot_hi + 63) >> 6;
+        for (long long w = w_lo + gtid; w < w_hi; w += stride)
+            reinterpret_cast<uint4*>(dirty_map)[w] = make_uint4(map_fill, map_fill, map_fill, map_fill);
     }
 }
 

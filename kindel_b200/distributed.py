@@ -321,7 +321,7 @@ class ShardedConsensus:
         if self.mode == "allreduce":
             # the all_reduce writes sums everywhere: the whole table is dirty every step
             table.dirty = (0, self.n_slots)
-            table.dirty_rest = True  # columns 5, 6 hold sums over ALL ranks after the all_reduce
+            table.dirty_rest = True  # columns 5, 6 hold sums over ALL ranks after the all_reduce: all of the map set
             engine.pileup(self.dbatch, check=False, table=table)
         else:  # only this shard's footprint is ever touched (kdl_table_alloc zero-filled the rest)
             engine.pileup(self.dbatch, check=False, table=table, slot_range=self.foot)

@@ -145,15 +145,32 @@ class CountTable:
     It remembers which slot range earlier pileups may have dirtied and whether the non-weight
     columns (5..18: indels, clips -- only complex reads write them) are dirty, and asks the kernels
     to overwrite / zero exactly that (KDL_PILEUP_FRESH_WEIGHTS / KDL_PILEUP_ZERO_REST) instead of
-    clearing 76 bytes per slot every time."""
+    clearing 76 bytes per slot every time.  Inside columns 5..18 its dirty-sector map (`dirty_map`,
+    kdl_pileup_range_map) narrows the zeroing to the 32-byte sectors complex reads wrote.
+
+    A table adopted from a caller's tensor starts with every sector marked dirty.  Setting `dirty_rest = True`
+    from outside says columns 5..18 were written by other means: every sector is marked dirty again."""
 
     def __init__(self, n_slots: int, device, tensor: torch.Tensor = None):
         self.n_slots = n_slots
         self.device = device
         self.t = tensor if tensor is not None else torch.zeros((_ffi.KDL_NCOL, n_slots), dtype=torch.int32,
                                                                 device=device)
-        self.dirty = None        # (lo, hi) slot range holding counts of an earlier pileup
-        self.dirty_rest = False  # columns 5..18 non-zero somewhere inside `dirty`
+        # uint32 per word (held as int32): 16 bytes per 64-slot window, byte b = column 5 + b, bit s = sector s
+        self.dirty_map = torch.full((4 * ((n_slots + 63) // 64),), 0 if tensor is None else -1, dtype=torch.int32,
+                                    device=device)
+        self.dirty = None         # (lo, hi) slot range holding counts of an earlier pileup
+        self._dirty_rest = False  # columns 5..18 non-zero somewhere inside `dirty` (where: dirty_map)
+
+    @property
+    def dirty_rest(self) -> bool:
+        return self._dirty_rest
+
+    @dirty_rest.setter
+    def dirty_rest(self, value: bool):
+        if value:
+            self.dirty_map.fill_(-1)
+        self._dirty_rest = bool(value)
 
 
 def _tile_align(lo: int, hi: int, n_slots: int):
@@ -192,10 +209,11 @@ def pileup(dbatch: DeviceBatch, counts: torch.Tensor = None, check: bool = True,
                 lo, hi = min(lo, table.dirty[0]), max(hi, table.dirty[1])
             lo, hi = _tile_align(lo, hi, n_slots)
             flags = _ffi.KDL_PILEUP_FRESH_WEIGHTS | (_ffi.KDL_PILEUP_ZERO_REST if table.dirty_rest else 0)
-            rc = lib.kdl_pileup_range(C.byref(dbatch.struct), counts.data_ptr(), n_slots, lo, hi, flags,
-                                      events.data_ptr(), flag.data_ptr(), _stream_ptr(dev))
+            rc = lib.kdl_pileup_range_map(C.byref(dbatch.struct), counts.data_ptr(), n_slots, lo, hi, flags,
+                                          table.dirty_map.data_ptr(), events.data_ptr(), flag.data_ptr(),
+                                          _stream_ptr(dev))
             table.dirty = (lo, hi)
-            table.dirty_rest = dbatch.host.n_complex > 0
+            table._dirty_rest = dbatch.host.n_complex > 0  # (the kernels marked where in the map)
         else:
             if counts is None:
                 counts = torch.zeros((_ffi.KDL_NCOL, n_slots), dtype=torch.int32, device=dev)

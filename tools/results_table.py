@@ -35,7 +35,7 @@ def row(path: str, d: dict) -> str:
         return (f"| `{name}` | reference arm ({cb.get('kind', '?')}, {cb.get('cores', '?')} core) | 1 host | — | "
                 f"{fmt(d.get('value'))} | — | — | — | — |")
     cfg = d.get("config", {})
-    roof = d.get("roofline", {})
+    roof = d.get("roofline") or {}  # (null on a line that does not take the roofline)
     e2e = d.get("e2e") or {}  # (null on an --iupac-threshold line: the host-buffer call has no IUPAC vote)
     km = d.get("kernels_ms", {})
     work = cfg.get("workload", "?")
@@ -48,6 +48,8 @@ def row(path: str, d: dict) -> str:
         work += ", + per-base qualities"
     if d.get("variants"):
         work += ", + variant sites (K6)"
+    if d.get("map_ab"):
+        work += ", zeroing A/B (dirty-sector map)"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
            f"{fmt(km.get('k0_k1_pileup'), '.4f')} | {fmt(roof.get('frac'), '.3f')} | {fmt(e2e.get('value'))} | "
            f"{d.get('parity')} |")
