@@ -309,13 +309,19 @@ class ShardedConsensus:
         `timers`: optional pair of CUDA events recorded around K1 (bench.py's roofline leg).
         iupac_threshold (extension): the IUPAC vote (kdl_vote_iupac) in "fused" and "allreduce" mode; "peer" mode
         has no such vote and raises ValueError."""
-        torch, dist, engine = self.torch, self.dist, self.engine
-        iupac_threshold = engine.check_iupac_threshold(iupac_threshold)
+        iupac_threshold = self.engine.check_iupac_threshold(iupac_threshold)
         if iupac_threshold is not None and self.mode == "peer":
             raise ValueError("iupac_threshold needs exchange mode 'fused' or 'allreduce', not 'peer'")
+        self.pile(timers)
+        return self.exchange(min_depth, iupac_threshold)
+
+    def pile(self, timers=None):
+        """First half of `step()`: the next epoch's parity table gets K1 on the shard.  A single process that drives
+        several ranks on one stream issues every rank's `pile` before any rank's `exchange`: the fused vote waits
+        for the peers' tables of the same epoch."""
+        engine = self.engine
         self.epoch += 1
-        par = self.epoch & 1
-        table = self.table[par]
+        table = self.table[self.epoch & 1]
         if timers:
             timers[0].record()
         if self.mode == "allreduce":
@@ -327,6 +333,16 @@ class ShardedConsensus:
             engine.pileup(self.dbatch, check=False, table=table, slot_range=self.foot)
         if timers:
             timers[1].record()
+
+    def exchange(self, min_depth=1, iupac_threshold=None):
+        """Second half of `step()`: the exchange and the vote of the epoch `pile` started.  Returns the complete call
+        bytes on every rank."""
+        torch, dist, engine = self.torch, self.dist, self.engine
+        iupac_threshold = engine.check_iupac_threshold(iupac_threshold)
+        if iupac_threshold is not None and self.mode == "peer":
+            raise ValueError("iupac_threshold needs exchange mode 'fused' or 'allreduce', not 'peer'")
+        par = self.epoch & 1
+        table = self.table[par]
         if self.mode == "fused":
             st = int(torch.cuda.current_stream(self.device).cuda_stream)
             with torch.cuda.device(self.device):

@@ -44,7 +44,8 @@ def load():
     lib.emu_map_last_error.restype = C.c_char_p
     lib.emu_map_pileup.restype = C.c_int
     vp = C.c_void_p
-    lib.emu_map_pileup.argtypes = [C.POINTER(_ffi.KdlBatch), vp, C.c_longlong, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp,
+    ll = C.c_longlong
+    lib.emu_map_pileup.argtypes = [C.POINTER(_ffi.KdlBatch), vp, ll, ll, ll, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp,
                                    C.c_int]
     _lib = lib
     return lib
@@ -56,10 +57,11 @@ def dirty_map_words(n_slots: int) -> int:
 
 
 def fresh_pileup(batch, counts: np.ndarray, dirty_map, zero_rest: bool, split: int = 1, cx: bool = None,
-                 grid: int = 3):
+                 grid: int = 3, slot_range=None):
     """What kdl_pileup_range_map does with KDL_PILEUP_FRESH_WEIGHTS (| KDL_PILEUP_ZERO_REST when zero_rest) over the
-    whole slot range: `counts` (int32 [19, n_slots]) is a reused table -- weight columns stale, columns 5..18 as the
-    previous pileup left them -- and `dirty_map` (uint32 [dirty_map_words], or None = zero all of columns 5..18) its
+    slot range `slot_range` = (lo, hi) (multiples of 4, of 512 for the tile kernel; default: the whole table):
+    `counts` (int32 [19, n_slots]) is a reused table -- weight columns stale, columns 5..18 as the previous pileup
+    left them -- and `dirty_map` (uint32 [dirty_map_words], or None = zero all of columns 5..18) its
     map; both are updated in place.  split > 1: the depth split.  cx: which K1 instantiation (default: the piece one
     when the batch has tile-eligible complex reads).  Returns the event rows; raises if a read raised."""
     from kindel_b200 import engine
@@ -74,7 +76,8 @@ def fresh_pileup(batch, counts: np.ndarray, dirty_map, zero_rest: bool, split: i
     index = np.zeros(8 * (n_slots // 512) + 8, dtype=np.uint32)
     events = np.full((max(int(batch.n_events), 1), 4), -1, dtype=np.int32)
     flag = np.zeros(4, dtype=np.int32)
-    rc = lib.emu_map_pileup(C.byref(st), counts.ctypes.data, n_slots, index.ctypes.data,
+    lo, hi = (0, n_slots) if slot_range is None else (int(slot_range[0]), int(slot_range[1]))
+    rc = lib.emu_map_pileup(C.byref(st), counts.ctypes.data, n_slots, lo, hi, index.ctypes.data,
                             None if dirty_map is None else dirty_map.ctypes.data, 1 if zero_rest else 0, split,
                             1 if cx else 0, events.ctypes.data, flag.ctypes.data, grid)
     del keep

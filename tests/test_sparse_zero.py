@@ -7,10 +7,15 @@ sectors; both 4 % complex, so their writers mark), a simple batch, A again, a co
 reads; dense: the range is left marked), and for the order-independent kernels an unsorted batch -- and after every
 pileup the table and the events equal the C oracle's and every non-zero (column 5..18, sector) has its bit set.  A map
 with every bit set gives the same results.  The emulator half runs the kernel sources on the CPU (tests/emu/); the
-`gpu` half runs the same through engine.pileup (masked reads, slot-range shards) and the host-buffer context."""
+`gpu` half runs the same through engine.pileup (masked reads, slot-range shards) and the host-buffer context.
+
+The emulator also runs the sharded step's table sequence: every rank's two parity tables, each bounded by the rank's
+footprint, piled into epoch after epoch with the fused exchange in between (tests/test_gpu_sharded_epochs.py runs
+distributed.ShardedConsensus itself the same way on one GPU)."""
 import numpy as np
 import pytest
 
+import emu_harness
 import emu_map_harness as E
 from kindel_b200 import distributed as D
 from kindel_b200 import synth
@@ -217,3 +222,75 @@ def test_host_context_alternating_batches():
             np.testing.assert_array_equal(calls, coracle.vote(want, 1), err_msg=what)
     finally:
         ctx.close()
+
+
+# ------------------------------------------------------------------------------- sharded epochs, emulated
+class _EmuRankTable:
+    """One parity table of a rank as distributed.ShardedConsensus holds it, on the host: adopted from a zero-filled
+    block (CountTable(tensor=...): every map bit set, nothing dirty yet), with engine.pileup's bookkeeping around
+    each pileup -- the range is the footprint joined with what earlier pileups dirtied, tile-aligned, and columns
+    5..18 are zeroed (where the map says) once a complex batch has been piled into the table."""
+
+    def __init__(self, n_slots):
+        self.t = np.zeros((19, n_slots), dtype=np.int32)
+        self.map = np.full(E.dirty_map_words(n_slots), 0xFFFFFFFF, dtype=np.uint32)
+        self.dirty, self.dirty_rest = None, False
+
+    def pileup(self, batch, slot_range):
+        n_slots = self.t.shape[1]
+        lo, hi = slot_range
+        if self.dirty is not None:
+            lo, hi = min(lo, self.dirty[0]), max(hi, self.dirty[1])
+        lo, hi = max(0, lo // 512 * 512), min(n_slots, (hi + 511) // 512 * 512)
+        cx = (batch.n_complex - batch.n_hard) * 16 >= batch.n_reads  # kdl_pileup_range_map's choice
+        ev = E.fresh_pileup(batch, self.t, self.map, self.dirty_rest, cx=cx, slot_range=(lo, hi))
+        self.dirty, self.dirty_rest = (lo, hi), batch.n_complex > 0
+        return ev
+
+
+def _sharded_case(kind):
+    if kind == "contigs":  # 3 ranks over 2 contigs: the middle rank gets no reads and a zero-width slice
+        return synth.mixed_reads(16, [3000, 2500], 30, 0.04), "contigs"
+    if kind == "dense":    # 1 in 16 and more complex, hard reads of the edge tail: ranges are left marked
+        return synth.complex_reads(17, L, 30), "reads"
+    return synth.mixed_reads(18, [L], 30, 0.04), "reads"  # sparse: the kernels mark sector by sector
+
+
+@emu
+@pytest.mark.parametrize("world,kind", [(2, "sparse"), (3, "sparse"), (2, "dense"), (3, "contigs")])
+def test_sharded_epochs_emulated(world, kind):
+    """The fused sharded step of every rank on the emulated kernels: each rank keeps its shard and its two parity
+    tables, piles into the epoch's table over its footprint with a live map (every table reused), then K2x + K2g run
+    over that epoch's tables.  After every epoch each rank's calls equal the oracle's vote of the whole batch, each
+    table equals its shard's oracle table (zero outside the footprint) with its map covering it, the tables add up to
+    the whole batch's and the shards' events merge into its events."""
+    full, plan = _sharded_case(kind)
+    n_slots = full.n_slots
+    want, want_ev = coracle.pileup(full)
+    want_calls = coracle.vote(want, 2)
+    idx = [D.shard_indices(full, r, world, plan) for r in range(world)]
+    shards = [D.select_reads(full, i) for i in idx]
+    shard_want = [coracle.pileup(s)[0] for s in shards]
+    feet = [D.footprint(s) for s in shards]
+    slices = D.footprint_slices(feet, n_slots)
+    if kind == "contigs":
+        assert [s.n_reads == 0 for s in shards] == [False, True, False] and slices[1][0] == slices[1][1]
+    tables = [[_EmuRankTable(n_slots) for _ in range(2)] for _ in range(world)]
+    calls = [[np.full(n_slots, 0xEE, dtype=np.uint8) for _ in range(world)] for _ in range(2)]
+    flags = {k: [np.zeros(16, dtype=np.int32) for _ in range(world)] for k in ("ready", "done")}
+    flags["counter"] = [np.zeros(1, dtype=np.int32) for _ in range(world)]
+    for epoch in range(1, 5):
+        par = epoch & 1
+        evs = [tables[r][par].pileup(shards[r], feet[r]) for r in range(world)]
+        emu_harness.exchange_epoch([tables[r][par].t for r in range(world)], feet, slices, calls[par], flags, epoch, min_depth=2)
+        for r in range(world):
+            what = "%s world %d epoch %d rank %d" % (kind, world, epoch, r)
+            np.testing.assert_array_equal(calls[par][r], want_calls, err_msg=what)
+            tab = tables[r][par]
+            np.testing.assert_array_equal(tab.t, shard_want[r], err_msg=what)
+            lo, hi = feet[r]
+            assert not tab.t[:, :lo].any() and not tab.t[:, hi:].any(), what
+            for k in range(2):
+                assert_map_covers(tables[r][k].t, tables[r][k].map, what + " parity %d" % k)
+        np.testing.assert_array_equal(sum(tables[r][par].t.astype(np.int64) for r in range(world)), want)
+        np.testing.assert_array_equal(D.merge_events(evs, idx), want_ev)
