@@ -291,6 +291,37 @@ int kdl_variant_scatter(const int32_t* counts, int64_t n_slots, const int64_t* c
                         int32_t n_contigs, int64_t abs_floor, double rel_threshold, const uint32_t* block_sums,
                         int64_t n_sites, int64_t* site_slot, int32_t* site_counts, uint8_t* site_mask, void* stream);
 
+/* K6r -- the candidate sites of `variants --vcf --reference` (extension): K6's passes against reference bases.
+ * ref[n_slots]: one code per slot, 0-3 = A, C, G, T, 4 = anything else (and every slot that is not a position),
+ * 4-byte aligned.  Per slot s of contig c, p = s - contig_slot[c], g = ref[s], t = columns 0-6 of counts and
+ * depth(s) = t[0] + ... + t[5]:
+ *   bit k (k = 0..3, SNV allele A, C, G, T), only at 0 <= p < L: k != g, t[k] > abs_floor and
+ *     (double)t[k] / (double)depth(s) > rel_threshold (0 at depth 0);
+ *   bit 6 (insertion candidate), at 0 <= p <= L: t[6] > abs_floor and t[6] / DPa > rel_threshold, DPa = depth(s - 1)
+ *     for p >= 1 and depth(s) for p = 0 (0 at DPa 0).
+ * abs_floor / rel_threshold as for K6.  Counting, scratch (kdl_variant_scratch_words) and the site total as for
+ * kdl_variant_count.  kdl_variant_ref_scatter writes, in ascending slot order, site_slot[i], site_counts[k * n_sites
+ * + i] (k = 0..6), site_dpa[i] (DPa) and site_mask[i].  All pointers are device pointers. */
+int kdl_variant_ref_count(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                          int32_t n_contigs, const uint8_t* ref, int64_t abs_floor, double rel_threshold,
+                          uint32_t* block_sums, void* stream);
+int kdl_variant_ref_scatter(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot,
+                            const int32_t* contig_len, int32_t n_contigs, const uint8_t* ref, int64_t abs_floor,
+                            double rel_threshold, const uint32_t* block_sums, int64_t n_sites, int64_t* site_slot,
+                            int32_t* site_counts, int64_t* site_dpa, uint8_t* site_mask, void* stream);
+
+/* K7 -- the deletion events of a batch (extension, for `variants --vcf --reference`).  Every read's CIGAR is walked
+ * with the reference's cursor (kindel.py:40-81: M/=/X and D advance; an S that is op #0 does not; any later S advances
+ * while the cursor is below the contig length L; I, N, H, P do not); simple reads have no D op.  A D of length n >= 1
+ * at cursor r is an event when 0 <= r and r + n <= L: (contig_slot + r, n).  kdl_deletion_count runs the per-CTA
+ * counts and their scan; the number of events is then block_sums[words - 1], with block_sums device scratch of
+ * words = kdl_deletion_scratch_words(n_reads) uint32.  kdl_deletion_scatter, on the same stream after it with
+ * n_events = that number, writes ev_slot[i] and ev_len[i] in read order, then op order.  Device pointers. */
+int64_t kdl_deletion_scratch_words(int64_t n_reads);
+int kdl_deletion_count(const kdl_batch* batch, uint32_t* block_sums, void* stream);
+int kdl_deletion_scatter(const kdl_batch* batch, const uint32_t* block_sums, int64_t n_events, int64_t* ev_slot,
+                         int32_t* ev_len, void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced

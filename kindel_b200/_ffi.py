@@ -122,7 +122,16 @@ _PROTOTYPES = {
                                     C.c_void_p, C.c_void_p]),
     "kdl_variant_scatter": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_double,
                                       C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "kdl_vote_peers": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+    "kdl_variant_ref_count": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                        C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
+    "kdl_variant_ref_scatter": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                          C.c_int64, C.c_double, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_deletion_scratch_words": (C.c_int64, [C.c_int64]),
+    "kdl_deletion_count": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p]),
+    "kdl_deletion_scatter": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
+    "kdl_vote_peers":(C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,
                                         C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),

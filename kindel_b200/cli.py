@@ -5,7 +5,7 @@ REPORT blocks to stderr and one `>name` / sequence pair per contig to stdout (cl
 extension one FASTQ record per contig instead),
 `weights` / `features` write TSV to stdout (cli.py:44,50), `version` prints `kindel <version>`;
 `variants` (in the reference's README only) is an extension, see kindel.variants; its `--vcf` writes a sites-only VCF
-(kindel.variants_vcf).
+(kindel.variants_vcf), against a FASTA with `--reference`.
 argh derived the flags from the function signatures (first letter as short option unless two
 parameters share it); argparse spells the same set out.  Note the CLI default `--min-overlap 7`
 (cli.py:13) differs from the API default 9 (kindel.py:492), as in the reference.
@@ -51,12 +51,13 @@ def features(bam_path, gpus=None, **filters):
 
 
 def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False, absolute=False, gpus=None, vcf=False,
-             **filters):
+             reference=None, **filters):
     """Output variants exceeding specified absolute and relative frequency thresholds"""
     from . import kindel
 
-    if vcf:  # extension: the sites of --only-variants as a sites-only VCF
-        sys.stdout.write(kindel.variants_vcf(bam_path, abs_threshold, rel_threshold, devices=gpus, **filters))
+    if vcf:  # extension: the sites of --only-variants as a sites-only VCF (against --reference when given)
+        extra = {} if reference is None else dict(reference=reference)
+        sys.stdout.write(kindel.variants_vcf(bam_path, abs_threshold, rel_threshold, devices=gpus, **filters, **extra))
         return
     kindel.variants(bam_path, abs_threshold, rel_threshold, only_variants, absolute, devices=gpus, **filters).to_csv(
         sys.stdout, sep="\t", index=False)
@@ -164,8 +165,12 @@ def build_parser() -> argparse.ArgumentParser:
     # extension: the variant sites as VCF (REF = the sample's most frequent allele; see kindel.variants_vcf)
     p.add_argument("--vcf", action="store_true",
                    help="write the variant sites as a sites-only VCF 4.2 instead of the table")
+    # extension: REF from the FASTA the alignment was made against; SNVs, insertions and deletions against it (no
+    # short option: -r is --rel-threshold)
+    p.add_argument("--reference", default=None, metavar="FASTA",
+                   help="with --vcf: call SNVs, insertions and deletions against this FASTA (plain or gzip)")
     p.set_defaults(func=lambda a: variants(a.bam_path, a.abs_threshold, a.rel_threshold, a.only_variants, a.absolute,
-                                           a.gpus, a.vcf, **_filters(a)))
+                                           a.gpus, a.vcf, a.reference, **_filters(a)))
 
     p = sub.add_parser("plot", help=plot.__doc__, description=plot.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")
@@ -182,6 +187,8 @@ def _check_variants_args(parser, args):
         for flag, on in (("--absolute", args.absolute), ("--only-variants", args.only_variants)):
             if on:
                 parser.error("variants: --vcf cannot be combined with %s (a table option)" % flag)
+    elif getattr(args, "reference", None) is not None:
+        parser.error("variants: --reference needs --vcf (the table has no reference mode)")
 
 
 def main(argv=None):

@@ -461,6 +461,80 @@ int kdl_variant_scatter(const int32_t* counts, int64_t n_slots, const int64_t* c
     return check_launch();
 }
 
+static int variant_ref_args(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot,
+                            const int32_t* contig_len, int32_t n_contigs, const uint8_t* ref, int64_t abs_floor,
+                            double rel_threshold, kdl::RefVariantArgs* a) {
+    kdl::VariantArgs v;
+    int rc = variant_args(counts, n_slots, contig_slot, contig_len, n_contigs, abs_floor, rel_threshold, &v);
+    if (rc != KDL_OK) return rc;
+    if (!ref || (reinterpret_cast<uintptr_t>(ref) & 3)) return KDL_ERR_INVALID_ARG;
+    *a = kdl::RefVariantArgs{};
+    a->counts = counts; a->n_slots = n_slots; a->layout = v.layout; a->ref = ref;
+    a->abs_floor = abs_floor; a->rel_threshold = rel_threshold;
+    return KDL_OK;
+}
+
+int kdl_variant_ref_count(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                          int32_t n_contigs, const uint8_t* ref, int64_t abs_floor, double rel_threshold,
+                          uint32_t* block_sums, void* stream) {
+    kdl::RefVariantArgs a;
+    int rc = variant_ref_args(counts, n_slots, contig_slot, contig_len, n_contigs, ref, abs_floor, rel_threshold, &a);
+    if (rc != KDL_OK) return rc;
+    if (!block_sums) return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
+    cudaStream_t st = (cudaStream_t)stream;
+    kdl::variant_ref_sums_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, st>>>(a, block_sums);
+    if ((rc = check_launch()) != KDL_OK) return rc;
+    kdl::assemble_scan_sums_kernel<<<1, kdl::A_THREADS, 0, st>>>(block_sums, n_blocks);
+    return check_launch();
+}
+
+int kdl_variant_ref_scatter(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot,
+                            const int32_t* contig_len, int32_t n_contigs, const uint8_t* ref, int64_t abs_floor,
+                            double rel_threshold, const uint32_t* block_sums, int64_t n_sites, int64_t* site_slot,
+                            int32_t* site_counts, int64_t* site_dpa, uint8_t* site_mask, void* stream) {
+    kdl::RefVariantArgs a;
+    int rc = variant_ref_args(counts, n_slots, contig_slot, contig_len, n_contigs, ref, abs_floor, rel_threshold, &a);
+    if (rc != KDL_OK) return rc;
+    if (!block_sums || n_sites < 0 || n_sites > n_slots ||
+        (n_sites > 0 && (!site_slot || !site_counts || !site_dpa || !site_mask)))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
+    kdl::variant_ref_scatter_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
+        a, block_sums, n_sites, site_slot, site_counts, site_dpa, site_mask);
+    return check_launch();
+}
+
+int64_t kdl_deletion_scratch_words(int64_t n_reads) {
+    return n_reads < 0 ? 0 : (n_reads + kdl::A_THREADS - 1) / kdl::A_THREADS + 1;
+}
+
+int kdl_deletion_count(const kdl_batch* batch, uint32_t* block_sums, void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (!block_sums || batch->n_reads > (int64_t)UINT32_MAX) return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (batch->n_reads + kdl::A_THREADS - 1) / kdl::A_THREADS;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_blocks > 0) {
+        kdl::deletion_sums_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, st>>>(*batch, block_sums);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+    }
+    kdl::assemble_scan_sums_kernel<<<1, kdl::A_THREADS, 0, st>>>(block_sums, n_blocks);
+    return check_launch();
+}
+
+int kdl_deletion_scatter(const kdl_batch* batch, const uint32_t* block_sums, int64_t n_events, int64_t* ev_slot,
+                         int32_t* ev_len, void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (!block_sums || n_events < 0 || (n_events > 0 && (!ev_slot || !ev_len))) return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (batch->n_reads + kdl::A_THREADS - 1) / kdl::A_THREADS;
+    if (n_blocks == 0) return KDL_OK;
+    kdl::deletion_scatter_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
+        *batch, block_sums, n_events, ev_slot, ev_len);
+    return check_launch();
+}
+
 int kdl_table_alloc(int64_t bytes, void** dev_ptr) {
     if (!dev_ptr || bytes <= 0) return KDL_ERR_INVALID_ARG;
     *dev_ptr = nullptr;

@@ -12,6 +12,12 @@
 // scatter that re-evaluates the rule and writes the records in ascending slot order: the order is the slot order, no
 // atomic decides it.  The extra slot behind a contig and the padding are never sites (K5's `is_position`).
 // n_slots % 4 == 0: one thread = 4 slots, six 128-bit loads; 24 B per slot are read by each of the two passes.
+//
+// The two passes are templates over a site policy (`variant_sums` / `variant_scatter`), the way the IUPAC vote is a
+// policy of K2: VariantArgs is K6's, RefVariantArgs (K6r, below) compares against reference bases.
+//
+// K7 `deletion_*_kernel` (extension, at the end): the deletion events (slot, length) of the complex reads' CIGARs,
+// in read order and then op order, with the same count / scan / scatter shape over reads instead of slots.
 
 namespace kdl {
 
@@ -21,6 +27,14 @@ struct VariantArgs {
     AssembleArgs layout;    // contig_slot / contig_len / n_contigs, for is_position
     long long abs_floor;
     double rel_threshold;
+
+    // the site policy of the two passes
+    struct Quad { int t[4][6]; };                                  // what one thread keeps of its 4 slots
+    struct Out { int64_t* slot; int32_t* counts; uint8_t* mask; };  // the records
+    __device__ __forceinline__ void load(long long, Quad&) const {}  // (every thread; nothing to share)
+    __device__ __forceinline__ void eval(long long s, Quad& q, unsigned (&bits)[4]) const;
+    __device__ __forceinline__ void write(const Out& out, const Quad& q, int j, long long o, long long n_sites,
+                                          long long slot, unsigned bits) const;
 };
 
 // bit k set: allele k is a variant at this slot (not yet restricted to positions)
@@ -60,14 +74,30 @@ __device__ __forceinline__ void variant_quad(const VariantArgs& a, long long s, 
     }
 }
 
-__global__ void __launch_bounds__(A_THREADS)
-variant_sums_kernel(VariantArgs a, uint32_t* __restrict__ block_sums) {
+__device__ __forceinline__ void VariantArgs::eval(long long s, Quad& q, unsigned (&bits)[4]) const {
+    variant_quad(*this, s, q.t, bits);
+}
+
+__device__ __forceinline__ void VariantArgs::write(const Out& out, const Quad& q, int j, long long o, long long n_sites,
+                                                   long long slot, unsigned bits) const {
+    out.slot[o] = slot;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) out.counts[(long long)k * n_sites + o] = q.t[j][k];
+    out.mask[o] = (uint8_t)bits;
+}
+
+// ---- the two passes, over any site policy P ------------------------------------------------------------------
+// P::load runs on every thread of the CTA (s may lie past the table: it may hold warp collectives); P::eval only for
+// s < n_slots, and sets bits[j] != 0 for each of the 4 slots that is a site; P::write stores site j as record o.
+template <class P>
+__device__ __forceinline__ void variant_sums(const P& a, uint32_t* __restrict__ block_sums) {
     const long long s = (long long)blockIdx.x * A_BLOCK + (long long)A_PER * threadIdx.x;
     uint32_t n = 0;
+    typename P::Quad q;
+    a.load(s, q);
     if (s < a.n_slots) {
-        int t[4][6];
         unsigned bits[4];
-        variant_quad(a, s, t, bits);
+        a.eval(s, q, bits);
         n = (bits[0] != 0) + (bits[1] != 0) + (bits[2] != 0) + (bits[3] != 0);
     }
     uint32_t total;
@@ -75,18 +105,16 @@ variant_sums_kernel(VariantArgs a, uint32_t* __restrict__ block_sums) {
     if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
 }
 
-// block_sums: the exclusive prefix assemble_scan_sums_kernel left.  Records: site_slot[i], site_counts[k * n_sites + i]
-// (k = 0..5, column-major like the table), site_mask[i] (bits 0-5 = the variant alleles).
-__global__ void __launch_bounds__(A_THREADS)
-variant_scatter_kernel(VariantArgs a, const uint32_t* __restrict__ block_sums, long long n_sites,
-                       int64_t* __restrict__ site_slot, int32_t* __restrict__ site_counts,
-                       uint8_t* __restrict__ site_mask) {
+template <class P>
+__device__ __forceinline__ void variant_scatter(const P& a, const uint32_t* __restrict__ block_sums, long long n_sites,
+                                                const typename P::Out& out) {
     const long long s = (long long)blockIdx.x * A_BLOCK + (long long)A_PER * threadIdx.x;
-    int t[4][6];
+    typename P::Quad q;
     unsigned bits[4] = {0u, 0u, 0u, 0u};
     uint32_t n = 0;
+    a.load(s, q);
     if (s < a.n_slots) {
-        variant_quad(a, s, t, bits);
+        a.eval(s, q, bits);
         n = (bits[0] != 0) + (bits[1] != 0) + (bits[2] != 0) + (bits[3] != 0);
     }
     uint32_t total;
@@ -95,14 +123,207 @@ variant_scatter_kernel(VariantArgs a, const uint32_t* __restrict__ block_sums, l
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         if (!bits[j]) continue;
-        if (o < n_sites) {  // (n_sites is the count the first pass found; the guard only keeps a wrong one in bounds)
-            site_slot[o] = s + j;
-#pragma unroll
-            for (int k = 0; k < 6; ++k) site_counts[(long long)k * n_sites + o] = t[j][k];
-            site_mask[o] = (uint8_t)bits[j];
-        }
+        // (n_sites is the count the first pass found; the guard only keeps a wrong one in bounds)
+        if (o < n_sites) a.write(out, q, j, o, n_sites, s + j, bits[j]);
         ++o;
     }
+}
+
+__global__ void __launch_bounds__(A_THREADS)
+variant_sums_kernel(VariantArgs a, uint32_t* __restrict__ block_sums) {
+    variant_sums(a, block_sums);
+}
+
+// block_sums: the exclusive prefix assemble_scan_sums_kernel left.  Records: site_slot[i], site_counts[k * n_sites + i]
+// (k = 0..5, column-major like the table), site_mask[i] (bits 0-5 = the variant alleles).
+__global__ void __launch_bounds__(A_THREADS)
+variant_scatter_kernel(VariantArgs a, const uint32_t* __restrict__ block_sums, long long n_sites,
+                       int64_t* __restrict__ site_slot, int32_t* __restrict__ site_counts,
+                       uint8_t* __restrict__ site_mask) {
+    variant_scatter(a, block_sums, n_sites, VariantArgs::Out{site_slot, site_counts, site_mask});
+}
+
+// ---- K6r: sites against reference bases (`variants --vcf --reference`) ---------------------------------------
+// Per slot s of contig c: p = s - contig_slot[c], g = ref[s] (0-3 = A, C, G, T; 4 = anything else, and every slot
+// that is not a position), t = columns 0-6, depth(s) = t0 + ... + t5.
+//   SNV bit k (k = 0..3), only at 0 <= p < L: k != g, t_k > abs_floor, t_k / depth(s) > rel (0 at depth 0).
+//   insertion-candidate bit 6, at 0 <= p <= L (slot L holds the insertions behind the last base): t6 > abs_floor and
+//   t6 / DPa > rel, DPa = depth(s - 1) for p >= 1 and depth(s) for p = 0.  Every inserted string's count is <= t6,
+//   so the bit is necessary for any string to pass; the host tests the strings.
+// depth(s - 1) of a thread's first slot comes from the lane that owns it (a shuffle); lane 0 loads it.  28 B of
+// counts and 1 B of reference per slot are read by each pass.
+struct RefVariantArgs {
+    const int32_t* counts;  // [19][n_slots]; columns 0-6 are read
+    long long n_slots;
+    AssembleArgs layout;    // contig_slot / contig_len / n_contigs
+    const uint8_t* ref;     // [n_slots] codes, 4-byte aligned
+    long long abs_floor;
+    double rel_threshold;
+
+    struct Quad {
+        int t[4][7];
+        long long depth[4];
+        long long prev;      // depth(s - 1) (0 at s = 0)
+        long long dpa[4];    // DPa of each slot (set by eval where a bit is set)
+        uint32_t g;          // the 4 reference codes, slot s in the low byte
+    };
+    struct Out { int64_t* slot; int32_t* counts; int64_t* dpa; uint8_t* mask; };
+    __device__ __forceinline__ void load(long long s, Quad& q) const;
+    __device__ __forceinline__ void eval(long long s, Quad& q, unsigned (&bits)[4]) const;
+    __device__ __forceinline__ void write(const Out& out, const Quad& q, int j, long long o, long long n_sites,
+                                          long long slot, unsigned bits) const;
+};
+
+__device__ __forceinline__ void RefVariantArgs::load(long long s, Quad& q) const {
+    long long last = 0;
+    if (s < n_slots) {
+#pragma unroll
+        for (int k = 0; k < 7; ++k) {
+            const int4 v = __ldg(reinterpret_cast<const int4*>(counts + (long long)k * n_slots + s));
+            q.t[0][k] = v.x; q.t[1][k] = v.y; q.t[2][k] = v.z; q.t[3][k] = v.w;
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            long long d = 0;
+#pragma unroll
+            for (int k = 0; k < 6; ++k) d += q.t[j][k];
+            q.depth[j] = d;
+        }
+        q.g = __ldg(reinterpret_cast<const uint32_t*>(ref + s));
+        last = q.depth[3];
+    }
+    long long prev = __shfl_up_sync(0xffffffffu, last, 1);  // every lane: the whole warp takes part
+    if ((threadIdx.x & 31) == 0) {                              // slot s - 1 belongs to the warp before
+        prev = 0;
+        if (s > 0 && s < n_slots) {
+#pragma unroll
+            for (int k = 0; k < 6; ++k) prev += __ldg(counts + (long long)k * n_slots + s - 1);
+        }
+    }
+    q.prev = prev;
+}
+
+__device__ __forceinline__ unsigned ref_site_bits(const RefVariantArgs& a, long long s, const int (&t)[7], unsigned g,
+                                                  long long depth, long long prev, long long* dpa) {
+    unsigned bits = 0;
+    const double d = (double)depth;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        if ((unsigned)k != g && (long long)t[k] > a.abs_floor) {
+            const double share = depth > 0 ? (double)t[k] / d : 0.0;
+            if (share > a.rel_threshold) bits |= 1u << k;
+        }
+    }
+    const bool ins = (long long)t[6] > a.abs_floor;
+    if (!bits && !ins) return 0u;
+    int lo = 0, hi = a.layout.n_contigs;  // the last contig with contig_slot <= s
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (a.layout.contig_slot[mid] <= s) lo = mid + 1; else hi = mid;
+    }
+    if (lo == 0) return 0u;
+    const long long p = s - a.layout.contig_slot[lo - 1], L = a.layout.contig_len[lo - 1];
+    if (p >= L) bits = 0u;  // SNVs at positions only
+    const long long da = p == 0 ? depth : prev;
+    if (ins && p <= L) {
+        const double share = da > 0 ? (double)t[6] / (double)da : 0.0;
+        if (share > a.rel_threshold) bits |= 1u << 6;
+    }
+    *dpa = da;
+    return bits;
+}
+
+__device__ __forceinline__ void RefVariantArgs::eval(long long s, Quad& q, unsigned (&bits)[4]) const {
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+        bits[j] = ref_site_bits(*this, s + j, q.t[j], (q.g >> (8 * j)) & 0xFFu, q.depth[j],
+                                j == 0 ? q.prev : q.depth[j - 1], &q.dpa[j]);
+}
+
+__device__ __forceinline__ void RefVariantArgs::write(const Out& out, const Quad& q, int j, long long o,
+                                                      long long n_sites, long long slot, unsigned bits) const {
+    out.slot[o] = slot;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) out.counts[(long long)k * n_sites + o] = q.t[j][k];
+    out.dpa[o] = q.dpa[j];
+    out.mask[o] = (uint8_t)bits;
+}
+
+__global__ void __launch_bounds__(A_THREADS)
+variant_ref_sums_kernel(RefVariantArgs a, uint32_t* __restrict__ block_sums) {
+    variant_sums(a, block_sums);
+}
+
+// Records: site_slot[i], site_counts[k * n_sites + i] (k = 0..6), site_dpa[i], site_mask[i] (bits 0-3 SNV alleles
+// A, C, G, T; bit 6 the insertion candidate).
+__global__ void __launch_bounds__(A_THREADS)
+variant_ref_scatter_kernel(RefVariantArgs a, const uint32_t* __restrict__ block_sums, long long n_sites,
+                           int64_t* __restrict__ site_slot, int32_t* __restrict__ site_counts,
+                           int64_t* __restrict__ site_dpa, uint8_t* __restrict__ site_mask) {
+    variant_scatter(a, block_sums, n_sites, RefVariantArgs::Out{site_slot, site_counts, site_dpa, site_mask});
+}
+
+// ---- K7: deletion events -------------------------------------------------------------------------------------
+// One thread per read.  Simple reads (l_seq bit 31 clear) have no D op.  A complex read's CIGAR block sits behind its
+// bases in seq4: [n_ops][evt_off][ops...].  The reference cursor moves as in kindel.py:40-81 (K1g restates it): M / = /
+// X and D advance it; an S that is op #0 does not; any other S advances it while r_pos < L; I, N, H, P do not.  Each D
+// of length n >= 1 at cursor r with 0 <= r and r + n <= L is the event (contig_slot + r, n); one that wraps (POS 0)
+// or runs past the contig end is still in the table's deletion column but is no event.
+template <class Emit>
+__device__ __forceinline__ void walk_deletions(const kdl_batch& b, long long r, Emit&& emit) {
+    const uint32_t lraw = (uint32_t)b.l_seq[r];
+    if (!(lraw & KDL_COMPLEX)) return;
+    const int c = find_contig(b.contig_read_off, b.n_contigs, r);
+    const long long L = b.contig_len[c];
+    const long long base = b.contig_slot[c];
+    const uint32_t* __restrict__ blk = b.seq4 + (size_t)b.seq_off[r] + ((complex_len(lraw) + 7) >> 3);
+    const uint32_t n_ops = blk[0];
+    const uint32_t* __restrict__ ops = blk + 2;
+    long long r_pos = b.ref_start[r];
+    for (uint32_t i = 0; i < n_ops; ++i) {
+        const uint32_t cg = ops[i];
+        const long long len = cg >> 4;
+        const int op = cg & 0xF;
+        if (op == 0 || op == 7 || op == 8) {  // M = X
+            r_pos += len;
+        } else if (op == 2) {                 // D
+            if (len > 0 && r_pos >= 0 && r_pos + len <= L) emit(base + r_pos, len);
+            r_pos += len;
+        } else if (op == 4 && i != 0) {       // right clip: advances while r_pos < L
+            long long n_adv = L - r_pos;
+            n_adv = n_adv < 0 ? 0 : (n_adv > len ? len : n_adv);
+            r_pos += n_adv;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(A_THREADS)
+deletion_sums_kernel(kdl_batch b, uint32_t* __restrict__ block_sums) {
+    const long long r = (long long)blockIdx.x * A_THREADS + threadIdx.x;
+    uint32_t n = 0;
+    if (r < b.n_reads) walk_deletions(b, r, [&](long long, long long) { ++n; });
+    uint32_t total;
+    cta_exclusive_scan(n, &total);
+    if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
+}
+
+// block_sums: the exclusive prefix of the per-CTA counts.  Events: ev_slot[i], ev_len[i], in read order, then op order.
+__global__ void __launch_bounds__(A_THREADS)
+deletion_scatter_kernel(kdl_batch b, const uint32_t* __restrict__ block_sums, long long n_events,
+                        int64_t* __restrict__ ev_slot, int32_t* __restrict__ ev_len) {
+    const long long r = (long long)blockIdx.x * A_THREADS + threadIdx.x;
+    uint32_t n = 0;
+    if (r < b.n_reads) walk_deletions(b, r, [&](long long, long long) { ++n; });
+    uint32_t total;
+    long long o = (long long)block_sums[blockIdx.x] + cta_exclusive_scan(n, &total);
+    if (!n) return;
+    walk_deletions(b, r, [&](long long slot, long long len) {
+        if (o < n_events) {  // (as in K6: the guard only keeps a wrong count in bounds)
+            ev_slot[o] = slot;
+            ev_len[o] = (int32_t)len;
+        }
+        ++o;
+    });
 }
 
 }  // namespace kdl

@@ -12,6 +12,8 @@ implementation behind these functions: without a CUDA device they raise.
     consensus_qual(counts, calls)  K2q: Phred quality of the base each slot emits (extension)
     assemble(calls, ...)       K5 (+ K5q): consensus text (and its quality text) of every contig
     variant_sites(counts, ...) K6: the variant sites of `variants --only-variants` and the VCF (extension)
+    variant_sites_ref(...)     K6r: the SNV and insertion-candidate sites against a reference (extension)
+    deletion_alleles(dbatch, counts, ...)  K7 + grouping: the deletion alleles against a reference (extension)
 """
 from __future__ import annotations
 
@@ -412,6 +414,92 @@ def variant_sites(counts: torch.Tensor, contig_slot, contig_len, abs_threshold, 
         if n == 0:
             return np.zeros(0, dtype=np.int64), np.zeros((6, 0), dtype=np.int32), np.zeros(0, dtype=np.uint8)
         return site_slot.cpu().numpy(), site_counts[:, :n].cpu().numpy(), site_mask.cpu().numpy()
+
+
+def _device_layout(contig_slot, contig_len, dev):
+    n_contigs = len(contig_len)
+    t_slot = torch.from_numpy(np.ascontiguousarray(contig_slot, dtype=np.int64) if n_contigs
+                              else np.zeros(1, dtype=np.int64)).to(dev)
+    t_len = torch.from_numpy(np.ascontiguousarray(contig_len, dtype=np.int32) if n_contigs
+                             else np.zeros(1, dtype=np.int32)).to(dev)
+    return t_slot, t_len, n_contigs
+
+
+def variant_sites_ref(counts: torch.Tensor, contig_slot, contig_len, ref, abs_threshold, rel_threshold):
+    """K6r (extension): the candidate sites of `variants --vcf --reference` in a device table (int32[>= 7, n_slots],
+    contiguous, n_slots % 4 == 0) against reference codes `ref` (uint8[n_slots], 0-3 = A, C, G, T, 4 = other; a device
+    tensor or a host array, uploaded).  Returns (slot int64[n], counts int32[7, n], dpa int64[n], mask uint8[n]) on the
+    host in ascending slot order: bits 0-3 of mask are the SNV alleles A, C, G, T, bit 6 the insertion candidate, dpa
+    the depth the slot's insertions are measured against (include/kindel_b200.h has the rule)."""
+    lib = _ffi.load()
+    dev = counts.device
+    n_slots = int(counts.shape[1])
+    a, r = variant_abs_floor(abs_threshold), float(rel_threshold)
+    with torch.cuda.device(dev):
+        if not isinstance(ref, torch.Tensor):
+            ref = torch.from_numpy(np.ascontiguousarray(ref, dtype=np.uint8))
+        ref = ref.to(dev).contiguous()
+        if ref.dtype != torch.uint8 or ref.numel() != n_slots:
+            raise ValueError("reference codes must be uint8[%d], got %s[%d]" % (n_slots, ref.dtype, ref.numel()))
+        t_slot, t_len, n_contigs = _device_layout(contig_slot, contig_len, dev)
+        sums = torch.empty(int(lib.kdl_variant_scratch_words(n_slots)), dtype=torch.int32, device=dev)
+        args = (counts.data_ptr(), n_slots, t_slot.data_ptr(), t_len.data_ptr(), n_contigs, ref.data_ptr(), a, r,
+                sums.data_ptr())
+        _ffi.check(lib.kdl_variant_ref_count(*args, _stream_ptr(dev)), "kdl_variant_ref_count")
+        n = int(sums[-1].item()) & 0xFFFFFFFF
+        site_slot = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+        site_counts = torch.empty((7, max(n, 1)), dtype=torch.int32, device=dev)
+        site_dpa = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+        site_mask = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        rc = lib.kdl_variant_ref_scatter(*args, n, site_slot.data_ptr(), site_counts.data_ptr(), site_dpa.data_ptr(),
+                                         site_mask.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_variant_ref_scatter")
+        if n == 0:
+            return (np.zeros(0, dtype=np.int64), np.zeros((7, 0), dtype=np.int32), np.zeros(0, dtype=np.int64),
+                    np.zeros(0, dtype=np.uint8))
+        return (site_slot.cpu().numpy(), site_counts[:, :n].cpu().numpy(), site_dpa.cpu().numpy(),
+                site_mask.cpu().numpy())
+
+
+def deletion_events(dbatch: DeviceBatch):
+    """K7 (extension): every deletion event (slot, length) of the batch's CIGARs, in read order and then op order, as
+    device tensors (int64[m], int32[m]).  A D op is an event when it lies inside its contig (include/kindel_b200.h)."""
+    lib = _ffi.load()
+    dev = dbatch.device
+    with torch.cuda.device(dev):
+        sums = torch.empty(int(lib.kdl_deletion_scratch_words(dbatch.host.n_reads)), dtype=torch.int32, device=dev)
+        _ffi.check(lib.kdl_deletion_count(C.byref(dbatch.struct), sums.data_ptr(), _stream_ptr(dev)),
+                   "kdl_deletion_count")
+        m = int(sums[-1].item()) & 0xFFFFFFFF
+        ev_slot = torch.empty(max(m, 1), dtype=torch.int64, device=dev)
+        ev_len = torch.empty(max(m, 1), dtype=torch.int32, device=dev)
+        rc = lib.kdl_deletion_scatter(C.byref(dbatch.struct), sums.data_ptr(), m, ev_slot.data_ptr(), ev_len.data_ptr(),
+                                      _stream_ptr(dev))
+        _ffi.check(rc, "kdl_deletion_scatter")
+    return ev_slot[:m], ev_len[:m]
+
+
+_LEN_BITS = 28  # a CIGAR op length has 28 bits
+
+
+def deletion_alleles(dbatch: DeviceBatch, counts: torch.Tensor, abs_threshold, rel_threshold):
+    """The deletion alleles of `variants --vcf --reference` (extension): K7's events grouped by (slot, length) on the
+    device, each with its count c and the six-allele depth D of its first slot (columns 0-5 of `counts`, a device
+    table of the same batch); kept when c > abs_threshold and c / D > rel_threshold (0 at D = 0).  Only the kept
+    groups leave the device: (slot, length, count, depth), int64 numpy arrays sorted by slot, then length."""
+    ev_slot, ev_len = deletion_events(dbatch)
+    if ev_slot.numel() == 0:
+        z = np.zeros(0, dtype=np.int64)
+        return z, z.copy(), z.copy(), z.copy()
+    with torch.cuda.device(counts.device):
+        key, cnt = torch.unique((ev_slot << _LEN_BITS) | ev_len.to(torch.int64), sorted=True, return_counts=True)
+        slot = key >> _LEN_BITS
+        length = key & ((1 << _LEN_BITS) - 1)
+        depth = counts[0:6].index_select(1, slot).to(torch.int64).sum(dim=0)
+        share = torch.where(depth > 0, cnt.to(torch.float64) / depth.clamp(min=1).to(torch.float64),
+                            torch.zeros((), dtype=torch.float64, device=counts.device))
+        keep = (cnt > variant_abs_floor(abs_threshold)) & (share > float(rel_threshold))
+        return tuple(x[keep].cpu().numpy().astype(np.int64) for x in (slot, length, cnt, depth))
 
 
 class HostContext:

@@ -907,7 +907,7 @@ _VCF_ALT = ((0, "A"), (1, "C"), (2, "G"), (3, "T"), (5, "*"))  # N (4) is not an
 
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
-                 exclude_flags=0) -> str:
+                 exclude_flags=0, reference=None) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -917,33 +917,50 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     missing due to an upstream deletion, which is what the per-position deletion count is); ID and QUAL `.`, FILTER
     PASS; INFO DP (the depth A+C+G+T+N+deletions), AD (the REF count, then each ALT's) and AF (each ALT's share of the
     depth, rounded to 4 decimals: the value `variants` prints).  A site whose only variant allele is N is not
-    written.  devices and the filters: extensions, see pileup_run."""
+    written.  devices and the filters: extensions, see pileup_run.
+
+    reference (extension: `--reference`): the FASTA the alignment was made against -- a path, or a Reference that
+    reference.load_reference returned for this file's batch.  REF is then the reference's base, and the records are
+    SNVs against it, deletions and insertions (variants_vcf_from_run has the rules)."""
     filters = (min_base_quality, min_mapq, exclude_flags)
     run = pileup_run(bam_path, devices, 1, *filters)[0]
-    return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters)
+    return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference)
 
 
-def _vcf_header(run, abs_threshold, rel_threshold, filters):
+def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None):
     from . import __version__
 
     mbq, mapq, flags = filters if filters is not None else (0, 0, 0)
     lines = ["##fileformat=VCFv4.2", "##source=kindel {}".format(__version__),
              "##kindelVariants=abs_threshold={};rel_threshold={};min_base_quality={};min_mapq={};exclude_flags={:#x}"
              .format(abs_threshold, rel_threshold, mbq, mapq, flags)]
+    if reference_name is not None:
+        lines.append("##reference={}".format(reference_name))
     lines += ["##contig=<ID={},length={}>".format(name, int(L))
               for name, L in zip(run.batch.contig_names, run.batch.contig_len)]
     lines += ['##INFO=<ID=DP,Number=1,Type=Integer,Description="Depth: A + C + G + T + N + deletions">',
               '##INFO=<ID=AD,Number=R,Type=Integer,Description="Count of REF (the most frequent allele) and of each '
-              'ALT allele">',
+              'ALT allele">' if reference_name is None else
+              '##INFO=<ID=AD,Number=R,Type=Integer,Description="Count of the REF base and of each ALT base (SNVs)">',
               '##INFO=<ID=AF,Number=A,Type=Float,Description="Share of the depth of each ALT allele, rounded to 4 '
-              'decimals">',
-              "#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO"]
+              'decimals">']
+    if reference_name is not None:
+        lines += ['##INFO=<ID=INDEL,Number=0,Type=Flag,Description="The record is an insertion or a deletion">',
+                  '##INFO=<ID=AO,Number=A,Type=Integer,Description="Count of the reads carrying the ALT allele">']
+    lines.append("#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO")
     return lines
 
 
-def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None) -> str:
+def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None, reference=None) -> str:
     """Host half of variants_vcf (see there): the VCF text of a finished pileup.  filters: (min_base_quality,
-    min_mapq, exclude_flags) as the pileup applied them, for the header."""
+    min_mapq, exclude_flags) as the pileup applied them, for the header.  reference: see variants_vcf; with it the
+    records are _reference_records'."""
+    if reference is not None:
+        from .reference import Reference, load_reference
+
+        ref = reference if isinstance(reference, Reference) else load_reference(reference, run.batch)
+        lines = _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=ref.name)
+        return "\n".join(lines + _reference_records(run, ref.codes, abs_threshold, rel_threshold)) + "\n"
     lines = _vcf_header(run, abs_threshold, rel_threshold, filters)
     site_slot, site_counts, site_mask = variant_sites(run, abs_threshold, rel_threshold)
     batch = run.batch
@@ -965,6 +982,90 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
         lines.append("\t".join((batch.contig_names[c], str(int(site_slot[i] - contig_slot[c]) + 1), ".", ref,
                                 ",".join(letter for _, letter in alts), ".", "PASS", info)))
     return "\n".join(lines) + "\n"
+
+
+_ACGTN = str.maketrans({c: "N" for c in "=MRSVWYHKDB"})  # inserted bases: anything but A, C, G, T, N becomes N
+
+
+def _af(count, depth) -> str:
+    """A share rounded to 4 decimals as `variants` prints it (0 at depth 0)."""
+    return repr(float(np.round(np.float64(count / depth if depth > 0 else 0.0), 4)))
+
+
+def _reference_records(run, ref_codes, abs_threshold, rel_threshold):
+    """The VCF data lines against reference codes ref_codes (uint8 per slot, reference.py): SNVs from K6r's sites,
+    deletions from K7's grouped events, insertions from K6r's candidate slots and their strings (InsertionTable).
+
+    SNV, per position p with a variant base: POS p + 1, REF the reference letter, ALT the variant bases in A, C, G, T
+    order; INFO DP (six-allele depth), AD (the REF base's count -- 0 when the reference has no A, C, G or T there --
+    then each ALT's) and AF.  Deletion (r, n), count c, D = the depth at r: POS r, REF ref[r-1 .. r+n], ALT ref[r-1];
+    at r = 0 POS 1, REF ref[0 .. n], ALT ref[n] (no record for n = L).  Insertion of string s at slot p (first-seen
+    order of the slot's strings, empty ones skipped), count c against DPa: POS p, REF ref[p-1], ALT ref[p-1] + s; at
+    p = 0 POS 1, REF ref[0], ALT s + ref[0].  Indels carry INFO INDEL;DP;AO (= c);AF.  An allele passes when its count
+    exceeds abs_threshold and its share exceeds rel_threshold.  Order: contigs as in the batch, then POS, then SNV <
+    deletion < insertion, then deletion length, then insertion slot and first-seen order."""
+    batch = run.batch
+    counts = run.counts
+    dbatch = run.dbatch
+    if counts is None:  # host tables (the multi-GPU result): the reduced table and the batch go to this process's GPU
+        import torch
+
+        dev = engine.require_cuda()
+        counts = torch.from_numpy(run.host_counts).to(dev)
+        dbatch = engine.upload(batch, dev)
+    contig_slot = np.asarray(batch.contig_slot, dtype=np.int64)
+    contig_len = np.asarray(batch.contig_len, dtype=np.int64)
+    letters = np.frombuffer(b"ACGTN", dtype=np.uint8)[np.minimum(np.asarray(ref_codes), 4)].tobytes().decode("ascii")
+    recs = []  # (contig, POS, kind, deletion length, insertion slot, first-seen rank, line)
+
+    slot, site_counts, dpa, mask = engine.variant_sites_ref(counts, contig_slot, contig_len, ref_codes, abs_threshold,
+                                                            rel_threshold)
+    t = site_counts.astype(np.int64)
+    depth = t[0:6].sum(axis=0)
+    contig = np.searchsorted(contig_slot, slot, side="right") - 1
+    ins_table = run.ins_table if (mask & 64).any() else None
+    for i in range(slot.shape[0]):
+        c, s, m = int(contig[i]), int(slot[i]), int(mask[i])
+        s0, L, name = int(contig_slot[c]), int(contig_len[c]), batch.contig_names[c]
+        p = s - s0
+        if m & 15:
+            alts = [k for k in range(4) if m >> k & 1]
+            g = int(ref_codes[s])
+            ad = [int(t[g, i]) if g < 4 else 0] + [int(t[k, i]) for k in alts]
+            info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(map(str, ad)),
+                                              ",".join(_af(int(t[k, i]), int(depth[i])) for k in alts))
+            recs.append((c, p + 1, 0, 0, 0, 0, "\t".join((name, str(p + 1), ".", letters[s],
+                                                            ",".join("ACGT"[k] for k in alts), ".", "PASS", info))))
+        if m & 64 and L > 0:
+            da = int(dpa[i])
+            for rank, (text, cnt) in enumerate(ins_table.dict_at(s).items()):
+                if not text or not (cnt > abs_threshold and (cnt / da if da > 0 else 0.0) > rel_threshold):
+                    continue
+                text = text.translate(_ACGTN)
+                if p >= 1:
+                    pos, ref, alt = p, letters[s - 1], letters[s - 1] + text
+                else:
+                    pos, ref, alt = 1, letters[s0], text + letters[s0]
+                recs.append((c, pos, 2, 0, s, rank, "\t".join((name, str(pos), ".", ref, alt, ".", "PASS",
+                                                                "INDEL;DP={};AO={};AF={}".format(da, cnt, _af(cnt, da))))))
+
+    d_slot, d_len, d_cnt, d_depth = engine.deletion_alleles(dbatch, counts, abs_threshold, rel_threshold)
+    d_contig = np.searchsorted(contig_slot, d_slot, side="right") - 1
+    for i in range(d_slot.shape[0]):
+        c, s, n = int(d_contig[i]), int(d_slot[i]), int(d_len[i])
+        s0, L, name = int(contig_slot[c]), int(contig_len[c]), batch.contig_names[c]
+        r = s - s0
+        if r >= 1:
+            pos, ref, alt = r, letters[s - 1:s + n], letters[s - 1]
+        elif n < L:
+            pos, ref, alt = 1, letters[s0:s0 + n + 1], letters[s0 + n]
+        else:
+            continue  # the whole contig deleted: no base is left to anchor the record
+        cnt, dp = int(d_cnt[i]), int(d_depth[i])
+        recs.append((c, pos, 1, n, 0, 0, "\t".join((name, str(pos), ".", ref, alt, ".", "PASS",
+                                                     "INDEL;DP={};AO={};AF={}".format(dp, cnt, _af(cnt, dp))))))
+    recs.sort(key=lambda x: x[:6])
+    return [x[6] for x in recs]
 
 
 def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0):
