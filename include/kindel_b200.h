@@ -322,6 +322,31 @@ int kdl_deletion_count(const kdl_batch* batch, uint32_t* block_sums, void* strea
 int kdl_deletion_scatter(const kdl_batch* batch, const uint32_t* block_sums, int64_t n_events, int64_t* ev_slot,
                          int32_t* ev_len, void* stream);
 
+/* K8 (extension: `variants --vcf --strand`): the sub-batch of the reads with keep[r] != 0, built on the device.  The
+ * result equals what the host's bamio.select_reads gives for np.flatnonzero(keep), field for field: the kept reads in
+ * their order; seq_off dense; l_seq the parent's word (classification is per read); seq4 each kept read's bases and, for
+ * a complex read, its [n_ops][evt_off][ops] trailer with evt_off the exclusive prefix of the kept reads' I-op counts;
+ * contig_read_off, complex_idx and hard_idx remapped; reads_sorted recomputed over the kept reads; max_simple_len,
+ * reach_right and reach_left the maxima over the kept reads (simple: the op length; tile-eligible: r_span + 1 and
+ * lead + 1 of the CIGAR walk); the mask list with read_idx remapped, off rebuilt and the qpos runs copied.
+ * contig_len / contig_slot / n_contigs are the parent's (the result may share them).
+ *   kdl_select_count    per-CTA counts and maxima, then one CTA combines them.  scratch: device uint32
+ *                       [kdl_select_scratch_words(n_reads)]; its last 16 words are the totals record, read back once:
+ *                       [0] reads, [1] seq4 words, [2] complex reads, [3] hard reads, [4] insertion events, [5] reads
+ *                       with masked bases, [6] masked bases, [7] reads_sorted, [8] max_simple_len, [9] reach_right,
+ *                       [10] reach_left.
+ *   kdl_select_scatter  on the same stream after it: writes the sub-batch into `out`, whose scalars the caller set
+ *                       from the totals and whose arrays it sized by them (complex_idx / hard_idx may be NULL when
+ *                       their count is 0; contig_read_off [n_contigs + 1]); out_mask (NULL when totals[5] == 0)
+ *                       receives the mask list.
+ * qmask may be NULL or empty.  One thread per read counts; the scatter copies each CTA's kept words as one coalesced
+ * range. */
+int64_t kdl_select_scratch_words(int64_t n_reads);
+int kdl_select_count(const kdl_batch* batch, const kdl_qmask* qmask, const uint8_t* keep, uint32_t* scratch,
+                     void* stream);
+int kdl_select_scatter(const kdl_batch* batch, const kdl_qmask* qmask, const uint8_t* keep, const uint32_t* scratch,
+                       const kdl_batch* out, const kdl_qmask* out_mask, void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced
@@ -427,7 +452,8 @@ int kdl_ctx_last_timing(kdl_ctx* ctx, float* h2d_ms, float* kernel_ms, float* d2
  *                    before classification.  Refused (KDL_ERR_INVALID_ARG) for SAM text whose MAPQ / QUAL fields the
  *                    text parser could not carry when the filter would read them.  prepare's info[13] = masked bases,
  *                    info[14] = reads with masked bases
- *   kdl_bam_fill_mask   after fill: the kdl_qmask arrays, read_idx [info[14]], off [info[14] + 1], qpos [info[13]] */
+ *   kdl_bam_fill_mask   after fill: the kdl_qmask arrays, read_idx [info[14]], off [info[14] + 1], qpos [info[13]]
+ *   kdl_bam_fill_strand after fill (extension): reverse [n_kept], 1 where the kept read's FLAG has 0x10, in read order */
 typedef struct kdl_bam kdl_bam;
 int kdl_bam_open(const char* path, int threads, kdl_bam** out);
 void kdl_bam_close(kdl_bam* h);
@@ -442,6 +468,7 @@ int kdl_bam_fill(kdl_bam* h, int threads, const int64_t* contig_slot, int32_t* r
                  uint32_t* complex_idx, uint32_t* hard_idx, int64_t* info);
 int kdl_bam_set_filter(kdl_bam* h, int32_t min_mapq, int32_t exclude_flags, int32_t min_base_quality);
 int kdl_bam_fill_mask(kdl_bam* h, int threads, uint32_t* read_idx, uint32_t* off, uint32_t* qpos);
+int kdl_bam_fill_strand(kdl_bam* h, int threads, uint8_t* reverse);
 
 #ifdef __cplusplus
 }

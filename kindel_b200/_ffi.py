@@ -131,6 +131,10 @@ _PROTOTYPES = {
     "kdl_deletion_count": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p]),
     "kdl_deletion_scatter": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                        C.c_void_p]),
+    "kdl_select_scratch_words": (C.c_int64, [C.c_int64]),
+    "kdl_select_count": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_select_scatter": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_void_p,
+                                     C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p]),
     "kdl_vote_peers":(C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,
@@ -164,6 +168,7 @@ _PROTOTYPES = {
                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_bam_set_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
     "kdl_bam_fill_mask": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_bam_fill_strand": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -26,6 +26,8 @@ nibble becomes N (15) in `seq4` before the reads are classified, and its query o
 (`mask_read` / `mask_off` / `mask_qpos`), from which K1q (csrc/pileup_mask.cu) takes back the count the N added to a
 base column.  A record without qualities (SAM `*`, BAM 0xff) is never masked; with min_base_quality == 0 QUAL is not
 read at all.
+With `strand=True` the batch also keeps each kept read's strand (`reverse`, FLAG & 0x10), which `variants --vcf
+--strand` splits the pileup by; it costs nothing when off.
 
 The result is a `ReadBatch` (numpy arrays in host memory) described in include/kindel_b200.h.
 """
@@ -84,6 +86,8 @@ class ReadBatch:
     mask_read: np.ndarray = field(default=None)     # uint32 [m]: ascending indices of the reads with masked bases
     mask_off: np.ndarray = field(default=None)      # uint32 [m+1]: their entries in mask_qpos
     mask_qpos: np.ndarray = field(default=None)     # uint32 [n_masked]: query offsets, ascending per read
+    # strand (extension; `strand=True` at decode): 1 where the read's FLAG has 0x10.  None = not asked for.
+    reverse: np.ndarray = field(default=None)       # uint8 [n]
 
     @property
     def n_reads(self) -> int:
@@ -224,7 +228,7 @@ def mask_bases(seq4: np.ndarray, seq_off: np.ndarray, counts: np.ndarray, qpos: 
 
 
 def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_seq, cig_off, cigar, seq4,
-             n_records=0, exotic=None, qual=None, min_base_quality=0, mask=None) -> ReadBatch:
+             n_records=0, exotic=None, qual=None, min_base_quality=0, mask=None, reverse=None) -> ReadBatch:
     """Classify reads (simple / tile-eligible complex / hard), lay the complex reads' CIGARs behind their bases,
     detect coordinate order.  All vectorised numpy; shared by the BAM, SAM and synthetic paths.
 
@@ -232,7 +236,8 @@ def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_se
     bases in `seq4` (any layout: gaps and extra words between reads are allowed and dropped).
     qual + min_base_quality > 0: concatenated Phred qualities (one byte per base, 0xff = none); the bases below the
     threshold are masked (N in seq4, listed in the mask) BEFORE classification.  mask = (per-read counts, query
-    offsets): a mask already applied to `seq4` (re-finalizing a masked batch), carried into the result."""
+    offsets): a mask already applied to `seq4` (re-finalizing a masked batch), carried into the result.
+    reverse: the reads' strand bytes (1 = FLAG & 0x10), carried into the result."""
     contig_len = np.ascontiguousarray(contig_len, dtype=np.int32)
     contig_read_off = np.ascontiguousarray(contig_read_off, dtype=np.int64)
     ref_start = np.ascontiguousarray(ref_start, dtype=np.int32)
@@ -344,6 +349,7 @@ def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_se
         complex_idx=complex_idx, n_events=n_events, reads_sorted=sorted_ok, aligned_bases=aligned,
         n_records=int(n_records), max_simple_len=int(oplen[simple].max()) if simple.any() else 0,
         reach_right=reach_right, reach_left=reach_left, mask_read=mask_read, mask_off=mask_off, mask_qpos=mask_qpos,
+        reverse=None if reverse is None else np.ascontiguousarray(reverse, dtype=np.uint8),
     )
 
 
@@ -365,7 +371,8 @@ def with_mask(batch: ReadBatch, counts: np.ndarray, qpos: np.ndarray) -> ReadBat
     qpos = np.asarray(qpos, dtype=np.uint32)
     seq4 = mask_bases(batch.seq4, batch.seq_off, counts, qpos)
     return finalize(batch.contig_names, batch.contig_len, batch.contig_read_off, batch.ref_start, batch.seq_off,
-                    batch.seq_len, batch.cig_off, batch.cigar, seq4, n_records=batch.n_records, mask=(counts, qpos))
+                    batch.seq_len, batch.cig_off, batch.cigar, seq4, n_records=batch.n_records, mask=(counts, qpos),
+                    reverse=batch.reverse)
 
 
 def select_reads(batch: ReadBatch, idx) -> ReadBatch:
@@ -388,7 +395,8 @@ def select_reads(batch: ReadBatch, idx) -> ReadBatch:
     seq_src = np.repeat(batch.seq_off.astype(np.int64)[idx], words) + (
         np.arange(int(seq_off[-1])) - np.repeat(seq_off[:-1], words))
     return finalize(batch.contig_names, batch.contig_len, read_off, batch.ref_start[idx], seq_off[:-1], lseq,
-                          cig_off, batch.cigar[cig_src], batch.seq4[seq_src], n_records=n, mask=_mask_of(batch, idx))
+                          cig_off, batch.cigar[cig_src], batch.seq4[seq_src], n_records=n, mask=_mask_of(batch, idx),
+                          reverse=None if batch.reverse is None else batch.reverse[idx])
 
 
 
@@ -402,7 +410,8 @@ def _ragged_gather(src: np.ndarray, starts: np.ndarray, lens: np.ndarray) -> np.
 
 def merge_batches(batches) -> ReadBatch:
     """All reads of several batches over the SAME contigs as one batch, coordinate-sorted inside every contig
-    (stable: ties keep batch order).  Used to mix synthetic read populations; not a hot path."""
+    (stable: ties keep batch order).  Used to mix synthetic read populations; not a hot path.  The strand bytes are
+    carried when every batch has them."""
     first = batches[0]
     for b in batches[1:]:
         if list(b.contig_names) != list(first.contig_names) or not np.array_equal(b.contig_len, first.contig_len):
@@ -427,8 +436,12 @@ def merge_batches(batches) -> ReadBatch:
         mcount = np.concatenate([b.mask_counts() for b in batches])
         mq = np.concatenate([b.mask_qpos if b.n_masked else np.zeros(0, dtype=np.uint32) for b in batches])
         mask = (mcount[order], _ragged_gather(mq, (np.cumsum(mcount) - mcount)[order], mcount[order]))
+    reverse = None
+    if all(b.reverse is not None for b in batches):
+        reverse = np.concatenate([b.reverse for b in batches])[order]
     return finalize(first.contig_names, first.contig_len, read_off, ref_start[order], base_at[order], lseq[order],
-                    cig_off, _ragged_gather(cigar, cig_at[order], nco), bases, n_records=int(order.shape[0]), mask=mask)
+                    cig_off, _ragged_gather(cigar, cig_at[order], nco), bases, n_records=int(order.shape[0]), mask=mask,
+                    reverse=reverse)
 
 
 _SAVE_FIELDS = ("contig_len", "contig_read_off", "contig_slot", "ref_start", "seq_off", "l_seq", "seq_len", "cig_off",
@@ -436,6 +449,7 @@ _SAVE_FIELDS = ("contig_len", "contig_read_off", "contig_slot", "ref_start", "se
 _SAVE_SCALARS = ("n_slots", "n_events", "reads_sorted", "aligned_bases", "n_records", "max_simple_len", "reach_right",
                  "reach_left")
 _MASK_FIELDS = ("mask_read", "mask_off", "mask_qpos")  # saved only when the batch has masked bases
+_STRAND_FIELDS = ("reverse",)  # saved only when the batch has its strands
 
 
 def save_batch(directory: str, batch: ReadBatch) -> None:
@@ -443,10 +457,11 @@ def save_batch(directory: str, batch: ReadBatch) -> None:
     import json
 
     os.makedirs(directory, exist_ok=True)
-    for f in _MASK_FIELDS:
+    for f in _MASK_FIELDS + _STRAND_FIELDS:
         if os.path.exists(os.path.join(directory, f + ".npy")):
             os.remove(os.path.join(directory, f + ".npy"))
-    for f in _SAVE_FIELDS + (_MASK_FIELDS if batch.n_masked else ()):
+    for f in (_SAVE_FIELDS + (_MASK_FIELDS if batch.n_masked else ())
+              + (_STRAND_FIELDS if batch.reverse is not None else ())):
         np.save(os.path.join(directory, f + ".npy"), np.ascontiguousarray(getattr(batch, f)))
     meta = {k: (bool(getattr(batch, k)) if k == "reads_sorted" else int(getattr(batch, k))) for k in _SAVE_SCALARS}
     meta["contig_names"] = list(batch.contig_names)
@@ -460,7 +475,7 @@ def load_batch(directory: str, mmap: bool = True) -> ReadBatch:
     with open(os.path.join(directory, "batch.json")) as fh:
         meta = json.load(fh)
     arrays = {f: np.load(os.path.join(directory, f + ".npy"), mmap_mode="r" if mmap else None) for f in _SAVE_FIELDS}
-    for f in _MASK_FIELDS:
+    for f in _MASK_FIELDS + _STRAND_FIELDS:
         if os.path.exists(os.path.join(directory, f + ".npy")):
             arrays[f] = np.load(os.path.join(directory, f + ".npy"), mmap_mode="r" if mmap else None)
     return ReadBatch(contig_names=meta.pop("contig_names"), **arrays, **meta)
@@ -548,11 +563,12 @@ def decode_threads() -> int:
 
 
 def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0, exclude_flags: int = 0,
-             min_base_quality: int = 0) -> ReadBatch:
+             min_base_quality: int = 0, strand: bool = False) -> ReadBatch:
     """.bam -> ReadBatch through the C++ decoder (bam_host.cpp): BGZF inflate, filter, classification and the
     device layout (inline CIGAR blocks included) in threads, no Python per-record or per-array work.
     pinned=True puts the arrays the device consumes into page-locked memory (needs torch + CUDA).
-    min_mapq / exclude_flags / min_base_quality: the filters of this module's docstring (extension)."""
+    min_mapq / exclude_flags / min_base_quality: the filters of this module's docstring (extension).  strand=True
+    (extension): also the kept reads' strands, `reverse` (kdl_bam_fill_strand)."""
     import ctypes as C
 
     filters = check_filters(min_mapq, exclude_flags, min_base_quality)
@@ -614,6 +630,10 @@ def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0,
                         mask_qpos=buf(n_masked, np.uint32))
             _ffi.check(lib.kdl_bam_fill_mask(h, threads, mask["mask_read"].ctypes.data, mask["mask_off"].ctypes.data,
                                              mask["mask_qpos"].ctypes.data), "kdl_bam_fill_mask")
+        if strand:
+            mask["reverse"] = np.zeros(n, dtype=np.uint8)
+            _ffi.check(lib.kdl_bam_fill_strand(h, threads, mask["reverse"].ctypes.data if n else None),
+                       "kdl_bam_fill_strand")
     finally:
         lib.kdl_bam_close(h)
     return ReadBatch(
@@ -682,10 +702,11 @@ def _sam_qual(text: str, seq: str) -> bytes:
     return bytes(c - 33 for c in raw)
 
 
-def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0) -> ReadBatch:
+def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0,
+             strand: bool = False) -> ReadBatch:
     min_mapq, exclude_flags, min_base_quality = check_filters(min_mapq, exclude_flags, min_base_quality)
     header = []
-    groups = {}  # rname -> list of (pos0, cigar words, seq, qualities)
+    groups = {}  # rname -> list of (pos0, cigar words, seq, qualities, reverse)
     n_records = 0
     with open(path, "rt") as fh:
         for line in fh:
@@ -712,7 +733,7 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
                 if mapq < min_mapq:
                     continue
             qual = _sam_qual(f[10], seq) if min_base_quality else None
-            g.append((int(f[3]) - 1, parse_cigar_text(f[5]), seq, qual))
+            g.append((int(f[3]) - 1, parse_cigar_text(f[5]), seq, qual, 1 if flag & 0x10 else 0))
     groups.pop("*", None)  # kindel.py:147-148
     names, lens = _sq_from_text("\n".join(header))
     sq = dict(zip(names, lens))
@@ -720,11 +741,11 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
     for nm in contig_names:
         if nm not in sq:
             raise KeyError(nm)  # refs_lens[ref_id], kindel.py:151
-    ref_start, l_seq, cig_off, cigar, seq_off, seq_parts, quals = [], [], [0], [], [], [], []
+    ref_start, l_seq, cig_off, cigar, seq_off, seq_parts, quals, rev = [], [], [0], [], [], [], [], []
     read_off = [0]
     words = 0
     for nm in contig_names:
-        for pos0, cig, seq, qual in groups[nm]:
+        for pos0, cig, seq, qual, is_rev in groups[nm]:
             ref_start.append(pos0)
             l_seq.append(len(seq))
             cigar.extend(cig)
@@ -734,6 +755,7 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
             words += enc.size
             seq_parts.append(enc)
             quals.append(qual)
+            rev.append(is_rev)
         read_off.append(len(ref_start))
     seq4 = np.concatenate(seq_parts) if seq_parts else np.zeros(0, dtype=np.uint32)
     qual = np.frombuffer(b"".join(quals), dtype=np.uint8) if min_base_quality else None
@@ -741,14 +763,17 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
                     np.array(read_off, dtype=np.int64), np.array(ref_start, dtype=np.int64),
                     np.array(seq_off, dtype=np.int64), np.array(l_seq, dtype=np.int64),
                     np.array(cig_off, dtype=np.int64), np.array(cigar, dtype=np.int64), seq4,
-                    n_records=n_records, qual=qual, min_base_quality=min_base_quality)
+                    n_records=n_records, qual=qual, min_base_quality=min_base_quality,
+                    reverse=np.array(rev, dtype=np.uint8) if strand else None)
 
 
-def read_alignment(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0) -> ReadBatch:
-    """.bam or .sam (by content, not by suffix) -> ReadBatch.  The filters (extension): see the module docstring."""
+def read_alignment(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0,
+                   strand: bool = False) -> ReadBatch:
+    """.bam or .sam (by content, not by suffix) -> ReadBatch.  The filters and strand (extensions): see the module
+    docstring."""
     path = os.fspath(path)
     filters = dict(zip(("min_mapq", "exclude_flags", "min_base_quality"),
-                       check_filters(min_mapq, exclude_flags, min_base_quality)))
+                       check_filters(min_mapq, exclude_flags, min_base_quality)), strand=bool(strand))
     with open(path, "rb") as fh:
         magic = fh.read(4)
     if magic[:2] == b"\x1f\x8b" or magic == b"BAM\x01":

@@ -5,7 +5,8 @@ REPORT blocks to stderr and one `>name` / sequence pair per contig to stdout (cl
 extension one FASTQ record per contig instead),
 `weights` / `features` write TSV to stdout (cli.py:44,50), `version` prints `kindel <version>`;
 `variants` (in the reference's README only) is an extension, see kindel.variants; its `--vcf` writes a sites-only VCF
-(kindel.variants_vcf), against a FASTA with `--reference`.
+(kindel.variants_vcf), against a FASTA with `--reference`, with per-strand counts and a strand odds ratio with
+`--strand` / `--max-sor`.
 argh derived the flags from the function signatures (first letter as short option unless two
 parameters share it); argparse spells the same set out.  Note the CLI default `--min-overlap 7`
 (cli.py:13) differs from the API default 9 (kindel.py:492), as in the reference.
@@ -51,12 +52,14 @@ def features(bam_path, gpus=None, **filters):
 
 
 def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False, absolute=False, gpus=None, vcf=False,
-             reference=None, **filters):
+             reference=None, strand=False, max_sor=None, **filters):
     """Output variants exceeding specified absolute and relative frequency thresholds"""
     from . import kindel
 
     if vcf:  # extension: the sites of --only-variants as a sites-only VCF (against --reference when given)
         extra = {} if reference is None else dict(reference=reference)
+        if strand or max_sor is not None:  # extension: ADF / ADR / SOR (and FILTER sor)
+            extra.update(strand=True, max_sor=max_sor)
         sys.stdout.write(kindel.variants_vcf(bam_path, abs_threshold, rel_threshold, devices=gpus, **filters, **extra))
         return
     kindel.variants(bam_path, abs_threshold, rel_threshold, only_variants, absolute, devices=gpus, **filters).to_csv(
@@ -98,6 +101,12 @@ def _iupac_threshold(text: str) -> float:
     from .kindel import check_iupac_threshold
 
     return check_iupac_threshold(float(text))  # ValueError (NaN, outside [0, 1]) -> argparse error
+
+
+def _max_sor(text: str) -> float:
+    from .kindel import check_max_sor
+
+    return check_max_sor(float(text))  # ValueError (NaN) -> argparse error
 
 
 def _filters(a) -> dict:
@@ -169,8 +178,13 @@ def build_parser() -> argparse.ArgumentParser:
     # short option: -r is --rel-threshold)
     p.add_argument("--reference", default=None, metavar="FASTA",
                    help="with --vcf: call SNVs, insertions and deletions against this FASTA (plain or gzip)")
+    # extension: forward / reverse strand counts and the strand odds ratio of every record, and a filter on it
+    p.add_argument("--strand", action="store_true",
+                   help="with --vcf: add ADF / ADR (per-strand allele counts) and SOR (strand odds ratio) to INFO")
+    p.add_argument("--max-sor", type=_max_sor, default=None, metavar="X",
+                   help="with --vcf: FILTER `sor` where an ALT's strand odds ratio is above X (implies --strand)")
     p.set_defaults(func=lambda a: variants(a.bam_path, a.abs_threshold, a.rel_threshold, a.only_variants, a.absolute,
-                                           a.gpus, a.vcf, a.reference, **_filters(a)))
+                                           a.gpus, a.vcf, a.reference, a.strand, a.max_sor, **_filters(a)))
 
     p = sub.add_parser("plot", help=plot.__doc__, description=plot.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")
@@ -189,6 +203,8 @@ def _check_variants_args(parser, args):
                 parser.error("variants: --vcf cannot be combined with %s (a table option)" % flag)
     elif getattr(args, "reference", None) is not None:
         parser.error("variants: --reference needs --vcf (the table has no reference mode)")
+    elif getattr(args, "strand", False) or getattr(args, "max_sor", None) is not None:
+        parser.error("variants: --strand and --max-sor need --vcf (the table has no strand columns)")
 
 
 def main(argv=None):

@@ -13,6 +13,7 @@
 #include "vote.cu"
 #include "assemble.cu"
 #include "variants.cu"
+#include "select.cu"
 
 namespace {
 
@@ -532,6 +533,53 @@ int kdl_deletion_scatter(const kdl_batch* batch, const uint32_t* block_sums, int
     if (n_blocks == 0) return KDL_OK;
     kdl::deletion_scatter_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
         *batch, block_sums, n_events, ev_slot, ev_len);
+    return check_launch();
+}
+
+static long long select_blocks(int64_t n_reads) { return (n_reads + kdl::S_THREADS) / kdl::S_THREADS; }
+
+static int select_qmask(const kdl_qmask* qmask, kdl_qmask* q) {
+    *q = kdl_qmask{};
+    if (!qmask || qmask->n_reads == 0) return KDL_OK;
+    if (qmask->n_reads < 0 || qmask->n_bases < 0 || !qmask->read_idx || !qmask->off || (qmask->n_bases > 0 && !qmask->qpos))
+        return KDL_ERR_INVALID_ARG;
+    *q = *qmask;
+    return KDL_OK;
+}
+
+int64_t kdl_select_scratch_words(int64_t n_reads) {
+    return n_reads < 0 ? 0 : (int64_t)kdl::S_REC * (select_blocks(n_reads) + 1);
+}
+
+int kdl_select_count(const kdl_batch* batch, const kdl_qmask* qmask, const uint8_t* keep, uint32_t* scratch,
+                     void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    kdl_qmask q;
+    if ((rc = select_qmask(qmask, &q)) != KDL_OK) return rc;
+    if (!scratch || (batch->n_reads > 0 && !keep) || batch->n_reads >= (int64_t)UINT32_MAX) return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = select_blocks(batch->n_reads);
+    cudaStream_t st = (cudaStream_t)stream;
+    kdl::select_sums_kernel<<<(unsigned)n_blocks, kdl::S_THREADS, 0, st>>>(*batch, q, keep, scratch);
+    if ((rc = check_launch()) != KDL_OK) return rc;
+    kdl::select_combine_kernel<<<1, kdl::S_THREADS, 0, st>>>(scratch, n_blocks);
+    return check_launch();
+}
+
+int kdl_select_scatter(const kdl_batch* batch, const kdl_qmask* qmask, const uint8_t* keep, const uint32_t* scratch,
+                       const kdl_batch* out, const kdl_qmask* out_mask, void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    kdl_qmask q, om;
+    if ((rc = select_qmask(qmask, &q)) != KDL_OK || (rc = select_qmask(out_mask, &om)) != KDL_OK) return rc;
+    if ((rc = validate_batch(out)) != KDL_OK) return rc;
+    if (!scratch || (batch->n_reads > 0 && !keep) || batch->n_reads >= (int64_t)UINT32_MAX ||
+        out->n_reads > batch->n_reads || out->n_contigs != batch->n_contigs || !out->contig_read_off ||
+        (out->n_reads > 0 && out->seq4_words > 0 && !out->seq4))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = select_blocks(batch->n_reads);
+    kdl::select_scatter_kernel<<<(unsigned)n_blocks, kdl::S_THREADS, 0, (cudaStream_t)stream>>>(
+        *batch, q, keep, scratch, *out, const_cast<int64_t*>(out->contig_read_off), om);
     return check_launch();
 }
 

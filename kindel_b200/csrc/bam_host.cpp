@@ -1086,4 +1086,23 @@ int kdl_bam_fill_mask(kdl_bam* h, int threads, uint32_t* read_idx, uint32_t* off
     return KDL_OK;
 }
 
+// The strand of the last prepare's kept reads, in read order: reverse[k] = 1 where FLAG & 0x10, else 0.
+int kdl_bam_fill_strand(kdl_bam* h, int threads, uint8_t* reverse) {
+    if (!h || !h->prepared || (h->n_kept > 0 && !reverse)) return KDL_ERR_INVALID_ARG;
+    const uint8_t* d = h->dptr;
+    const int32_t n_ref = (int32_t)h->ref_name.size();
+    const int64_t n_tasks = (int64_t)h->chunk_lo.size() - 1;
+    h->pool->run(n_tasks, threads, [&](int64_t t, int) {
+        std::vector<int64_t> cr(h->cur_read.begin() + t * n_ref, h->cur_read.begin() + (t + 1) * n_ref);
+        RecView r;
+        for (int64_t i = h->chunk_lo[(size_t)t]; i < h->chunk_lo[(size_t)t + 1]; ++i) {
+            if (h->cls[(size_t)i].cls == CLS_DROP) continue;
+            const int64_t off_i = h->rec_off[(size_t)i];
+            parse_record(d + off_i, h->rec_off[(size_t)i + 1] - off_i, &r);
+            reverse[cr[(size_t)r.ref_id]++] = (r.flag & 0x10u) ? 1 : 0;
+        }
+    });
+    return KDL_OK;
+}
+
 }  // extern "C"

@@ -14,6 +14,7 @@ implementation behind these functions: without a CUDA device they raise.
     variant_sites(counts, ...) K6: the variant sites of `variants --only-variants` and the VCF (extension)
     variant_sites_ref(...)     K6r: the SNV and insertion-candidate sites against a reference (extension)
     deletion_alleles(dbatch, counts, ...)  K7 + grouping: the deletion alleles against a reference (extension)
+    select_reads(dbatch, keep) K8: the sub-batch of the kept reads, built on the device (extension)
 """
 from __future__ import annotations
 
@@ -77,6 +78,26 @@ def make_struct(host: ReadBatch, ptr: dict) -> _ffi.KdlBatch:
     s.hard_idx = ptr["hard_idx"] if host.n_hard else None
     s.tile_index = ptr.get("tile_index")
     return s
+
+
+@dataclass
+class BatchShape:
+    """The scalars of a batch that lives only on the device (a K8 result): what DeviceBatch and the pileup read of
+    their host batch, without the read data."""
+
+    n_reads: int
+    n_words: int
+    n_contigs: int
+    n_slots: int
+    n_complex: int
+    n_hard: int
+    n_events: int
+    n_masked: int
+    n_mask_reads: int
+    reads_sorted: bool
+    max_simple_len: int
+    reach_right: int
+    reach_left: int
 
 
 _FIELDS = ("ref_start", "seq_off", "l_seq", "seq4", "contig_read_off", "contig_len", "contig_slot", "complex_idx",
@@ -461,6 +482,76 @@ def variant_sites_ref(counts: torch.Tensor, contig_slot, contig_len, ref, abs_th
                 site_mask.cpu().numpy())
 
 
+_SELECT_TOTALS = 16  # words of K8's totals record (include/kindel_b200.h)
+
+
+def select_reads(dbatch: DeviceBatch, keep: torch.Tensor) -> DeviceBatch:
+    """K8 (extension): the sub-batch of the reads with keep[r] != 0 (uint8[n_reads], device), built on the device;
+    it equals bamio.select_reads(host, np.flatnonzero(keep)) field for field.  One 64-byte read-back sizes it; its
+    host side is a BatchShape (scalars only), and contig_len / contig_slot are shared with the parent."""
+    lib = _ffi.load()
+    dev = dbatch.device
+    n = int(dbatch.struct.n_reads)
+    with torch.cuda.device(dev):
+        keep = keep.to(dev, torch.uint8).contiguous()
+        if keep.numel() != n:
+            raise ValueError("keep must hold one byte per read (%d), got %d" % (n, keep.numel()))
+        qmask = C.byref(dbatch.qmask) if dbatch.qmask is not None else None
+        scratch = torch.empty(int(lib.kdl_select_scratch_words(n)), dtype=torch.int32, device=dev)
+        args = (C.byref(dbatch.struct), qmask, keep.data_ptr() if n else None, scratch.data_ptr())
+        _ffi.check(lib.kdl_select_count(*args, _stream_ptr(dev)), "kdl_select_count")
+        tot = scratch[-_SELECT_TOTALS:].cpu().numpy().view(np.uint32).astype(np.int64)
+        n_out, n_words, n_cx, n_hard, n_evt, n_mr, n_mb = (int(x) for x in tot[:7])
+
+        def empty(k, dtype=torch.int32):
+            return torch.empty(max(k, 1), dtype=dtype, device=dev)
+
+        t = dict(ref_start=empty(n_out), seq_off=empty(n_out), l_seq=empty(n_out), seq4=empty(n_words),
+                 contig_read_off=empty(dbatch.struct.n_contigs + 1, torch.int64), complex_idx=empty(n_cx),
+                 hard_idx=empty(n_hard), contig_len=dbatch.tensors["contig_len"],
+                 contig_slot=dbatch.tensors["contig_slot"],
+                 tile_index=torch.empty(8 * (dbatch.n_slots // _ffi.KDL_TILE), dtype=torch.int32, device=dev))
+        if n_mr:
+            t.update(mask_read=empty(n_mr), mask_off=empty(n_mr + 1), mask_qpos=empty(n_mb))
+        host = BatchShape(n_reads=n_out, n_words=n_words, n_contigs=int(dbatch.struct.n_contigs), n_slots=dbatch.n_slots,
+                          n_complex=n_cx, n_hard=n_hard, n_events=n_evt, n_masked=n_mb, n_mask_reads=n_mr,
+                          reads_sorted=bool(tot[7]), max_simple_len=int(tot[8]), reach_right=int(tot[9]),
+                          reach_left=int(tot[10]))
+        ptr = {f: int(x.data_ptr()) for f, x in t.items()}
+        s = _ffi.KdlBatch()
+        s.n_reads, s.seq4_words, s.n_contigs = n_out, n_words, host.n_contigs
+        s.reads_sorted, s.max_simple_len = int(host.reads_sorted), host.max_simple_len
+        s.reach_right, s.reach_left = host.reach_right, host.reach_left
+        for f in ("ref_start", "seq_off", "l_seq", "seq4", "contig_read_off", "contig_len", "contig_slot", "tile_index"):
+            setattr(s, f, ptr[f])
+        s.n_complex, s.n_hard = n_cx, n_hard
+        s.complex_idx = ptr["complex_idx"] if n_cx else None
+        s.hard_idx = ptr["hard_idx"] if n_hard else None
+        q = make_qmask(host, ptr) if n_mr else None
+        rc = lib.kdl_select_scatter(*args, C.byref(s), C.byref(q) if q is not None else None, _stream_ptr(dev))
+        _ffi.check(rc, "kdl_select_scatter")
+    return DeviceBatch(host=host, device=dev, tensors=t, struct=s, qmask=q)
+
+
+def download_fields(dbatch: DeviceBatch) -> dict:
+    """The device arrays and scalars of a batch, as host numpy (for checking a K8 result against the host's)."""
+    h = dbatch.host
+    sizes = dict(ref_start=h.n_reads, seq_off=h.n_reads, l_seq=h.n_reads, contig_read_off=h.n_contigs + 1,
+                 complex_idx=h.n_complex, hard_idx=h.n_hard)
+    sizes["seq4"] = h.n_words if isinstance(h, BatchShape) else int(h.seq4.shape[0])
+    if h.n_masked:
+        sizes.update(mask_read=h.n_mask_reads, mask_off=h.n_mask_reads + 1, mask_qpos=h.n_masked)
+    out = {f: dbatch.tensors[f][:k].cpu().numpy() for f, k in sizes.items()}
+    for f in ("seq_off", "seq4", "complex_idx", "hard_idx", "mask_read", "mask_off", "mask_qpos"):
+        if f in out:
+            out[f] = out[f].view(np.uint32)
+    if not h.n_masked:
+        out.update(mask_read=None, mask_off=None, mask_qpos=None)
+    out.update(n_events=h.n_events, reads_sorted=bool(h.reads_sorted), max_simple_len=int(h.max_simple_len),
+               reach_right=int(h.reach_right), reach_left=int(h.reach_left))
+    return out
+
+
 def deletion_events(dbatch: DeviceBatch):
     """K7 (extension): every deletion event (slot, length) of the batch's CIGARs, in read order and then op order, as
     device tensors (int64[m], int32[m]).  A D op is an event when it lies inside its contig (include/kindel_b200.h)."""
@@ -500,6 +591,22 @@ def deletion_alleles(dbatch: DeviceBatch, counts: torch.Tensor, abs_threshold, r
                             torch.zeros((), dtype=torch.float64, device=counts.device))
         keep = (cnt > variant_abs_floor(abs_threshold)) & (share > float(rel_threshold))
         return tuple(x[keep].cpu().numpy().astype(np.int64) for x in (slot, length, cnt, depth))
+
+
+def deletion_counts(dbatch: DeviceBatch, slot, length) -> np.ndarray:
+    """K7 over `dbatch` grouped on the device: how many of its deletion events are (slot[i], length[i]), for each
+    queried pair (host int64 arrays); int64 numpy.  `variants --vcf --strand` asks it of the reverse-strand reads."""
+    q = (np.asarray(slot, dtype=np.int64) << _LEN_BITS) | np.asarray(length, dtype=np.int64)
+    if q.size == 0:
+        return np.zeros(0, dtype=np.int64)
+    ev_slot, ev_len = deletion_events(dbatch)
+    if ev_slot.numel() == 0:
+        return np.zeros(q.shape[0], dtype=np.int64)
+    with torch.cuda.device(dbatch.device):
+        key, cnt = torch.unique((ev_slot << _LEN_BITS) | ev_len.to(torch.int64), sorted=True, return_counts=True)
+        tq = torch.from_numpy(q).to(key.device)
+        at = torch.searchsorted(key, tq).clamp(max=key.numel() - 1)
+        return torch.where(key[at] == tq, cnt[at], torch.zeros_like(cnt[at])).cpu().numpy().astype(np.int64)
 
 
 class HostContext:

@@ -15,13 +15,14 @@ There is no CPU implementation of the pileup or the vote in this package.
 from __future__ import annotations
 
 import logging
+import math
 import os
 from collections import OrderedDict, namedtuple
 
 import numpy as np
 
 from . import bamio, engine, quality
-from .insertions import InsertionTable, dict_consensus
+from .insertions import InsertionTable, decode_events, dict_consensus
 from .views import Alignment, BaseCounts, Insertions
 
 Region = namedtuple("Region", ["start", "end", "seq", "direction"])
@@ -52,6 +53,9 @@ except Exception:  # dnaio not installed: same three attributes
 class PileupRun:
     """One file's pileup on the device: count table, events, and lazily the host copies."""
 
+    _device = None   # (count table, DeviceBatch) of host tables, uploaded on demand (device_tables)
+    _reverse = None  # (count table, DeviceBatch) of the reverse-strand reads (reverse_table)
+
     def __init__(self, batch: bamio.ReadBatch, device=None):
         self.batch = batch
         self.dbatch = engine.upload(batch, device)
@@ -71,6 +75,33 @@ class PileupRun:
         run._host_derived = np.ascontiguousarray(derived, dtype=np.int32)
         run._ins = InsertionTable(batch, events)
         return run
+
+    def device_tables(self):
+        """(count table, DeviceBatch) on a device.  Host tables (a multi-GPU result): the reduced table and the batch
+        go to this process's GPU, once."""
+        if self.counts is not None:
+            return self.counts, self.dbatch
+        if self._device is None:
+            import torch
+
+            dev = engine.require_cuda()
+            self._device = (torch.from_numpy(self.host_counts).to(dev), engine.upload(self.batch, dev))
+        return self._device
+
+    def reverse_table(self):
+        """(count table, DeviceBatch) of the reverse-strand reads alone (extension: `variants --vcf --strand`), built
+        once: K8 selects the reads whose `reverse` byte is set into a device batch, and the unchanged pileup counts
+        them.  The forward table is the total minus this one.  Needs a batch decoded with strand=True."""
+        if self._reverse is None:
+            import torch
+
+            if self.batch.reverse is None:
+                raise ValueError("strand needs the reads' strands: decode the batch with strand=True")
+            _, dbatch = self.device_tables()
+            keep = torch.from_numpy(np.ascontiguousarray(self.batch.reverse, dtype=np.uint8)).to(dbatch.device)
+            sub = engine.select_reads(dbatch, keep)
+            self._reverse = (engine.pileup(sub)[0], sub)
+        return self._reverse
 
     def vote(self, min_depth=1, iupac_threshold=None) -> np.ndarray:
         """K2 over the whole table -> call bytes on the host (the device copy is kept for K5).  iupac_threshold:
@@ -152,16 +183,17 @@ def _default_devices(devices):
 
 
 def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq=0, exclude_flags=0,
-               iupac_threshold=None):
+               iupac_threshold=None, strand=False):
     """(PileupRun, calls) of an alignment file on `devices` GPUs.  devices > 1: one process per GPU, reads (or whole
     contigs) sharded, counts exchanged over NVLink in front of the vote (distributed.run_sharded); the result is
     bit-identical to one GPU.  min_base_quality / min_mapq / exclude_flags (extension, all off by default): a record
     with MAPQ < min_mapq or FLAG & exclude_flags is treated as unmapped; a base with Phred quality < min_base_quality
     is read as N and not counted (kindel_b200/bamio.py).  iupac_threshold: the vote of the sharded job (extension,
-    see bam_to_consensus); calls is None for one GPU, where the caller votes."""
+    see bam_to_consensus); calls is None for one GPU, where the caller votes.  strand (extension): the batch keeps
+    the reads' strands (PileupRun.reverse_table)."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
     batch = bamio.read_alignment(bam_path, min_mapq=min_mapq, exclude_flags=exclude_flags,
-                                 min_base_quality=min_base_quality)
+                                 min_base_quality=min_base_quality, strand=strand)
     devices = _default_devices(devices)
     if devices <= 1:
         run = PileupRun(batch)
@@ -907,7 +939,7 @@ _VCF_ALT = ((0, "A"), (1, "C"), (2, "G"), (3, "T"), (5, "*"))  # N (4) is not an
 
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
-                 exclude_flags=0, reference=None) -> str:
+                 exclude_flags=0, reference=None, strand=False, max_sor=None) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -921,19 +953,65 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
 
     reference (extension: `--reference`): the FASTA the alignment was made against -- a path, or a Reference that
     reference.load_reference returned for this file's batch.  REF is then the reference's base, and the records are
-    SNVs against it, deletions and insertions (variants_vcf_from_run has the rules)."""
+    SNVs against it, deletions and insertions (variants_vcf_from_run has the rules).
+
+    strand (extension: `--strand`): every record also carries ADF / ADR, the forward- and reverse-strand counts of REF
+    and of each ALT, and SOR, the strand odds ratio of each ALT; max_sor (`--max-sor`, implies strand): FILTER `sor`
+    where some ALT's SOR exceeds it.  _strand_fields has the rules."""
+    max_sor = check_max_sor(max_sor)
+    strand = bool(strand) or max_sor is not None
     filters = (min_base_quality, min_mapq, exclude_flags)
-    run = pileup_run(bam_path, devices, 1, *filters)[0]
-    return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference)
+    run = pileup_run(bam_path, devices, 1, *filters, strand=strand)[0]
+    return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference, strand=strand,
+                                 max_sor=max_sor)
 
 
-def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None):
+def check_max_sor(max_sor):
+    """None (no filter) or a float; NaN raises ValueError."""
+    if max_sor is None:
+        return None
+    x = float(max_sor)
+    if math.isnan(x):
+        raise ValueError("max_sor must be a number, got %r" % max_sor)
+    return x
+
+
+def strand_odds_ratio(f_ref, r_ref, f_alt, r_alt) -> float:
+    """GATK's StrandOddsRatio of one ALT from the forward / reverse counts of REF and of the ALT, in float64."""
+    t00, t01, t10, t11 = float(f_ref + 1), float(r_ref + 1), float(f_alt + 1), float(r_alt + 1)
+    ratio = (t00 / t01) * (t11 / t10) + (t01 / t00) * (t10 / t11)
+    return math.log(ratio) + math.log(min(t00, t01) / max(t00, t01)) - math.log(min(t10, t11) / max(t10, t11))
+
+
+def _strand_fields(adf, adr, max_sor):
+    """(FILTER, INFO tail) of a record whose REF and ALTs have forward counts adf and reverse counts adr: the tail is
+    ;ADF=..;ADR=..;SOR=.. (SOR per ALT, "%.3f"); FILTER is `sor` when max_sor is set and some ALT's SOR as written
+    exceeds it, else PASS."""
+    sor = ["%.3f" % strand_odds_ratio(adf[0], adr[0], adf[k], adr[k]) for k in range(1, len(adf))]
+    filt = "sor" if max_sor is not None and any(float(x) > max_sor for x in sor) else "PASS"
+    return filt, ";ADF={};ADR={};SOR={}".format(",".join(map(str, adf)), ",".join(map(str, adr)), ",".join(sor))
+
+
+def _rows_at(table, slots):
+    """Columns 0-5 of a device table at host slots, int64 [6, n] on the host."""
+    import torch
+
+    slots = np.asarray(slots, dtype=np.int64)
+    if slots.size == 0:
+        return np.zeros((6, 0), dtype=np.int64)
+    idx = torch.from_numpy(slots).to(table.device)
+    return table[0:6].index_select(1, idx).cpu().numpy().astype(np.int64)
+
+
+def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None, strand=False, max_sor=None):
     from . import __version__
 
     mbq, mapq, flags = filters if filters is not None else (0, 0, 0)
     lines = ["##fileformat=VCFv4.2", "##source=kindel {}".format(__version__),
              "##kindelVariants=abs_threshold={};rel_threshold={};min_base_quality={};min_mapq={};exclude_flags={:#x}"
              .format(abs_threshold, rel_threshold, mbq, mapq, flags)]
+    if strand:
+        lines.append("##kindelStrand=max_sor={}".format("." if max_sor is None else max_sor))
     if reference_name is not None:
         lines.append("##reference={}".format(reference_name))
     lines += ["##contig=<ID={},length={}>".format(name, int(L))
@@ -947,22 +1025,45 @@ def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None)
     if reference_name is not None:
         lines += ['##INFO=<ID=INDEL,Number=0,Type=Flag,Description="The record is an insertion or a deletion">',
                   '##INFO=<ID=AO,Number=A,Type=Integer,Description="Count of the reads carrying the ALT allele">']
+    if strand:
+        lines += ['##INFO=<ID=ADF,Number=R,Type=Integer,Description="Forward-strand count of REF and of each ALT '
+                  'allele">',
+                  '##INFO=<ID=ADR,Number=R,Type=Integer,Description="Reverse-strand count of REF and of each ALT '
+                  'allele">',
+                  '##INFO=<ID=SOR,Number=A,Type=Float,Description="Strand odds ratio of each ALT allele against REF">']
+        if max_sor is not None:
+            lines.append('##FILTER=<ID=sor,Description="The strand odds ratio of an ALT allele is above {}">'
+                         .format(max_sor))
     lines.append("#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO")
     return lines
 
 
-def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None, reference=None) -> str:
+def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None, reference=None, strand=False,
+                          max_sor=None) -> str:
     """Host half of variants_vcf (see there): the VCF text of a finished pileup.  filters: (min_base_quality,
-    min_mapq, exclude_flags) as the pileup applied them, for the header.  reference: see variants_vcf; with it the
-    records are _reference_records'."""
+    min_mapq, exclude_flags) as the pileup applied them, for the header.  reference, strand, max_sor: see variants_vcf;
+    with a reference the records are _reference_records'.  Strand needs a run whose batch has `reverse`
+    (ValueError otherwise).
+
+    Strand counts (ADF, ADR): without a reference they are the reverse table's counts of the record's AD columns and
+    the total's minus those, so ADF + ADR == AD.  With one, an SNV's the same (REF 0 where the reference has no A, C,
+    G or T); an indel's ALT entry is its reads on that strand (the reverse sub-batch's deletion events, the insertion
+    events of reverse reads) and its REF entry max(DP_s - AO_s, 0), DP_s the record's DP taken from strand s's table,
+    so ADF[1] + ADR[1] == AO."""
+    max_sor = check_max_sor(max_sor)
+    strand = bool(strand) or max_sor is not None
+    if strand and run.batch.reverse is None:
+        raise ValueError("strand needs the reads' strands: decode the batch with strand=True")
+    sargs = dict(strand=strand, max_sor=max_sor)
     if reference is not None:
         from .reference import Reference, load_reference
 
         ref = reference if isinstance(reference, Reference) else load_reference(reference, run.batch)
-        lines = _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=ref.name)
-        return "\n".join(lines + _reference_records(run, ref.codes, abs_threshold, rel_threshold)) + "\n"
-    lines = _vcf_header(run, abs_threshold, rel_threshold, filters)
+        lines = _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=ref.name, **sargs)
+        return "\n".join(lines + _reference_records(run, ref.codes, abs_threshold, rel_threshold, **sargs)) + "\n"
+    lines = _vcf_header(run, abs_threshold, rel_threshold, filters, **sargs)
     site_slot, site_counts, site_mask = variant_sites(run, abs_threshold, rel_threshold)
+    rev = _rows_at(run.reverse_table()[0], site_slot) if strand else None
     batch = run.batch
     contig_slot = np.asarray(batch.contig_slot, dtype=np.int64)
     t = site_counts.astype(np.int64)
@@ -977,10 +1078,16 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
         c = int(contig[i])
         tp = int(top[i])
         ref = "ACGT"[tp] if tp < 4 and depth[i] > 0 else "N"
-        info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(str(int(t[k, i])) for k in [tp] + [k for k, _ in alts]),
+        ks = [tp] + [k for k, _ in alts]
+        info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(str(int(t[k, i])) for k in ks),
                                           ",".join(repr(float(rounded[k, i])) for k, _ in alts))
+        filt = "PASS"
+        if strand:
+            adr = [int(rev[k, i]) for k in ks]
+            filt, tail = _strand_fields([int(t[k, i]) - x for k, x in zip(ks, adr)], adr, max_sor)
+            info += tail
         lines.append("\t".join((batch.contig_names[c], str(int(site_slot[i] - contig_slot[c]) + 1), ".", ref,
-                                ",".join(letter for _, letter in alts), ".", "PASS", info)))
+                                ",".join(letter for _, letter in alts), ".", filt, info)))
     return "\n".join(lines) + "\n"
 
 
@@ -992,7 +1099,7 @@ def _af(count, depth) -> str:
     return repr(float(np.round(np.float64(count / depth if depth > 0 else 0.0), 4)))
 
 
-def _reference_records(run, ref_codes, abs_threshold, rel_threshold):
+def _reference_records(run, ref_codes, abs_threshold, rel_threshold, strand=False, max_sor=None):
     """The VCF data lines against reference codes ref_codes (uint8 per slot, reference.py): SNVs from K6r's sites,
     deletions from K7's grouped events, insertions from K6r's candidate slots and their strings (InsertionTable).
 
@@ -1003,16 +1110,12 @@ def _reference_records(run, ref_codes, abs_threshold, rel_threshold):
     order of the slot's strings, empty ones skipped), count c against DPa: POS p, REF ref[p-1], ALT ref[p-1] + s; at
     p = 0 POS 1, REF ref[0], ALT s + ref[0].  Indels carry INFO INDEL;DP;AO (= c);AF.  An allele passes when its count
     exceeds abs_threshold and its share exceeds rel_threshold.  Order: contigs as in the batch, then POS, then SNV <
-    deletion < insertion, then deletion length, then insertion slot and first-seen order."""
+    deletion < insertion, then deletion length, then insertion slot and first-seen order.  strand / max_sor: the
+    strand fields of variants_vcf_from_run."""
     batch = run.batch
-    counts = run.counts
-    dbatch = run.dbatch
-    if counts is None:  # host tables (the multi-GPU result): the reduced table and the batch go to this process's GPU
-        import torch
-
-        dev = engine.require_cuda()
-        counts = torch.from_numpy(run.host_counts).to(dev)
-        dbatch = engine.upload(batch, dev)
+    # host tables (the multi-GPU result): the reduced table and the batch go to this process's GPU
+    counts, dbatch = run.device_tables()
+    rev_table, rev_batch = run.reverse_table() if strand else (None, None)
     contig_slot = np.asarray(batch.contig_slot, dtype=np.int64)
     contig_len = np.asarray(batch.contig_len, dtype=np.int64)
     letters = np.frombuffer(b"ACGTN", dtype=np.uint8)[np.minimum(np.asarray(ref_codes), 4)].tobytes().decode("ascii")
@@ -1024,6 +1127,10 @@ def _reference_records(run, ref_codes, abs_threshold, rel_threshold):
     depth = t[0:6].sum(axis=0)
     contig = np.searchsorted(contig_slot, slot, side="right") - 1
     ins_table = run.ins_table if (mask & 64).any() else None
+    if strand:
+        rev_site = _rows_at(rev_table, slot)
+        # the reverse depth each insertion is measured against: DPa's slot
+        rev_dpa = _rows_at(rev_table, np.where(slot - contig_slot[contig] >= 1, slot - 1, slot)).sum(axis=0)
     for i in range(slot.shape[0]):
         c, s, m = int(contig[i]), int(slot[i]), int(mask[i])
         s0, L, name = int(contig_slot[c]), int(contig_len[c]), batch.contig_names[c]
@@ -1034,23 +1141,41 @@ def _reference_records(run, ref_codes, abs_threshold, rel_threshold):
             ad = [int(t[g, i]) if g < 4 else 0] + [int(t[k, i]) for k in alts]
             info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(map(str, ad)),
                                               ",".join(_af(int(t[k, i]), int(depth[i])) for k in alts))
+            filt = "PASS"
+            if strand:
+                adr = [int(rev_site[g, i]) if g < 4 else 0] + [int(rev_site[k, i]) for k in alts]
+                filt, tail = _strand_fields([a - b for a, b in zip(ad, adr)], adr, max_sor)
+                info += tail
             recs.append((c, p + 1, 0, 0, 0, 0, "\t".join((name, str(p + 1), ".", letters[s],
-                                                            ",".join("ACGT"[k] for k in alts), ".", "PASS", info))))
+                                                            ",".join("ACGT"[k] for k in alts), ".", filt, info))))
         if m & 64 and L > 0:
             da = int(dpa[i])
-            for rank, (text, cnt) in enumerate(ins_table.dict_at(s).items()):
+            strings = ins_table.dict_at(s)
+            if strand:  # each string's reverse-strand reads: the event rows whose read is reverse
+                rows = ins_table.rows_at(s)
+                rev_of = {}
+                for text, r in zip(decode_events(batch, rows), batch.reverse[rows[:, 1].astype(np.int64)].tolist()):
+                    rev_of[text] = rev_of.get(text, 0) + r
+            for rank, (text, cnt) in enumerate(strings.items()):
                 if not text or not (cnt > abs_threshold and (cnt / da if da > 0 else 0.0) > rel_threshold):
                     continue
+                info = "INDEL;DP={};AO={};AF={}".format(da, cnt, _af(cnt, da))
+                filt = "PASS"
+                if strand:
+                    filt, tail = _indel_strand(da, int(rev_dpa[i]), cnt, rev_of.get(text, 0), max_sor)
+                    info += tail
                 text = text.translate(_ACGTN)
                 if p >= 1:
                     pos, ref, alt = p, letters[s - 1], letters[s - 1] + text
                 else:
                     pos, ref, alt = 1, letters[s0], text + letters[s0]
-                recs.append((c, pos, 2, 0, s, rank, "\t".join((name, str(pos), ".", ref, alt, ".", "PASS",
-                                                                "INDEL;DP={};AO={};AF={}".format(da, cnt, _af(cnt, da))))))
+                recs.append((c, pos, 2, 0, s, rank, "\t".join((name, str(pos), ".", ref, alt, ".", filt, info))))
 
     d_slot, d_len, d_cnt, d_depth = engine.deletion_alleles(dbatch, counts, abs_threshold, rel_threshold)
     d_contig = np.searchsorted(contig_slot, d_slot, side="right") - 1
+    if strand:
+        d_rev = engine.deletion_counts(rev_batch, d_slot, d_len)
+        d_rev_depth = _rows_at(rev_table, d_slot).sum(axis=0)
     for i in range(d_slot.shape[0]):
         c, s, n = int(d_contig[i]), int(d_slot[i]), int(d_len[i])
         s0, L, name = int(contig_slot[c]), int(contig_len[c]), batch.contig_names[c]
@@ -1062,10 +1187,21 @@ def _reference_records(run, ref_codes, abs_threshold, rel_threshold):
         else:
             continue  # the whole contig deleted: no base is left to anchor the record
         cnt, dp = int(d_cnt[i]), int(d_depth[i])
-        recs.append((c, pos, 1, n, 0, 0, "\t".join((name, str(pos), ".", ref, alt, ".", "PASS",
-                                                     "INDEL;DP={};AO={};AF={}".format(dp, cnt, _af(cnt, dp))))))
+        info = "INDEL;DP={};AO={};AF={}".format(dp, cnt, _af(cnt, dp))
+        filt = "PASS"
+        if strand:
+            filt, tail = _indel_strand(dp, int(d_rev_depth[i]), cnt, int(d_rev[i]), max_sor)
+            info += tail
+        recs.append((c, pos, 1, n, 0, 0, "\t".join((name, str(pos), ".", ref, alt, ".", filt, info))))
     recs.sort(key=lambda x: x[:6])
     return [x[6] for x in recs]
+
+
+def _indel_strand(dp, dp_rev, ao, ao_rev, max_sor):
+    """_strand_fields of an indel record: DP and AO in total and on the reverse strand; forward = total - reverse;
+    REF's entry on strand s is max(DP_s - AO_s, 0)."""
+    dp_fwd, ao_fwd = dp - dp_rev, ao - ao_rev
+    return _strand_fields([max(dp_fwd - ao_fwd, 0), ao_fwd], [max(dp_rev - ao_rev, 0), ao_rev], max_sor)
 
 
 def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0):

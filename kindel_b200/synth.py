@@ -3,6 +3,7 @@
     simple_reads(...)    coordinate-sorted `nM` short reads over one or more random contigs
                          (configs 2, 4, 5: 30 kb x 2000x, 5 Mb x 200x, 64 x 100 kb x 500x)
     complex_reads(...)   indel- and soft-clip-heavy CIGARs plus a tail of edge-case reads (config 3)
+    strands(...)         seeded strand bytes, with reads that must lie on one strand (alleles carried by one strand)
 
 Reads copy the contig's bases on M segments with a substitution rate (to A/C/G/T/N uniformly);
 inserted and clipped bases are random.  Everything is vectorised numpy so the 5 Mb x 200x case
@@ -229,7 +230,8 @@ def to_records(batch: bamio.ReadBatch):
             lseq = int(batch.seq_len[r])
             base = int(batch.seq_off[r])
             nib = bamio.unpack_nibbles(batch.seq4[base:base + (lseq + 7) // 8])[:lseq]
-            recs.append((c, int(batch.ref_start[r]), 0, words, "".join(bamio.NIBBLES[x] for x in nib.tolist())))
+            flag = 0 if batch.reverse is None else 16 * int(batch.reverse[r])
+            recs.append((c, int(batch.ref_start[r]), flag, words, "".join(bamio.NIBBLES[x] for x in nib.tolist())))
     return contigs, recs
 
 
@@ -262,7 +264,7 @@ def write_simple_bam(path, batch: bamio.ReadBatch, level: int = 1, threads: int 
     rec[:, 13] = 60
     put(14, np.full(n, 4680), "<u2")
     put(16, np.ones(n), "<u2")            # n_cigar_op
-    put(18, np.zeros(n), "<u2")           # flag
+    put(18, np.zeros(n) if batch.reverse is None else 16 * batch.reverse.astype(np.int64), "<u2")  # flag
     put(20, np.full(n, L), "<i4")
     put(24, np.full(n, -1), "<i4")
     put(28, np.full(n, -1), "<i4")
@@ -286,6 +288,25 @@ def write_simple_bam(path, batch: bamio.ReadBatch, level: int = 1, threads: int 
         for blk in blocks:
             fh.write(blk)
         fh.write(bamio._bgzf_block(b"", level))
+
+
+def strands(seed: int, n: int, p: float = 0.5, forward=None, reverse=None) -> np.ndarray:
+    """Seeded strand bytes of n reads (1 = reverse, FLAG 0x10): each read reverse with probability p, except the
+    reads listed in `forward` (all forward) and in `reverse` (all reverse) -- how a truth set plants alleles that only
+    one strand carries."""
+    out = (np.random.default_rng(seed).random(n) < p).astype(np.uint8)
+    if forward is not None:
+        out[np.asarray(forward, dtype=np.int64)] = 0
+    if reverse is not None:
+        out[np.asarray(reverse, dtype=np.int64)] = 1
+    return out
+
+
+def with_strands(batch: bamio.ReadBatch, seed: int, p: float = 0.5) -> bamio.ReadBatch:
+    """`batch` with seeded strands (strands(seed, n_reads, p)); the read data is shared."""
+    import dataclasses
+
+    return dataclasses.replace(batch, reverse=strands(seed, batch.n_reads, p))
 
 
 def qualities(seed: int, seq_len, low_frac: float = 0.05, chunk: int = 1 << 26) -> np.ndarray:

@@ -1,0 +1,158 @@
+"""Bench line of `variants --vcf --strand` (K8 and the reverse-strand pileup; an extension): BASELINE.json configs[3]
+(`cfg4_5Mb_200x`, as bench.py builds it) with seeded strands (each read reverse with probability 0.5), bench.py's
+single-GPU step, then K8 and the reverse pileup over its batch.
+
+    python tools/bench_strand.py [--steps K] [--warmup W]      # one JSON line on stdout
+
+The timed step is bench.py's.  On top of bench.py's fields the line carries:
+  `strand_ms`   K8 alone (kdl_select_count + kdl_select_scatter with the outputs allocated once), the reverse pileup
+                alone (K0 + K1 + K1e + K1g of the K8 sub-batch into a reused table) and K2 for scale, over the step's
+                batch and table, in 7 alternating rounds of 20 launches;
+  `e2e_vcf`     variants_vcf(path, strand=True) against variants_vcf(path) on a 10^6-read BAM with seeded strands,
+                best of 3, alternating;
+  `gpu`         the card's name and power limit, read in the same run;
+  `parity`      the reverse table's sha256 equals that of the pileup of the host bamio.select_reads sub-batch, and the
+                step's calls equal the C oracle's.
+Writes nothing into the tree."""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+import hashlib
+import json
+import os
+import sys
+import tempfile
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import bench  # noqa: E402
+from bench_fastq import alternate  # noqa: E402
+from bench_variants_ref import gpu_info  # noqa: E402
+
+WORKLOAD = "cfg4_5Mb_200x"
+STRAND_SEED = 10
+
+
+def e2e_vcf(rounds=3):
+    from kindel_b200 import kindel as K
+    from kindel_b200 import synth
+
+    sub = synth.with_strands(synth.simple_reads(4, [750_000], 200), STRAND_SEED)  # 10^6 reads, both strands
+    with tempfile.TemporaryDirectory() as tmp:
+        path = os.path.join(tmp, "slice.bam")
+        synth.write_simple_bam(path, sub)
+        K.variants_vcf(path, strand=True), K.variants_vcf(path)  # warm
+        best = {"strand": None, "sites_only": None}
+        for _ in range(rounds):
+            for key, fn in (("strand", lambda: K.variants_vcf(path, strand=True)),
+                            ("sites_only", lambda: K.variants_vcf(path))):
+                t0 = time.perf_counter()
+                text = fn()
+                dt = time.perf_counter() - t0
+                best[key] = dt if best[key] is None or dt < best[key] else best[key]
+                if key == "strand":
+                    n_rec = sum(1 for ln in text.splitlines() if not ln.startswith("#"))
+    return {"strand_s": best["strand"], "sites_only_s": best["sites_only"], "records": n_rec,
+            "reads": int(sub.n_reads), "reverse_reads": int(sub.reverse.sum()),
+            "note": "variants_vcf(path, strand=True) vs variants_vcf(path), best of %d, alternating" % rounds}
+
+
+def sha(t) -> str:
+    return hashlib.sha256(t.cpu().numpy().tobytes()).hexdigest()
+
+
+def main(argv=None) -> int:
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    args = ap.parse_args(argv)
+
+    import torch
+
+    from kindel_b200 import _ffi, bamio, engine, synth
+    from oracle import coracle
+
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    lib = _ffi.load()
+    gpu = gpu_info()
+    batch = synth.with_strands(bench.gen_reads(WORKLOAD), STRAND_SEED)
+    n_slots = batch.n_slots
+    db = engine.upload(batch, dev)
+    table = engine.CountTable(n_slots, dev)
+    calls_buf = torch.empty(n_slots, dtype=torch.uint8, device=dev)
+
+    def step(timers=None):
+        if timers:
+            timers[0].record()
+        engine.pileup(db, check=False, table=table)
+        if timers:
+            timers[1].record()
+        out = engine.vote(table.t, 1, out=calls_buf)
+        if timers:
+            timers[2].record()
+        return out
+
+    tm = bench.time_steps(step, args.steps, args.warmup, torch, None, 1, dev)
+    calls = tm["out"].cpu().numpy()
+
+    keep = torch.from_numpy(batch.reverse).to(dev)
+    sub = engine.select_reads(db, keep)
+    rev_fresh = engine.pileup(sub)[0]
+    scratch = torch.empty(int(lib.kdl_select_scratch_words(batch.n_reads)), dtype=torch.int32, device=dev)
+    st = int(torch.cuda.current_stream(dev).cuda_stream)
+
+    def k8():
+        base = (C.byref(db.struct), None, keep.data_ptr(), scratch.data_ptr())
+        lib.kdl_select_count(*base, st)
+        lib.kdl_select_scatter(*base, C.byref(sub.struct), None, st)
+
+    rev_table = engine.CountTable(n_slots, dev)
+    vote_buf = torch.empty(n_slots, dtype=torch.uint8, device=dev)
+    timing = alternate((("k2_vote", lambda: engine.vote(table.t, 1, out=vote_buf)), ("k8_select", k8),
+                        ("reverse_pileup", lambda: engine.pileup(sub, check=False, table=rev_table))), torch)
+    k8_again = engine.pileup(sub)[0]  # the sub-batch the timed K8 launches rewrote, piled again
+    host = sub.host
+    read_bytes = 4 * 3 * int(batch.n_reads) + batch.n_reads + 4 * host.n_words  # l_seq, seq_off, ref_start, keep, words
+    write_bytes = 4 * 3 * host.n_reads + 4 * host.n_words
+    timing.update(reads=int(batch.n_reads), reverse_reads=int(host.n_reads), reverse_complex=int(host.n_complex),
+                  k8_bytes_read=int(read_bytes), k8_bytes_written=int(write_bytes),
+                  note="k8_select: the two entry points over preallocated outputs, no read-back; reverse_pileup: "
+                       "engine.pileup of the K8 sub-batch into a reused CountTable, unchecked")
+    e2e = e2e_vcf()
+
+    want = bamio.select_reads(batch, np.flatnonzero(batch.reverse))
+    want_rev = engine.pileup(engine.upload(want, dev))[0]
+    parity_rev = sha(rev_fresh) == sha(want_rev) == sha(k8_again)
+    fields_equal = all(
+        (a is None and b is None) or (a is not None and b is not None and np.array_equal(np.asarray(a, np.int64),
+                                                                                      np.asarray(b, np.int64)))
+        for a, b in ((engine.download_fields(sub)[f], getattr(want, f)) for f in
+                     ("ref_start", "seq_off", "l_seq", "seq4", "contig_read_off", "complex_idx", "hard_idx")))
+    want_calls = coracle.vote(coracle.pileup(batch)[0], 1)
+    parity = bool(parity_rev and fields_equal and np.array_equal(calls, want_calls))
+    ms_per_step = tm["total_ms"] / tm["reps"]
+    line = {
+        "metric": bench.METRIC, "value": batch.aligned_bases / (ms_per_step * 1e-3), "unit": bench.UNIT, "n_gpus": 1,
+        "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True,
+        "dtype": "int32", "data": "synthetic", "steps_timed": tm["reps"], "step_ms": bench.quantiles(tm["step_ms"]),
+        "parity": parity, "parity_detail": {"reverse_table_sha256": sha(rev_fresh), "reverse_table": bool(parity_rev),
+                                            "k8_fields": bool(fields_equal)},
+        "config": {"workload": WORKLOAD, "reads_per_rank": int(batch.n_reads),
+                   "complex_reads_per_rank": int(batch.n_complex), "aligned_bases_total": int(batch.aligned_bases),
+                   "strand_seed": STRAND_SEED, "tool": "tools/bench_strand.py",
+                   "parity_oracle": "the pileup of bamio.select_reads' host sub-batch; the step's calls against "
+                                    "oracle/kindel_oracle.c"},
+        "gpu": gpu, "strand_ms": timing, "e2e_vcf": e2e, "e2e": None,
+    }
+    print(json.dumps(line))
+    return 0
+
+
+if __name__ == "__main__":
+    raise SystemExit(main())

@@ -50,6 +50,8 @@ def row(path: str, d: dict) -> str:
         work += ", + variant sites (K6)"
     if d.get("variant_ref_ms"):
         work += ", + variants against a reference (K6r, K7)"
+    if d.get("strand_ms"):
+        work += ", + strand split (K8, reverse pileup)"
     if d.get("map_ab"):
         work += ", zeroing A/B (dirty-sector map)"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
