@@ -26,6 +26,7 @@ inline int grid_for(long long items, int per_block, int cap) {
     return (int)g;
 }
 
+#ifndef KDL_HOST_EMU
 constexpr int kMaxDevices = 64;
 
 inline int current_device() {
@@ -59,6 +60,23 @@ inline int ensure_tile_smem() {
     return KDL_OK;
 }
 
+inline int check_launch() {
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaGetLastError() == cudaSuccess ? KDL_OK : KDL_ERR_CUDA;
+}
+#else
+// the kernel emulator (tests/emu/cuda_emu.h): the SM count it is set to, no shared-memory limit, its launch error
+inline int sm_count() { return emu::M().sm_count; }
+
+template <int kFlush, bool kCx>
+inline int ensure_tile_smem() { return KDL_OK; }
+
+inline int check_launch() {
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return emu::take_launch_error() ? KDL_ERR_CUDA : KDL_OK;
+}
+#endif
+
 template <int kFlush, bool kCx>
 inline int launch_tile(const kdl_batch& b, int32_t* counts, long long n_slots, long long tile_lo, long long n_tiles,
                        int split, int zero_rest, uint32_t* dirty_map, uint32_t map_after, cudaStream_t st) {
@@ -66,14 +84,10 @@ inline int launch_tile(const kdl_batch& b, int32_t* counts, long long n_slots, l
     if (rc != KDL_OK) return rc;
     const long long units = n_tiles * split, max_grid = (long long)sm_count() * 2;  // two CTAs per SM, persistent
     const long long grid = units < max_grid ? units : max_grid;
-    kdl::pileup_tile_kernel<kFlush, kCx><<<(unsigned)grid, kdl::W_THREADS, sizeof(kdl::TileSmem<kdl::TileCfg<kCx>>), st>>>(
-        b, counts, n_slots, b.tile_index, tile_lo, n_tiles, split, zero_rest, dirty_map, map_after);
+    KDL_LAUNCH((kdl::pileup_tile_kernel<kFlush, kCx>), (unsigned)grid, kdl::W_THREADS,
+               sizeof(kdl::TileSmem<kdl::TileCfg<kCx>>), st,
+               b, counts, n_slots, b.tile_index, tile_lo, n_tiles, split, zero_rest, dirty_map, map_after);
     return KDL_OK;
-}
-
-inline int check_launch() {
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError() == cudaSuccess ? KDL_OK : KDL_ERR_CUDA;
 }
 
 int validate_batch(const kdl_batch* b) {
@@ -164,8 +178,8 @@ int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slot
     uint32_t* mark_map = saturate ? nullptr : dirty_map;
     if (zero_pass) {
         uint32_t* zmap = saturate || (zero_from <= 5 && zero_to == KDL_NCOL) ? dirty_map : nullptr;
-        kdl::zero_cols_kernel<<<sm_count() * 4, 256, 0, st>>>(counts, n_slots, zero_from, zero_to, slot_lo, slot_hi,
-                                                              zmap, saturate ? ~0u : 0u);
+        KDL_LAUNCH(kdl::zero_cols_kernel, sm_count() * 4, 256, 0, st, counts, n_slots, zero_from, zero_to, slot_lo,
+                   slot_hi, zmap, saturate ? ~0u : 0u);
         if ((rc = check_launch()) != KDL_OK) return rc;
     }
     const uint32_t map_after = saturate && k1_stores ? ~0u : 0u;
@@ -173,8 +187,8 @@ int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slot
     if (tiled) {
         if (n_tiles > 0) {
             // K0: read range per tile of the slot range (the linear index of a sorted BAM, built on device)
-            kdl::tile_index_kernel<<<(unsigned)((n_tiles * 32 + 255) / 256), 256, 0, st>>>(*batch, tile_lo, n_tiles,
-                                                                                          batch->tile_index);
+            KDL_LAUNCH(kdl::tile_index_kernel, (unsigned)((n_tiles * 32 + 255) / 256), 256, 0, st, *batch, tile_lo,
+                       n_tiles, batch->tile_index);
             if ((rc = check_launch()) != KDL_OK) return rc;
             // K1: the tile-owner kernel.  Tile-eligible complex reads go through its piece machinery (kCx) when
             // they are a sizeable share of the batch; when they are rare (< 1/16 of the reads) the lean instantiation
@@ -197,30 +211,30 @@ int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slot
         }
         if (batch->n_complex > batch->n_hard) {  // K1e: insertions / deletions / clips of the tile-eligible complex reads
             if (cx_by_atomics)  // their bases too: 8 lanes per read
-                kdl::pileup_events_kernel<8><<<(unsigned)((batch->n_complex + 31) / 32), 256, 0, st>>>(
-                    *batch, counts, n_slots, ins_events, 1, mark_map);
+                KDL_LAUNCH(kdl::pileup_events_kernel<8>, (unsigned)((batch->n_complex + 31) / 32), 256, 0, st,
+                           *batch, counts, n_slots, ins_events, 1, mark_map);
             else                // a few scattered REDs per read: one thread per read
-                kdl::pileup_events_kernel<1><<<(unsigned)((batch->n_complex + 255) / 256), 256, 0, st>>>(
-                    *batch, counts, n_slots, ins_events, 0, mark_map);
+                KDL_LAUNCH(kdl::pileup_events_kernel<1>, (unsigned)((batch->n_complex + 255) / 256), 256, 0, st,
+                           *batch, counts, n_slots, ins_events, 0, mark_map);
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
         if (batch->n_hard > 0) {  // K1g: the reads that may wrap or raise, atomically, after the tile stores
             const int grid = grid_for(batch->n_hard, 8, cap);
-            kdl::pileup_general_kernel<<<grid, 256, 0, st>>>(*batch, batch->hard_idx, batch->n_hard, counts, n_slots,
-                                                            ins_events, err_flag, mark_map);
+            KDL_LAUNCH(kdl::pileup_general_kernel, grid, 256, 0, st, *batch, batch->hard_idx, batch->n_hard, counts,
+                       n_slots, ins_events, err_flag, mark_map);
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
     } else {
         // order-independent fallback (unsorted input): K1s for the simple reads, K1g for every complex read
         if (batch->n_reads > batch->n_complex) {
             const int grid = grid_for(batch->n_reads, 8, cap);  // 8 warps (reads) per 256-thread CTA
-            kdl::pileup_simple_atomic_kernel<<<grid, 256, 0, st>>>(*batch, counts, n_slots, err_flag);
+            KDL_LAUNCH(kdl::pileup_simple_atomic_kernel, grid, 256, 0, st, *batch, counts, n_slots, err_flag);
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
         if (batch->n_complex > 0) {
             const int grid = grid_for(batch->n_reads, 8, cap);
-            kdl::pileup_general_kernel<<<grid, 256, 0, st>>>(*batch, nullptr, batch->n_reads, counts, n_slots,
-                                                            ins_events, err_flag, mark_map);
+            KDL_LAUNCH(kdl::pileup_general_kernel, grid, 256, 0, st, *batch, nullptr, batch->n_reads, counts, n_slots,
+                       ins_events, err_flag, mark_map);
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
     }
@@ -235,7 +249,8 @@ int kdl_unmask(const kdl_batch* batch, const kdl_qmask* qmask, int32_t* counts, 
     if (qmask->n_reads == 0) return KDL_OK;
     if (!qmask->read_idx || !qmask->off || !qmask->qpos) return KDL_ERR_INVALID_ARG;
     const long long grid = (qmask->n_reads + kdl::kQThreads - 1) / kdl::kQThreads;
-    kdl::unmask_kernel<<<(unsigned)grid, kdl::kQThreads, 0, (cudaStream_t)stream>>>(*batch, *qmask, counts, n_slots);
+    KDL_LAUNCH(kdl::unmask_kernel, (unsigned)grid, kdl::kQThreads, 0, (cudaStream_t)stream, *batch, *qmask, counts,
+               n_slots);
     return check_launch();
 }
 
@@ -244,14 +259,14 @@ int kdl_diagnose(const kdl_batch* batch, kdl_diag* diag_dev, void* stream) {
     if (rc != KDL_OK) return rc;
     if (!diag_dev) return KDL_ERR_INVALID_ARG;
     cudaStream_t st = (cudaStream_t)stream;
-    kdl::diagnose_init_kernel<<<1, 1, 0, st>>>(diag_dev);
+    KDL_LAUNCH(kdl::diagnose_init_kernel, 1, 1, 0, st, diag_dev);
     if ((rc = check_launch()) != KDL_OK) return rc;
     if (batch->n_hard > 0) {
         const long long grid = (batch->n_hard + 255) / 256;
-        kdl::diagnose_kernel<<<(unsigned)grid, 256, 0, st>>>(*batch, diag_dev);
+        KDL_LAUNCH(kdl::diagnose_kernel, (unsigned)grid, 256, 0, st, *batch, diag_dev);
         if ((rc = check_launch()) != KDL_OK) return rc;
     }
-    kdl::diagnose_final_kernel<<<1, 1, 0, st>>>(diag_dev);
+    KDL_LAUNCH(kdl::diagnose_final_kernel, 1, 1, 0, st, diag_dev);
     return check_launch();
 }
 
@@ -262,8 +277,8 @@ int kdl_vote(const int32_t* counts, int64_t n_slots, int64_t min_depth_ceil, uin
     none.n = 0;
     const long long quads = n_slots / 4;
     const long long grid = (quads + 255) / 256;
-    kdl::vote_kernel<false><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(
-        counts, none, n_slots, 0, n_slots, min_depth_ceil, calls, nullptr, kdl::MajorityVote{});
+    KDL_LAUNCH(kdl::vote_kernel<false>, (unsigned)grid, 256, 0, (cudaStream_t)stream,
+               counts, none, n_slots, 0, n_slots, min_depth_ceil, calls, nullptr, kdl::MajorityVote{});
     return check_launch();
 }
 
@@ -276,15 +291,15 @@ int kdl_vote_iupac(const int32_t* counts, int64_t n_slots, int64_t min_depth_cei
     none.n = 0;
     const long long quads = n_slots / 4;
     const long long grid = (quads + 255) / 256;
-    kdl::vote_kernel<false, kdl::IupacVote><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(
-        counts, none, n_slots, 0, n_slots, min_depth_ceil, calls, nullptr, kdl::IupacVote{threshold});
+    KDL_LAUNCH((kdl::vote_kernel<false, kdl::IupacVote>), (unsigned)grid, 256, 0, (cudaStream_t)stream,
+               counts, none, n_slots, 0, n_slots, min_depth_ceil, calls, nullptr, kdl::IupacVote{threshold});
     return check_launch();
 }
 
 int kdl_derive(const int32_t* counts, int64_t n_slots, int32_t* out, void* stream) {
     if (!counts || !out || n_slots <= 0) return KDL_ERR_INVALID_ARG;
     const long long grid = (n_slots + 255) / 256;
-    kdl::derive_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(counts, n_slots, out);
+    KDL_LAUNCH(kdl::derive_kernel, (unsigned)grid, 256, 0, (cudaStream_t)stream, counts, n_slots, out);
     return check_launch();
 }
 
@@ -323,7 +338,7 @@ int kdl_exchange_signal(const kdl_exchange* x, int32_t epoch, void* stream) {
     kdl::Exchange e;
     int rc = make_exchange(x, &e, 0);
     if (rc != KDL_OK) return rc;
-    kdl::exchange_signal_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(e, epoch);
+    KDL_LAUNCH(kdl::exchange_signal_kernel, 1, 32, 0, (cudaStream_t)stream, e, epoch);
     return check_launch();
 }
 
@@ -332,7 +347,7 @@ int kdl_exchange_wait(const kdl_exchange* x, int32_t epoch, void* stream) {
     int rc = make_exchange(x, &e, 0);
     if (rc != KDL_OK) return rc;
     dim3 grid((unsigned)(sm_count() * 2 / x->n_ranks + 1), (unsigned)x->n_ranks);
-    kdl::exchange_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(e, epoch);
+    KDL_LAUNCH(kdl::exchange_gather_kernel, grid, 256, 0, (cudaStream_t)stream, e, epoch);
     return check_launch();
 }
 
@@ -349,8 +364,8 @@ int exchange_vote(const kdl_exchange* x, int64_t n_slots, int64_t min_depth_ceil
     const long long cap = (long long)sm_count() * 8;
     if (grid > cap) grid = cap;
     if (grid < 1) grid = 1;  // an empty slice still has to take part in the flag protocol
-    kdl::vote_exchange_kernel<Vote><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(e, n_slots, min_depth_ceil, epoch,
-                                                                                     vote);
+    KDL_LAUNCH(kdl::vote_exchange_kernel<Vote>, (unsigned)grid, 256, 0, (cudaStream_t)stream, e, n_slots,
+               min_depth_ceil, epoch, vote);
     return check_launch();
 }
 
@@ -371,8 +386,8 @@ int kdl_cdr_flags(const int32_t* counts, int64_t n_slots, int64_t slot_lo, int64
         return KDL_ERR_INVALID_ARG;
     if (slot_hi == slot_lo) return KDL_OK;
     const long long grid = (slot_hi - slot_lo + 255) / 256;
-    kdl::cdr_flags_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(counts, n_slots, slot_lo, slot_hi,
-                                                                            clip_decay_threshold, flags, bases);
+    KDL_LAUNCH(kdl::cdr_flags_kernel, (unsigned)grid, 256, 0, (cudaStream_t)stream, counts, n_slots, slot_lo, slot_hi,
+               clip_decay_threshold, flags, bases);
     return check_launch();
 }
 
@@ -392,18 +407,18 @@ int kdl_assemble(const uint8_t* calls, int64_t n_slots, const int64_t* contig_sl
     const long long n_blocks = (n_slots + 1 + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    kdl::assemble_sums_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, st>>>(a, block_sums);
+    KDL_LAUNCH(kdl::assemble_sums_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, st, a, block_sums);
     if ((rc = check_launch()) != KDL_OK) return rc;
-    kdl::assemble_scan_sums_kernel<<<1, kdl::A_THREADS, 0, st>>>(block_sums, n_blocks);
+    KDL_LAUNCH(kdl::assemble_scan_sums_kernel, 1, kdl::A_THREADS, 0, st, block_sums, n_blocks);
     if ((rc = check_launch()) != KDL_OK) return rc;
-    kdl::assemble_scatter_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, st>>>(a, block_sums, offsets, out);
+    KDL_LAUNCH(kdl::assemble_scatter_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, st, a, block_sums, offsets, out);
     return check_launch();
 }
 
 int kdl_consensus_qual(const int32_t* counts, const uint8_t* calls, int64_t n_slots, uint8_t* qual, void* stream) {
     if (!counts || !calls || !qual || n_slots <= 0 || (n_slots & 3)) return KDL_ERR_INVALID_ARG;
     const long long grid = (n_slots / 4 + 255) / 256;
-    kdl::consensus_qual_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(counts, calls, n_slots, qual);
+    KDL_LAUNCH(kdl::consensus_qual_kernel, (unsigned)grid, 256, 0, (cudaStream_t)stream, counts, calls, n_slots, qual);
     return check_launch();
 }
 
@@ -412,8 +427,8 @@ int kdl_assemble_qual(const uint32_t* offsets, const uint8_t* qual, int64_t n_sl
     if (!offsets || !qual || !out || n_slots <= 0 || n_ins < 0 || (n_ins > 0 && (!ins_slot || !ins_qual)))
         return KDL_ERR_INVALID_ARG;
     const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
-    kdl::assemble_qual_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
-        offsets, qual, n_slots, ins_slot, ins_qual, n_ins, out);
+    KDL_LAUNCH(kdl::assemble_qual_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream,
+               offsets, qual, n_slots, ins_slot, ins_qual, n_ins, out);
     return check_launch();
 }
 
@@ -442,9 +457,9 @@ int kdl_variant_count(const int32_t* counts, int64_t n_slots, const int64_t* con
     if (!block_sums) return KDL_ERR_INVALID_ARG;
     const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
     cudaStream_t st = (cudaStream_t)stream;
-    kdl::variant_sums_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, st>>>(a, block_sums);
+    KDL_LAUNCH(kdl::variant_sums_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, st, a, block_sums);
     if ((rc = check_launch()) != KDL_OK) return rc;
-    kdl::assemble_scan_sums_kernel<<<1, kdl::A_THREADS, 0, st>>>(block_sums, n_blocks);
+    KDL_LAUNCH(kdl::assemble_scan_sums_kernel, 1, kdl::A_THREADS, 0, st, block_sums, n_blocks);
     return check_launch();
 }
 
@@ -457,8 +472,8 @@ int kdl_variant_scatter(const int32_t* counts, int64_t n_slots, const int64_t* c
     if (!block_sums || n_sites < 0 || n_sites > n_slots || (n_sites > 0 && (!site_slot || !site_counts || !site_mask)))
         return KDL_ERR_INVALID_ARG;
     const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
-    kdl::variant_scatter_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
-        a, block_sums, n_sites, site_slot, site_counts, site_mask);
+    KDL_LAUNCH(kdl::variant_scatter_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream,
+               a, block_sums, n_sites, site_slot, site_counts, site_mask);
     return check_launch();
 }
 
@@ -484,9 +499,9 @@ int kdl_variant_ref_count(const int32_t* counts, int64_t n_slots, const int64_t*
     if (!block_sums) return KDL_ERR_INVALID_ARG;
     const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
     cudaStream_t st = (cudaStream_t)stream;
-    kdl::variant_ref_sums_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, st>>>(a, block_sums);
+    KDL_LAUNCH(kdl::variant_ref_sums_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, st, a, block_sums);
     if ((rc = check_launch()) != KDL_OK) return rc;
-    kdl::assemble_scan_sums_kernel<<<1, kdl::A_THREADS, 0, st>>>(block_sums, n_blocks);
+    KDL_LAUNCH(kdl::assemble_scan_sums_kernel, 1, kdl::A_THREADS, 0, st, block_sums, n_blocks);
     return check_launch();
 }
 
@@ -501,8 +516,8 @@ int kdl_variant_ref_scatter(const int32_t* counts, int64_t n_slots, const int64_
         (n_sites > 0 && (!site_slot || !site_counts || !site_dpa || !site_mask)))
         return KDL_ERR_INVALID_ARG;
     const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
-    kdl::variant_ref_scatter_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
-        a, block_sums, n_sites, site_slot, site_counts, site_dpa, site_mask);
+    KDL_LAUNCH(kdl::variant_ref_scatter_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream,
+               a, block_sums, n_sites, site_slot, site_counts, site_dpa, site_mask);
     return check_launch();
 }
 
@@ -517,10 +532,10 @@ int kdl_deletion_count(const kdl_batch* batch, uint32_t* block_sums, void* strea
     const long long n_blocks = (batch->n_reads + kdl::A_THREADS - 1) / kdl::A_THREADS;
     cudaStream_t st = (cudaStream_t)stream;
     if (n_blocks > 0) {
-        kdl::deletion_sums_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, st>>>(*batch, block_sums);
+        KDL_LAUNCH(kdl::deletion_sums_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, st, *batch, block_sums);
         if ((rc = check_launch()) != KDL_OK) return rc;
     }
-    kdl::assemble_scan_sums_kernel<<<1, kdl::A_THREADS, 0, st>>>(block_sums, n_blocks);
+    KDL_LAUNCH(kdl::assemble_scan_sums_kernel, 1, kdl::A_THREADS, 0, st, block_sums, n_blocks);
     return check_launch();
 }
 
@@ -531,8 +546,8 @@ int kdl_deletion_scatter(const kdl_batch* batch, const uint32_t* block_sums, int
     if (!block_sums || n_events < 0 || (n_events > 0 && (!ev_slot || !ev_len))) return KDL_ERR_INVALID_ARG;
     const long long n_blocks = (batch->n_reads + kdl::A_THREADS - 1) / kdl::A_THREADS;
     if (n_blocks == 0) return KDL_OK;
-    kdl::deletion_scatter_kernel<<<(unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream>>>(
-        *batch, block_sums, n_events, ev_slot, ev_len);
+    KDL_LAUNCH(kdl::deletion_scatter_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream,
+               *batch, block_sums, n_events, ev_slot, ev_len);
     return check_launch();
 }
 
@@ -560,9 +575,9 @@ int kdl_select_count(const kdl_batch* batch, const kdl_qmask* qmask, const uint8
     if (!scratch || (batch->n_reads > 0 && !keep) || batch->n_reads >= (int64_t)UINT32_MAX) return KDL_ERR_INVALID_ARG;
     const long long n_blocks = select_blocks(batch->n_reads);
     cudaStream_t st = (cudaStream_t)stream;
-    kdl::select_sums_kernel<<<(unsigned)n_blocks, kdl::S_THREADS, 0, st>>>(*batch, q, keep, scratch);
+    KDL_LAUNCH(kdl::select_sums_kernel, (unsigned)n_blocks, kdl::S_THREADS, 0, st, *batch, q, keep, scratch);
     if ((rc = check_launch()) != KDL_OK) return rc;
-    kdl::select_combine_kernel<<<1, kdl::S_THREADS, 0, st>>>(scratch, n_blocks);
+    KDL_LAUNCH(kdl::select_combine_kernel, 1, kdl::S_THREADS, 0, st, scratch, n_blocks);
     return check_launch();
 }
 
@@ -578,11 +593,12 @@ int kdl_select_scatter(const kdl_batch* batch, const kdl_qmask* qmask, const uin
         (out->n_reads > 0 && out->seq4_words > 0 && !out->seq4))
         return KDL_ERR_INVALID_ARG;
     const long long n_blocks = select_blocks(batch->n_reads);
-    kdl::select_scatter_kernel<<<(unsigned)n_blocks, kdl::S_THREADS, 0, (cudaStream_t)stream>>>(
-        *batch, q, keep, scratch, *out, const_cast<int64_t*>(out->contig_read_off), om);
+    KDL_LAUNCH(kdl::select_scatter_kernel, (unsigned)n_blocks, kdl::S_THREADS, 0, (cudaStream_t)stream,
+               *batch, q, keep, scratch, *out, const_cast<int64_t*>(out->contig_read_off), om);
     return check_launch();
 }
 
+#ifndef KDL_HOST_EMU  // device memory and IPC handles: nothing the kernel emulator can stand in for
 int kdl_table_alloc(int64_t bytes, void** dev_ptr) {
     if (!dev_ptr || bytes <= 0) return KDL_ERR_INVALID_ARG;
     *dev_ptr = nullptr;
@@ -606,6 +622,7 @@ int kdl_ipc_open(const uint8_t handle[64], void** dev_ptr) {
     return cudaIpcOpenMemHandle(dev_ptr, h, cudaIpcMemLazyEnablePeerAccess) == cudaSuccess ? KDL_OK : KDL_ERR_CUDA;
 }
 int kdl_ipc_close(void* dev_ptr) { return cudaIpcCloseMemHandle(dev_ptr) == cudaSuccess ? KDL_OK : KDL_ERR_CUDA; }
+#endif
 
 int kdl_vote_peers_sparse(const int32_t* const* peer_counts, const int64_t* foot_lo, const int64_t* foot_hi,
                           int32_t n_peers, int64_t n_slots, int64_t slot_lo, int64_t slot_hi,
@@ -625,11 +642,13 @@ int kdl_vote_peers_sparse(const int32_t* const* peer_counts, const int64_t* foot
     }
     const long long quads = (slot_hi - slot_lo) / 4;
     const long long grid = (quads + 255) / 256;
-    kdl::vote_kernel<true><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(
-        nullptr, peers, n_slots, slot_lo, slot_hi, min_depth_ceil, calls, reduced, kdl::MajorityVote{});
+    KDL_LAUNCH(kdl::vote_kernel<true>, (unsigned)grid, 256, 0, (cudaStream_t)stream,
+               nullptr, peers, n_slots, slot_lo, slot_hi, min_depth_ceil, calls, reduced, kdl::MajorityVote{});
     return check_launch();
 }
 
 }  // extern "C"
 
+#ifndef KDL_HOST_EMU
 #include "host_ctx.inl"
+#endif

@@ -13,6 +13,16 @@
 #define KDL_DYNAMIC_SMEM(name) extern unsigned char name[]
 #endif
 
+// Every kernel launch of api.cu.  Under KDL_HOST_EMU the emulator runs the grid on the host, row by row of a
+// two-dimensional grid, and keeps a failure for check_launch() as the runtime keeps a launch error.  A kernel name
+// with a comma in its template arguments goes in parentheses.
+#ifndef KDL_HOST_EMU
+#define KDL_LAUNCH(kernel, grid, block, smem, stream, ...) kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#else
+#define KDL_LAUNCH(kernel, grid, block, smem, stream, ...) \
+    emu::launch_grid(dim3(grid), dim3(block), [&] { kernel(__VA_ARGS__); })
+#endif
+
 namespace kdl {
 
 // BAM nibble ("=ACMGRSVTWYHKDBN") -> weight column 0..4 (A,C,G,T,N) or -1.  Only the five keys

@@ -1,9 +1,9 @@
 // cuda_emu.h -- TEST INFRASTRUCTURE: a functional emulator of the CUDA execution model for the host.
 //
-// Purpose: run the SOURCE TEXT of the tile-owner kernels (kindel_b200/csrc/pileup_tiled.cu, pileup_wide.cu, pileup_ws.cu)
-// on the CPU, so that indexing, sentinels, flush conditions, warp collectives and the staging protocol of a
-// kernel can be checked against the oracle without a GPU.  It models behaviour, not performance, and only the
-// constructs those kernels use:
+// Purpose: run the SOURCE TEXT of the kernels and of the C ABI that launches them (kindel_b200/csrc/api.cu, through
+// KDL_LAUNCH; tests/emu/emu_api.cpp) on the CPU, so that indexing, sentinels, flush conditions, warp collectives, the
+// staging protocol of a kernel and the launch decisions can be checked against the oracle without a GPU.  It models
+// behaviour, not performance, and only the constructs those kernels use:
 //
 //   * one fibre (ucontext) per CUDA thread, blocks run one after another; fibres switch only at
 //     __syncthreads / __syncwarp / warp collectives / mbarrier waits, round-robin in thread order;
@@ -78,6 +78,9 @@ struct Machine {
     std::vector<int> order;
     int schedule = 0;            // 0: threads in order each round, 1: reverse order, 2: a fresh random order per round
     uint64_t rng = 0x9E3779B97F4A7C15ull;
+    int sm_count = 2;            // what api.cu's sm_count() returns: small, so that grid-stride loops stride
+    char launch_error[256] = {0};  // the first failure since check_launch() last looked (launch_grid)
+    char last_error[256] = {0};    // the failure check_launch() last reported
 };
 
 inline Machine& M() {
@@ -266,6 +269,28 @@ inline const char* launch(unsigned grid, unsigned block, const std::function<voi
 inline const char* launch_y(unsigned grid, unsigned block_y, unsigned grid_y, unsigned block,
                             const std::function<void()>& body) {
     return launch(grid, block, body, block_y, grid_y);
+}
+
+// a launch <<<grid, block>>> as KDL_LAUNCH makes it: the rows of a two-dimensional grid one after another; a failure
+// is kept until take_launch_error() reads it, as the runtime keeps a launch error for cudaGetLastError
+inline void launch_grid(dim3 grid, dim3 block, const std::function<void()>& body) {
+    Machine& m = M();
+    for (unsigned y = 0; y < grid.y; ++y) {
+        const char* err = launch_y(grid.x, y, grid.y, block.x, body);
+        if (err) {
+            if (!m.launch_error[0]) snprintf(m.launch_error, sizeof m.launch_error, "%s", err);
+            return;
+        }
+    }
+}
+
+// true if a launch failed since the last call; its text moves to last_error
+inline bool take_launch_error() {
+    Machine& m = M();
+    if (!m.launch_error[0]) return false;
+    memcpy(m.last_error, m.launch_error, sizeof m.last_error);
+    m.launch_error[0] = 0;
+    return true;
 }
 
 }  // namespace emu

@@ -70,3 +70,32 @@ def parse(lines):
         info = dict(kv.split("=") if "=" in kv else (kv, True) for kv in f[7].split(";"))
         out[(int(f[1]), f[3], f[4])] = (f[6], info)
     return out
+
+
+# ---- K8 results against bamio.select_reads, field for field ----------------------------------------------------
+_ARRAYS = ("ref_start", "seq_off", "l_seq", "seq4", "contig_read_off", "complex_idx", "hard_idx")
+_SCALARS = ("n_events", "reads_sorted", "max_simple_len", "reach_right", "reach_left")
+_MASK = ("mask_read", "mask_off", "mask_qpos")
+
+
+def fields(batch) -> dict:
+    """The fields K8 produces, of a host ReadBatch (what select_reads gives)."""
+    out = {f: np.asarray(getattr(batch, f)) for f in _ARRAYS}
+    out.update({f: getattr(batch, f) for f in _SCALARS})
+    out.update({f: (np.asarray(getattr(batch, f)) if batch.n_masked else None) for f in _MASK})
+    return out
+
+
+def assert_equal(got: dict, want: dict, what=""):
+    for f in _ARRAYS:
+        g, w = np.asarray(got[f]), np.asarray(want[f])
+        assert g.shape == w.shape and np.array_equal(g.view(np.uint8) if g.size else g,
+                                                     w.astype(g.dtype).view(np.uint8) if w.size else w.astype(g.dtype)), (what, f)
+    for f in _SCALARS:
+        assert int(got[f]) == int(want[f]), (what, f, got[f], want[f])
+    for f in _MASK:
+        if want[f] is None:
+            assert got[f] is None, (what, f)
+        else:
+            assert got[f] is not None and np.array_equal(np.asarray(got[f], dtype=np.int64),
+                                                         np.asarray(want[f], dtype=np.int64)), (what, f)

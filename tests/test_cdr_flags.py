@@ -5,11 +5,11 @@ equal to `tot * decay`, and slot ranges that are not multiples of the block size
 import numpy as np
 import pytest
 
-import emu_iupac_harness as EI
+import emu_harness as E
 from kindel_b200 import kindel as K
 from kindel_b200.views import BaseCounts
 
-pytestmark = pytest.mark.skipif(not EI.available(), reason="needs g++ and the CUDA headers")
+pytestmark = pytest.mark.skipif(not E.available(), reason="needs g++ and the CUDA headers")
 
 DECAYS = (0.0, 0.1, 0.5, 1.0, 0.3, 0.9)
 BIG = (1 << 31) - 1
@@ -89,7 +89,7 @@ def test_k4_emulated_equals_host_predicates(decay):
     for seed, (n, lo, hi) in enumerate(((1000, 0, 1000), (777, 3, 770), (2048, 255, 1793), (300, 1, 2))):
         t = adversarial_table(seed + int(decay * 100), n, decay)
         want_f, want_b = host_predicates(t, lo, hi, decay)
-        got_f, got_b = EI.cdr_flags(t, lo, hi, decay)
+        got_f, got_b = E.cdr_flags(t, lo, hi, decay)
         bad = np.flatnonzero((got_f != want_f) | (got_b != want_b))
         assert not bad.size, (decay, seed, lo + bad[:5], t[:, lo + bad[:1]].ravel().tolist(), got_f[bad[:3]],
                               want_f[bad[:3]])

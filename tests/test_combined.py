@@ -14,9 +14,6 @@ import torch
 
 import combo_cases as CC
 import emu_harness as E
-import emu_iupac_harness as EI
-import emu_mask_harness as EM
-import emu_qual_harness as EQ
 import helpers as H
 from kindel_b200 import bamio
 from kindel_b200 import kindel as K
@@ -39,7 +36,7 @@ def corpus(tmp_path_factory):
 
 def _emulated_k2q(run, calls_all):
     """K2q from its CUDA source over the host tables (stands in for the device copy of _slot_qualities)."""
-    return torch.from_numpy(EQ.consensus_qual(run.host_counts, calls_all))
+    return torch.from_numpy(E.consensus_qual(run.host_counts, calls_all))
 
 
 def _host_result(path, piled, t, md, realign, trim, upper, filters):
@@ -143,7 +140,7 @@ def test_record_filters_equal_rewriting_as_unmapped(corpus, monkeypatch, tmp_pat
             batch = bamio.read_alignment(p, min_mapq=filters[1], exclude_flags=filters[2], min_base_quality=bq)
             counts, events = _emulated_pileup(batch)
             run = K.PileupRun.from_host_tables(batch, counts, E.derive(counts), events)
-            results.append(K.consensus_from_run(run, EI.vote_iupac(counts, 3, 0.6), p, True, 3, filters=filters,
+            results.append(K.consensus_from_run(run, E.vote_iupac(counts, 3, 0.6), p, True, 3, filters=filters,
                                                 iupac_threshold=0.6, qualities=True))
         a, b_ = results
         assert [(r.sequence, r.qualities) for r in a.consensuses] == [(r.sequence, r.qualities) for r in b_.consensuses]
@@ -154,7 +151,7 @@ def test_record_filters_equal_rewriting_as_unmapped(corpus, monkeypatch, tmp_pat
 
 def _emulated_pileup(batch):
     counts, events = E.pileup_pipeline(batch)
-    return EM.unmask(batch, counts), events
+    return E.unmask(batch, counts), events
 
 
 @needs_emu
@@ -172,8 +169,8 @@ def test_emulated_device_chain_equals_composed_oracle(corpus):
             piled = CC.Piled(contigs, recs, d / "oracle.bam", bq, mq, ex)
             np.testing.assert_array_equal(counts, piled.counts)
             np.testing.assert_array_equal(events, piled.events)
-            calls = E.vote(counts, md) if t is None else EI.vote_iupac(counts, md, t)
-            qual = EQ.consensus_qual(counts, calls)
+            calls = E.vote(counts, md) if t is None else E.vote_iupac(counts, md, t)
+            qual = E.consensus_qual(counts, calls)
             run = K.PileupRun.from_host_tables(masked, counts, E.derive(counts), events)
             slots = K._insertion_slots(masked, calls)
             iq = K._insertion_qualities(run, slots)
@@ -181,7 +178,7 @@ def test_emulated_device_chain_equals_composed_oracle(corpus):
             for sl in slots.tolist():
                 text, tie = run.ins_table.consensus_at(sl)
                 strings.append("N" if tie else text.lower())
-            texts, quals = EQ.assemble_qual(calls, qual, masked, slots, strings, [iq[s] for s in slots.tolist()])
+            texts, quals = E.assemble_qual(calls, qual, masked, slots, strings, [iq[s] for s in slots.tolist()])
             for trim, upper in ((False, False), (True, True)):
                 want = piled.consensus(t, md, trim_ends=trim, uppercase=upper)
                 for c, (name, seq, _, q) in enumerate(want):

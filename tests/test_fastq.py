@@ -5,7 +5,7 @@ There is no reference to pin them against, so two restatements written in differ
 other: oracle/kindel_fqoracle.c (`fqoracle`: a linear search over q per slot, then a sequential walk over the
 positions writing text and qualities side by side) and oracle/py_fqoracle.py (numpy: all 61 q at once per slot).  The
 host assembly of the product (kindel.assemble_consensus with qualities) must reproduce the C walk, and K2q / K5q run
-from their CUDA source under the host emulator (tests/emu/emu_qual.cpp) and must reproduce the C oracle."""
+from their CUDA source under the host emulator (tests/emu/emu_api.cpp) and must reproduce the C oracle."""
 import math
 import os
 import re
@@ -14,7 +14,7 @@ from decimal import Decimal, getcontext
 import numpy as np
 import pytest
 
-import emu_qual_harness as EQ
+import emu_harness as E
 import helpers as H
 from kindel_b200 import _ffi, cli, quality
 from kindel_b200 import kindel as K
@@ -22,7 +22,7 @@ from oracle import coracle, fqoracle, ioracle, py_fqoracle
 from oracle.py_oracle import base_call
 from test_iupac import MIN_DEPTHS, _adversarial, _contigs, _piled, _table
 
-needs_emu = pytest.mark.skipif(not EQ.available(), reason="needs g++ and the CUDA headers")
+needs_emu = pytest.mark.skipif(not E.available(), reason="needs g++ and the CUDA headers")
 THRESHOLDS = (0.0, 0.6, 0.99)
 WORKED = [  # (D, k, Q) of the definition, two of them exact equalities of the product and the bound
     (8, 8, 10), (98, 98, 20), (1, 1, 4), (10, 10, 10), (100, 100, 20), (1000, 1000, 30), (100, 90, 9), (30, 29, 12),
@@ -75,8 +75,8 @@ def test_worked_values():
     want = np.array([q for _, _, q in WORKED] + [20], dtype=np.uint8)
     assert np.array_equal(fqoracle.qual(tab, calls)[:11], want)
     assert np.array_equal(py_fqoracle.qual(tab, calls)[:11], want)
-    if EQ.available():
-        assert np.array_equal(EQ.consensus_qual(tab, calls)[:11], want)
+    if E.available():
+        assert np.array_equal(E.consensus_qual(tab, calls)[:11], want)
 
 
 def _boundary_tables():
@@ -112,8 +112,8 @@ def test_boundaries():
         assert got[s] == quality.phred(int(w[:, s].sum()), k), s
     assert got[6] == quality.phred(4 * ((1 << 31) - 1), (1 << 31) - 1) > 0  # D near 2^33
     assert got[12] == 10 and got[13] == 20
-    if EQ.available():
-        assert np.array_equal(EQ.consensus_qual(tab, full), got)
+    if E.available():
+        assert np.array_equal(E.consensus_qual(tab, full), got)
 
 
 def test_insertion_rule():
@@ -222,7 +222,7 @@ def test_emulated_k2q_equals_oracle(schedule, seed, tmp_path):
     from fuzz_cases import random_case
     from kindel_b200 import bamio
 
-    EQ.set_schedule(schedule, seed)
+    E.set_schedule(schedule, seed)
     try:
         tables = _adversarial(seed + 21) + [_boundary_tables()[0]]
         for s in range(0, 400, 16):
@@ -235,10 +235,10 @@ def test_emulated_k2q_equals_oracle(schedule, seed, tmp_path):
         for tab in tables:
             for md in (0, 7):
                 for vote, calls in _votes(tab, md):
-                    np.testing.assert_array_equal(EQ.consensus_qual(tab, calls), fqoracle.qual(tab, calls),
+                    np.testing.assert_array_equal(E.consensus_qual(tab, calls), fqoracle.qual(tab, calls),
                                                   err_msg="%s %s md=%d" % (schedule, vote, md))
     finally:
-        EQ.set_schedule("forward")
+        E.set_schedule("forward")
 
 
 @needs_emu
@@ -246,7 +246,7 @@ def test_emulated_k2q_equals_oracle(schedule, seed, tmp_path):
 def test_emulated_k5q_equals_oracle(schedule, seed, manifest, tmp_path):
     """K5 then K5q from their source: every contig's text and qualities equal the C walk -- insertion slots, 'D' calls,
     contig ends and multi-contig slot spaces included."""
-    EQ.set_schedule(schedule, seed)
+    E.set_schedule(schedule, seed)
     n_ins = n_del = n_multi = 0
     try:
         for k, (name, batch, counts, events) in enumerate(_piled(manifest, tmp_path)):
@@ -266,13 +266,13 @@ def test_emulated_k5q_equals_oracle(schedule, seed, manifest, tmp_path):
                     text, tie = run.ins_table.consensus_at(sl)
                     strings.append("N" if tie else text.lower())
                     iq.append(allq[sl])
-                texts, quals = EQ.assemble_qual(calls, qual, batch, slots, strings, iq)
+                texts, quals = E.assemble_qual(calls, qual, batch, slots, strings, iq)
                 n_ins += len(strings)
                 n_del += int(np.count_nonzero(((calls >> 4) & 3) == 1))
                 for c, (s0, L, ins_c) in enumerate(contigs):
                     assert (texts[c], quals[c]) == fqoracle.fastq(counts, calls, s0, L, ins_c), (name, vote, c)
     finally:
-        EQ.set_schedule("forward")
+        E.set_schedule("forward")
     assert n_ins > 50 and n_del > 50 and n_multi >= 1
 
 

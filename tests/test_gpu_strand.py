@@ -7,7 +7,6 @@ import sys
 import numpy as np
 import pytest
 
-import emu_select_harness as ES
 import helpers as H
 import strand_cases as S
 from kindel_b200 import bamio, engine, synth
@@ -41,7 +40,7 @@ def _check_select(batch, db, seed, what):
         keep = np.ascontiguousarray(keep, dtype=np.uint8)
         sub = engine.select_reads(db, torch.from_numpy(keep))
         want = bamio.select_reads(batch, np.flatnonzero(keep))
-        ES.assert_equal(engine.download_fields(sub), ES.fields(want), (what, j))
+        S.assert_equal(engine.download_fields(sub), S.fields(want), (what, j))
         got_t, got_e = engine.pileup(sub)
         want_t, want_e = engine.pileup(engine.upload(want))
         assert np.array_equal(got_t.cpu().numpy(), want_t.cpu().numpy()), (what, j)

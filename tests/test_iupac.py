@@ -11,7 +11,6 @@ import numpy as np
 import pytest
 
 import emu_harness as E
-import emu_iupac_harness as EI
 import helpers as H
 from clip_cases import clip_case
 from conftest import golden_input
@@ -146,7 +145,7 @@ def test_worked_examples():
         assert _letter(got) == want, (a, c, g, t_, n, thr)
         assert py_ioracle.iupac_call({"A": a, "C": c, "G": g, "T": t_, "N": n}, thr) == want
         if E.available():
-            assert _letter(EI.vote_iupac(tab, 1, thr)[0]) == want
+            assert _letter(E.vote_iupac(tab, 1, thr)[0]) == want
 
 
 # ------------------------------------------------------------------------------------------ kernels
@@ -171,7 +170,7 @@ def _adversarial(seed):
 @needs_emu
 @pytest.mark.parametrize("schedule,seed", [("forward", 0), ("reverse", 0), ("random", 1)])
 def test_emulated_k2_iupac_equals_oracle(schedule, seed, tmp_path):
-    EI.set_schedule(schedule, seed)
+    E.set_schedule(schedule, seed)
     try:
         tables = _adversarial(seed + 11)
         for s in range(0, 400, 8):
@@ -184,10 +183,10 @@ def test_emulated_k2_iupac_equals_oracle(schedule, seed, tmp_path):
         for tab in tables:
             for md in MIN_DEPTHS:
                 for t in THRESHOLDS:
-                    np.testing.assert_array_equal(EI.vote_iupac(tab, md, t), ioracle.vote_iupac(tab, md, t),
+                    np.testing.assert_array_equal(E.vote_iupac(tab, md, t), ioracle.vote_iupac(tab, md, t),
                                                   err_msg="%s md=%d t=%s" % (schedule, md, t))
     finally:
-        EI.set_schedule("forward")
+        E.set_schedule("forward")
 
 
 @needs_emu
@@ -209,7 +208,7 @@ def test_emulated_exchange_iupac_equals_one_table(world):
         if bufs is None:
             bufs = [[np.full(n_slots, 0xEE, dtype=np.uint8) for _ in range(world)] for _ in range(2)]
         calls = bufs[epoch & 1]
-        EI.exchange_epoch(tables, feet, slices, calls, flags, epoch, t, min_depth=2)
+        E.exchange_epoch_iupac(tables, feet, slices, calls, flags, epoch, t, min_depth=2)
         want = ioracle.vote_iupac(full, 2, t)
         assert (want & 0x80).any()
         for r in range(world):
@@ -238,7 +237,7 @@ def test_emulated_k5_on_iupac_calls_equals_host_assembly(manifest, tmp_path):
         for t in (0.0, 0.7, 1.0):
             calls = ioracle.vote_iupac(counts, 1, t)
             n_mixed += int(np.count_nonzero(calls & 0x80))
-            got = EI.assemble(calls, batch, *_insertion_strings(run, calls))
+            got = E.assemble(calls, batch, *_insertion_strings(run, calls))
             for c in range(batch.n_contigs):
                 s, e = run.contig_slice(c)
                 want, _ = K.assemble_consensus(calls[s:e - 1], lambda p, s=s: run.ins_table.consensus_at(s + p))

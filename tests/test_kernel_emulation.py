@@ -30,23 +30,26 @@ CASES = {
 
 @pytest.mark.parametrize("cx", [False, True], ids=["lean", "cx"])
 @pytest.mark.parametrize("name", list(CASES))
-def test_tile_owner_kernel_source_equals_oracle(name, cx):
-    """Simple reads through both instantiations of K1 (the kCx one has smaller stages and the piece machinery)."""
+def test_tile_owner_kernel_source_equals_oracle(name, cx, monkeypatch):
+    """Simple reads through both instantiations of K1 (the kCx one has smaller stages and the piece machinery; no entry
+    point runs it on simple reads alone, so it is launched directly)."""
     batch = CASES[name]()
     want, _ = coracle.pileup(batch)
-    for mode in (E.F_ADD, E.F_STORE):
-        got = E.run_pileup(batch, mode, cx=cx)
-        np.testing.assert_array_equal(got[:5], want[:5], err_msg="%s mode=%s" % (name, mode))
+    monkeypatch.setenv("KDL_SPLIT", "1")
+    for fresh in (False, True):
+        got = E.tile_cx_pileup(batch, fresh) if cx else E.run_pileup(batch, fresh)
+        np.testing.assert_array_equal(got[:5], want[:5], err_msg="%s fresh=%s" % (name, fresh))
         assert not got[5:].any()
 
 
 @pytest.mark.parametrize("split", [2, 5])
 @pytest.mark.parametrize("name", ["deep", "cfg4_like", "multi_contig", "sparse"])
-def test_depth_split_units_share_a_tile(name, split):
+def test_depth_split_units_share_a_tile(name, split, monkeypatch):
     """`split` CTAs per tile, each a contiguous part of the tile's reads, flushing with REDs into a zeroed table."""
     batch = CASES[name]()
     want, _ = coracle.pileup(batch)
-    got = E.run_pileup(batch, E.F_ATOMIC, split=split, grid=7)
+    monkeypatch.setenv("KDL_SPLIT", str(split))
+    got = E.run_pileup(batch, fresh=False, sm_count=3)
     np.testing.assert_array_equal(got[:5], want[:5])
     assert not got[5:].any()
 
@@ -59,51 +62,54 @@ CX_CASES = {
 
 
 @pytest.mark.parametrize("name", list(CX_CASES) + ["mixed"])
-def test_rare_complex_reads_by_atomics(name):
+def test_rare_complex_reads_by_atomics(name, monkeypatch):
     """The other way kdl_pileup_range handles tile-eligible complex reads (when they are rare): the lean K1 treats them
-    as inert and K1e counts their M/=/X bases too, with REDs behind the tile stores."""
+    as inert and K1e counts their M/=/X bases too, with REDs behind the tile stores (and K1g the hard reads)."""
     batch = synth.mixed_reads(93, [9000, 4000], 80, 0.05) if name == "mixed" else CX_CASES[name]()
     want_c, want_e = coracle.pileup(batch)
-    hard = D.select_reads(batch, batch.hard_idx)
-    wh = coracle.pileup(hard)[0] if batch.n_hard else 0
-    for mode in (E.F_ADD, E.F_STORE):
-        got, ev = E.run_pileup(batch, mode, cx=False, want_events=True, zero_rest=mode == E.F_STORE)
-        np.testing.assert_array_equal(got, want_c - wh)
+    monkeypatch.setenv("KDL_CX", "atomics")
+    monkeypatch.setenv("KDL_SPLIT", "1")
+    for fresh in (False, True):
+        got, ev = E.run_pileup(batch, fresh, want_events=True, zero_rest=fresh)
+        np.testing.assert_array_equal(got, want_c)
+        np.testing.assert_array_equal(ev, want_e)
 
 
 @pytest.mark.parametrize("split", [1, 3])
 @pytest.mark.parametrize("name", list(CX_CASES))
-def test_complex_reads_in_the_tile_kernel(name, split):
+def test_complex_reads_in_the_tile_kernel(name, split, monkeypatch):
     """Tile-eligible complex reads: M segments as masked pieces through the bit-sliced counters, I / D / clip
     updates and insertion events from the producers; hard reads (K1g) on top."""
     batch = CX_CASES[name]()
     assert batch.n_complex > batch.n_hard
     want_c, want_e = coracle.pileup(batch)
-    got_c, got_e = E.pileup_pipeline(batch, split=split)
+    monkeypatch.setenv("KDL_CX", "pieces")
+    monkeypatch.setenv("KDL_SPLIT", str(split))
+    got_c, got_e = E.pileup_pipeline(batch)
     np.testing.assert_array_equal(got_c, want_c)
     np.testing.assert_array_equal(got_e, want_e)
-    if split == 1:  # stale columns are overwritten / zeroed in the flush, K1 + K1e = everything but the hard reads
-        got2, ev2 = E.run_pileup(batch, E.F_STORE, want_events=True, zero_rest=True)
-        hard = __import__("kindel_b200.distributed", fromlist=["x"]).select_reads(batch, batch.hard_idx)
-        wh, _ = coracle.pileup(hard)
-        np.testing.assert_array_equal(got2, want_c - wh)
+    if split == 1:  # stale columns are overwritten / zeroed in K1's flush before K1e and K1g add to them
+        got2, ev2 = E.run_pileup(batch, want_events=True, zero_rest=True)
+        np.testing.assert_array_equal(got2, want_c)
+        np.testing.assert_array_equal(ev2, want_e)
 
 
-@pytest.mark.parametrize("mode", [E.F_ADD, E.F_STORE], ids=["add", "store"])
-def test_accumulate_and_slot_ranges(mode):
+@pytest.mark.parametrize("fresh", [False, True], ids=["add", "store"])
+def test_accumulate_and_slot_ranges(fresh, monkeypatch):
     """Two batches added into one table (accumulate mode), then a fresh pass over a tile sub-range only."""
     a = synth.simple_reads(81, [20_000], 30)
     b = synth.simple_reads(81, [20_000], 50, read_seed=9)
     wa, _ = coracle.pileup(a)
     wb, _ = coracle.pileup(b)
-    t = E.run_pileup(a, E.F_ADD)
-    t = E.run_pileup(b, E.F_ADD, counts=t)
+    monkeypatch.setenv("KDL_SPLIT", "1")
+    t = E.run_pileup(a, fresh=False)
+    t = E.run_pileup(b, fresh=False, counts=t)
     np.testing.assert_array_equal(t[:5], (wa + wb)[:5])
     # overwrite (F_STORE) / add (F_ADD) on tiles [7, 19) with batch a: outside the range untouched
     lo, n = 7, 12
-    t2 = E.run_pileup(a, mode, tile_lo=lo, n_tiles=n, counts=t.copy())
     s0, s1 = lo * 512, (lo + n) * 512
-    inside = wa[:5, s0:s1] if mode == E.F_STORE else (t + wa)[:5, s0:s1]
+    t2 = E.run_pileup(a, fresh, slot_range=(s0, s1), counts=t.copy())
+    inside = wa[:5, s0:s1] if fresh else (t + wa)[:5, s0:s1]
     np.testing.assert_array_equal(t2[:5, s0:s1], inside)
     np.testing.assert_array_equal(t2[:5, :s0], t[:5, :s0])
     np.testing.assert_array_equal(t2[:5, s1:], t[:5, s1:])
@@ -240,15 +246,16 @@ def test_fused_exchange_epochs(world, cut):
 
 
 @pytest.mark.parametrize("schedule,seed", [("reverse", 0), ("random", 1), ("random", 2)])
-def test_other_thread_interleavings(schedule, seed):
+def test_other_thread_interleavings(schedule, seed, monkeypatch):
     """The staging protocol (full / landed / empty mbarrier ring, producer barrier, cp.async prefetch, the piece
     queue of the consumers) under other thread orders than the emulator's default."""
     E.set_schedule(schedule, seed)
+    monkeypatch.setenv("KDL_SPLIT", "1")
     try:
         for name in ("shallow", "multi_contig", "long_reads"):
             batch = CASES[name]()
             want, _ = coracle.pileup(batch)
-            got = E.run_pileup(batch, E.F_STORE, grid=4)
+            got = E.run_pileup(batch)
             np.testing.assert_array_equal(got[:5], want[:5], err_msg="%s %s/%d" % (name, schedule, seed))
         batch = CX_CASES["cfg3_like"]()
         want_c, want_e = coracle.pileup(batch)

@@ -14,7 +14,6 @@ import numpy as np
 import pytest
 
 import emu_harness as E
-import emu_mask_harness
 import limit_cases as LC
 from conftest import GOLDEN, ROOT
 from kindel_b200 import _ffi, bamio
@@ -217,23 +216,31 @@ def _hard_table(batch):
 @emu
 @pytest.mark.parametrize("cx", [False, True], ids=["lean", "cx"])
 @pytest.mark.parametrize("name", GROUPS)
-def test_limit_tile_kernel(files, name, cx):
-    """K0 + K1 (+ K1e<8> behind the lean instantiation, K1e<1> behind kCx) in F_STORE over garbage, F_ADD, and
-    F_ATOMIC with 1, 2 and 5 CTAs per tile: everything but the hard reads, exactly."""
+def test_limit_tile_kernel(files, name, cx, monkeypatch):
+    """K0 + K1 (+ K1e<8> behind the lean instantiation, K1e<1> behind kCx, + K1g) as kdl_pileup_range launches them, in
+    F_STORE over garbage, F_ADD, and F_ATOMIC with 2 and 5 CTAs per tile: the whole table and every event, exactly.  A
+    group without tile-eligible complex reads runs kCx by a direct launch (no entry point picks it there): everything
+    but the hard reads."""
     b = batch_of(files, name)
     assert E.tileable(b)
     want_c, want_e = coracle.pileup(b)
-    want = want_c - _hard_table(b)
-    for mode, split in ((E.F_STORE, 1), (E.F_ADD, 1), (E.F_ATOMIC, 2), (E.F_ATOMIC, 5)):
-        got, ev = E.run_pileup(b, mode, cx=cx, split=split, grid=4, want_events=True, zero_rest=mode == E.F_STORE)
-        np.testing.assert_array_equal(got, want, err_msg="%s mode=%d split=%d" % (name, mode, split))
-        hard_rows = np.isin(want_e[:, 1], b.hard_idx.astype(np.int64)) if b.n_hard else np.zeros(len(want_e), bool)
-        np.testing.assert_array_equal(ev[~hard_rows], want_e[~hard_rows])
+    direct = cx and b.n_complex == b.n_hard
+    monkeypatch.setenv("KDL_CX", "pieces" if cx else "atomics")
+    for fresh, split in ((True, 1), (False, 1), (False, 2), (False, 5)):
+        what = "%s fresh=%s split=%d" % (name, fresh, split)
+        if direct:
+            got = E.tile_cx_pileup(b, fresh, split, zero_rest=fresh)
+            np.testing.assert_array_equal(got, want_c - _hard_table(b), err_msg=what)
+            continue
+        monkeypatch.setenv("KDL_SPLIT", str(split))
+        got, ev = E.run_pileup(b, fresh, want_events=True, zero_rest=fresh)
+        np.testing.assert_array_equal(got, want_c, err_msg=what)
+        np.testing.assert_array_equal(ev, want_e, err_msg=what)
 
 
 @emu
 @pytest.mark.parametrize("schedule,seed", [("forward", 0), ("reverse", 0), ("random", 3)])
-def test_limit_pipeline(files, schedule, seed):
+def test_limit_pipeline(files, schedule, seed, monkeypatch):
     """The whole pileup pipeline (K0 + K1 + K1e + K1g, as kdl_pileup launches them) under three thread orders."""
     E.set_schedule(schedule, seed)
     try:
@@ -241,7 +248,8 @@ def test_limit_pipeline(files, schedule, seed):
             b = batch_of(files, name)
             want_c, want_e = coracle.pileup(b)
             for split in ((1, 2) if schedule == "forward" else (1,)):
-                got_c, got_e = E.pileup_pipeline(b, split=split)
+                monkeypatch.setenv("KDL_SPLIT", str(split))
+                got_c, got_e = E.pileup_pipeline(b)
                 np.testing.assert_array_equal(got_c, want_c, err_msg="%s %s split=%d" % (name, schedule, split))
                 np.testing.assert_array_equal(got_e, want_e, err_msg=name)
     finally:
@@ -250,10 +258,9 @@ def test_limit_pipeline(files, schedule, seed):
 
 @emu
 @pytest.mark.parametrize("schedule", ["forward", "random"])
-def test_limit_k1q_mask_lattice(files, schedule):
+def test_limit_k1q_mask_lattice(files, schedule, monkeypatch):
     """K1q after the pipeline on the corpus's quality lattice equals the masking oracle."""
     E.set_schedule(schedule, 7)
-    emu_mask_harness.set_schedule(schedule, 7)
     try:
         for name in GROUPS:
             text, sam, bam = files[name]
@@ -263,12 +270,12 @@ def test_limit_k1q_mask_lattice(files, schedule):
             assert masked.n_masked == int((qual < LC.MASK_QUAL).sum()) > 0
             want_c, want_e = qoracle.pileup(plain, qual, LC.MASK_QUAL)
             for split in (1, 3):
-                got_c, got_e = E.pileup_pipeline(masked, split=split)
-                np.testing.assert_array_equal(emu_mask_harness.unmask(masked, got_c), want_c, err_msg=name)
+                monkeypatch.setenv("KDL_SPLIT", str(split))
+                got_c, got_e = E.pileup_pipeline(masked)
+                np.testing.assert_array_equal(E.unmask(masked, got_c), want_c, err_msg=name)
                 np.testing.assert_array_equal(got_e, want_e, err_msg=name)
     finally:
         E.set_schedule("forward")
-        emu_mask_harness.set_schedule("forward")
 
 
 # ---- footprints ---------------------------------------------------------------------------------------------------

@@ -8,7 +8,6 @@ import numpy as np
 import pytest
 
 import emu_harness
-import emu_mask_harness
 from fuzz_cases import random_case
 from kindel_b200 import bamio, cli, kindel, synth
 from kindel_b200 import distributed as D
@@ -154,7 +153,7 @@ def test_masked_exotic_base_is_simple_and_does_not_raise(tmp_path):
             assert batch.n_masked == 1 and not batch.n_complex  # masked R reads as N: a simple read
             want, _ = qoracle.pileup(bamio.read_alignment(p), qual_bytes, thr)
             got, _ = emu_harness.pileup_pipeline(batch)
-            assert np.array_equal(emu_mask_harness.unmask(batch, got), want)
+            assert np.array_equal(emu_harness.unmask(batch, got), want)
             assert want[4].sum() == 0 and want[0:4].sum() == 4
 
 
@@ -179,7 +178,7 @@ def _emu_vs_oracle(text, thr):
         want = e
     try:
         counts, events = emu_harness.pileup_pipeline(masked)
-        got = (emu_mask_harness.unmask(masked, counts), events)
+        got = (emu_harness.unmask(masked, counts), events)
     except (IndexError, KeyError) as e:
         got = e
     if isinstance(want, Exception) or isinstance(got, Exception):
@@ -195,7 +194,6 @@ def _emu_vs_oracle(text, thr):
 @pytest.mark.parametrize("schedule", ["forward", "reverse", "random"])
 def test_k1q_emulated_equals_masking_oracle(schedule):
     emu_harness.set_schedule(schedule, 5)
-    emu_mask_harness.set_schedule(schedule, 5)
     seeds = range(400) if schedule == "forward" else range(0, 400, 4)
     total = 0
     try:
@@ -203,20 +201,20 @@ def test_k1q_emulated_equals_masking_oracle(schedule):
             total += _emu_vs_oracle(with_fields(random_case(seed), seed), THRESHOLDS[seed % 4 + 1]) or 0
     finally:
         emu_harness.set_schedule("forward")
-        emu_mask_harness.set_schedule("forward")
     assert total > 0
 
 
 @pytest.mark.skipif(not emu_harness.available(), reason="needs g++ and the CUDA headers")
-def test_k1q_emulated_on_synthetic_reads():
+def test_k1q_emulated_on_synthetic_reads(monkeypatch):
     """Tile-eligible complex reads, hard reads (POS 0 wrap, overhanging right clips) and the depth split."""
     for seed, batch in ((1, synth.complex_reads(1, 4000, 60)), (2, synth.mixed_reads(3, [20000], 30, 0.1))):
         masked, qual = synth.with_qualities(batch, seed)
         assert masked.n_masked > 0 and masked.n_hard > 0 or seed == 2
         want = qoracle.pileup(batch, qual, 20)
         for split in (1, 3):
-            counts, events = emu_harness.pileup_pipeline(masked, split=split)
-            assert np.array_equal(emu_mask_harness.unmask(masked, counts), want[0])
+            monkeypatch.setenv("KDL_SPLIT", str(split))
+            counts, events = emu_harness.pileup_pipeline(masked)
+            assert np.array_equal(emu_harness.unmask(masked, counts), want[0])
             assert np.array_equal(events, want[1])
 
 

@@ -15,8 +15,7 @@ distributed.ShardedConsensus itself the same way on one GPU)."""
 import numpy as np
 import pytest
 
-import emu_harness
-import emu_map_harness as E
+import emu_harness as E
 from kindel_b200 import distributed as D
 from kindel_b200 import synth
 from oracle import coracle, qoracle
@@ -64,7 +63,9 @@ emu = pytest.mark.skipif(not E.available(), reason="needs g++ and the CUDA heade
 @emu
 @pytest.mark.parametrize("split", [1, 3])
 @pytest.mark.parametrize("cx", [False, True], ids=["atomics", "pieces"])
-def test_reused_table_sequence_emulated(cx, split):
+def test_reused_table_sequence_emulated(cx, split, monkeypatch):
+    monkeypatch.setenv("KDL_CX", "pieces" if cx else "atomics")
+    monkeypatch.setenv("KDL_SPLIT", str(split))
     seq = _sequence(unsorted=True)
     n_slots = seq[0][1].n_slots
     table = np.zeros((19, n_slots), dtype=np.int32)   # what CountTable allocates: zeros, map zero
@@ -76,7 +77,7 @@ def test_reused_table_sequence_emulated(cx, split):
     for name, b in seq:
         want, want_ev = coracle.pileup(b)
         what = "%s (cx=%s, split=%d)" % (name, cx, split)
-        ev = E.fresh_pileup(b, table, dmap, zero_rest=prev_complex, split=split, cx=cx)
+        ev = E.fresh_pileup(b, table, dmap, zero_rest=prev_complex)
         np.testing.assert_array_equal(table, want, err_msg=what)
         np.testing.assert_array_equal(ev, want_ev, err_msg=what)
         assert_map_covers(table, dmap, what)
@@ -85,7 +86,7 @@ def test_reused_table_sequence_emulated(cx, split):
         if b.n_complex * 16 >= b.n_reads:
             assert (dmap == 0xFFFFFFFF).all(), what + ": dense complex reads leave the range marked"
         marked.append(map_bits(dmap).mean())
-        ev = E.fresh_pileup(b, ones, omap, zero_rest=True, split=split, cx=cx)
+        ev = E.fresh_pileup(b, ones, omap, zero_rest=True)
         np.testing.assert_array_equal(ones, want, err_msg=what + " (map of ones)")
         np.testing.assert_array_equal(ev, want_ev, err_msg=what + " (map of ones)")
         assert_map_covers(ones, omap, what + " (map of ones)")
@@ -242,8 +243,7 @@ class _EmuRankTable:
         if self.dirty is not None:
             lo, hi = min(lo, self.dirty[0]), max(hi, self.dirty[1])
         lo, hi = max(0, lo // 512 * 512), min(n_slots, (hi + 511) // 512 * 512)
-        cx = (batch.n_complex - batch.n_hard) * 16 >= batch.n_reads  # kdl_pileup_range_map's choice
-        ev = E.fresh_pileup(batch, self.t, self.map, self.dirty_rest, cx=cx, slot_range=(lo, hi))
+        ev = E.fresh_pileup(batch, self.t, self.map, self.dirty_rest, slot_range=(lo, hi))
         self.dirty, self.dirty_rest = (lo, hi), batch.n_complex > 0
         return ev
 
@@ -282,7 +282,7 @@ def test_sharded_epochs_emulated(world, kind):
     for epoch in range(1, 5):
         par = epoch & 1
         evs = [tables[r][par].pileup(shards[r], feet[r]) for r in range(world)]
-        emu_harness.exchange_epoch([tables[r][par].t for r in range(world)], feet, slices, calls[par], flags, epoch, min_depth=2)
+        E.exchange_epoch([tables[r][par].t for r in range(world)], feet, slices, calls[par], flags, epoch, min_depth=2)
         for r in range(world):
             what = "%s world %d epoch %d rank %d" % (kind, world, epoch, r)
             np.testing.assert_array_equal(calls[par][r], want_calls, err_msg=what)

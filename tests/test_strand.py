@@ -1,5 +1,5 @@
 """`variants --vcf --strand` (extension) without a GPU: the strand byte at decode and through the batch helpers, K8
-from its CUDA source under the host emulator (tests/emu/emu_select.cpp) against bamio.select_reads, the oracle
+from its CUDA source under the host emulator (tests/emu/emu_api.cpp) against bamio.select_reads, the oracle
 (oracle/py_soracle.py) against a truth set with alleles planted on one strand, the SOR rule and the CLI."""
 import os
 
@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import combo_cases as CC
-import emu_select_harness as ES
+import emu_harness as E
 import helpers as H
 import limit_cases as LC
 import strand_cases as S
@@ -17,7 +17,7 @@ from kindel_b200 import kindel as K
 from oracle import py_soracle as SO
 from oracle import samdecode
 
-needs_emu = pytest.mark.skipif(not ES.available(), reason="needs g++ and the CUDA headers")
+needs_emu = pytest.mark.skipif(not E.available(), reason="needs g++ and the CUDA headers")
 INPUTS = os.path.join(H.ROOT, "tests", "golden", "inputs")
 FIXTURES = sorted(f for f in os.listdir(INPUTS) if f.endswith((".bam", ".sam")))
 
@@ -120,7 +120,7 @@ def _unsorted(batch):
 @needs_emu
 @pytest.mark.parametrize("schedule,seed", [("forward", 0), ("reverse", 0), ("random", 3)])
 def test_emulated_k8_equals_select_reads(schedule, seed, tmp_path):
-    ES.set_schedule(schedule, seed)
+    E.set_schedule(schedule, seed)
     n = hard = masked = cx = 0
     for name, b in _corpus(tmp_path):
         rng = np.random.default_rng(seed + len(name))
@@ -132,7 +132,7 @@ def test_emulated_k8_equals_select_reads(schedule, seed, tmp_path):
             keeps.append(k)
         for j, keep in enumerate(keeps):
             want = bamio.select_reads(b, np.flatnonzero(keep))
-            ES.assert_equal(ES.select(b, keep), ES.fields(want), (name, j))
+            S.assert_equal(E.select(b, keep), S.fields(want), (name, j))
             n += 1
         hard += b.n_hard > 0
         cx += b.n_complex > b.n_hard
@@ -146,16 +146,16 @@ def test_emulated_k8_sorts_a_subset_of_an_unsorted_batch():
     assert b.reads_sorted and b.ref_start[0] != b.ref_start[1]
     parent, keep = _unsorted(b)
     assert not parent.reads_sorted
-    got = ES.select(parent, keep)
+    got = E.select(parent, keep)
     want = bamio.select_reads(parent, np.flatnonzero(keep))
     assert want.reads_sorted and got["reads_sorted"]
-    ES.assert_equal(got, ES.fields(want), "unsorted parent")
+    S.assert_equal(got, S.fields(want), "unsorted parent")
     # and a subset that keeps the swapped pair stays unsorted
     keep2 = np.ones(b.n_reads, np.uint8)
     keep2[5] = 0
-    got2 = ES.select(parent, keep2)
+    got2 = E.select(parent, keep2)
     assert not got2["reads_sorted"]
-    ES.assert_equal(got2, ES.fields(bamio.select_reads(parent, np.flatnonzero(keep2))), "unsorted subset")
+    S.assert_equal(got2, S.fields(bamio.select_reads(parent, np.flatnonzero(keep2))), "unsorted subset")
 
 
 # ------------------------------------------------------------------------------------------------ oracle, SOR

@@ -1,6 +1,6 @@
 """`variants --vcf --reference` (extension) without a GPU: the FASTA loader, a truth set of planted SNVs, insertions and
 deletions that pins the oracle (oracle/py_rvoracle.py), K6r and K7 from their CUDA source under the host emulator
-(tests/emu/emu_variants_ref.cpp) against the oracle, and the host VCF writer over the emulated kernels.
+(tests/emu/emu_api.cpp) against the oracle, and the host VCF writer over the emulated kernels.
 
 The truth set (`truth_set`) is generated here: a random reference, alleles planted at chosen fractions -- at the first
 and last positions, next to each other, several at one locus -- and error-free reads whose CIGARs are taken from the
@@ -10,7 +10,7 @@ import gzip
 import numpy as np
 import pytest
 
-import emu_variants_ref_harness as ER
+import emu_harness as E
 import limit_cases as LC
 from fuzz_cases import random_case
 from kindel_b200 import bamio, cli, engine, _ffi
@@ -21,7 +21,7 @@ from oracle import py_oracle as PO
 from oracle import py_rvoracle as RV
 from test_variants_vcf import GRID, adversarial
 
-needs_emu = pytest.mark.skipif(not ER.available(), reason="needs g++ and the CUDA headers")
+needs_emu = pytest.mark.skipif(not E.available(), reason="needs g++ and the CUDA headers")
 NAN = float("nan")
 OPS = "MIDNSHP=X"
 
@@ -283,26 +283,26 @@ def _sites_equal(got, want, what):
 def test_emulated_k6r_equals_oracle(schedule, seed, tmp_path):
     """K6r from its source == RV.sites: adversarial tables over the whole threshold grid, the fuzz and limit tables
     at two grid points each and the default thresholds."""
-    ER.set_schedule(schedule, seed)
+    E.set_schedule(schedule, seed)
     try:
         n_sites = 0
         for s in (1, 2):
             table, cs, cl, codes = ref_adversarial(s + seed)
             for a, r in GRID:
                 want = RV.sites(table, cs, cl, codes, a, r)
-                got = ER.variant_sites_ref(table, cs, cl, codes, engine.variant_abs_floor(a), r)
+                got = E.variant_sites_ref(table, cs, cl, codes, engine.variant_abs_floor(a), r)
                 _sites_equal(got, want, (schedule, s, a, r))
                 n_sites += len(want[0])
         for j, (name, batch, table, codes, _) in enumerate(corpus(tmp_path, range(seed, 400, 4))):
             for a, r in [GRID[(7 * j + i) % len(GRID)] for i in range(2)] + [(1, 0.01), (0, 0.0)]:
                 want = RV.sites(table, batch.contig_slot, batch.contig_len, codes, a, r)
-                got = ER.variant_sites_ref(table, batch.contig_slot, batch.contig_len, codes,
+                got = E.variant_sites_ref(table, batch.contig_slot, batch.contig_len, codes,
                                            engine.variant_abs_floor(a), r)
                 _sites_equal(got, want, (schedule, name, a, r))
                 n_sites += len(want[0])
         assert n_sites > 20_000
     finally:
-        ER.set_schedule("forward")
+        E.set_schedule("forward")
 
 
 def _oracle_events(batch, groups):
@@ -319,11 +319,11 @@ def _oracle_events(batch, groups):
 def test_emulated_k7_equals_oracle(schedule, seed, tmp_path):
     """K7 from its source: the events of every fuzz and limit case (POS 0, mid-read S, D past the end) in read order
     == the oracle's walk over the decoded records, and on an unsorted copy of a batch the same events."""
-    ER.set_schedule(schedule, seed)
+    E.set_schedule(schedule, seed)
     try:
         n = 0
         for name, batch, _, _, groups in corpus(tmp_path, range(400) if schedule == "forward" else range(seed, 400, 3)):
-            slot, length = ER.deletion_events(batch)
+            slot, length = E.deletion_events(batch)
             got = list(zip(slot.tolist(), length.tolist()))
             assert got == _oracle_events(batch, groups), name
             n += len(got)
@@ -332,11 +332,11 @@ def test_emulated_k7_equals_oracle(schedule, seed, tmp_path):
         p = tmp_path / "truth.bam"
         bamio.write_bam(p, [("t", len(ref))], bam_records(reads[::-1]))  # reversed: not coordinate-sorted
         batch = bamio.read_alignment(p)
-        slot, length = ER.deletion_events(batch)
+        slot, length = E.deletion_events(batch)
         assert sorted(zip(slot.tolist(), length.tolist())) == sorted(
             (r, n) for r, n in RV.deletion_events(len(ref), _recs(reads[::-1])))
     finally:
-        ER.set_schedule("forward")
+        E.set_schedule("forward")
 
 
 # ------------------------------------------------------------------------------------------- host VCF
@@ -348,10 +348,10 @@ class _Emulated:
         self.batch = batch
 
     def sites(self, counts, contig_slot, contig_len, ref, a, r):
-        return ER.variant_sites_ref(counts, contig_slot, contig_len, ref, engine.variant_abs_floor(a), r)
+        return E.variant_sites_ref(counts, contig_slot, contig_len, ref, engine.variant_abs_floor(a), r)
 
     def deletions(self, dbatch, counts, a, r):
-        slot, length = ER.deletion_events(self.batch)
+        slot, length = E.deletion_events(self.batch)
         groups = {}
         for key in zip(slot.tolist(), length.tolist()):
             groups[key] = groups.get(key, 0) + 1

@@ -2,7 +2,7 @@
 
 oracle/py_voracle.py restates the rule as a per-position loop over plain ints and floats.  The product's numpy helper
 (kindel.variant_alleles, through kindel.variant_sites on host tables) and K6 -- run from its CUDA source under the
-host emulator (tests/emu/emu_variants.cpp) -- must both reproduce it, over a threshold grid that includes negative,
+host emulator (tests/emu/emu_api.cpp) -- must both reproduce it, over a threshold grid that includes negative,
 NaN, non-integer and out-of-range thresholds, on the fuzz, combo and limit corpora and on adversarial tables with counts
 planted in the slot behind each contig and in the padding.  The VCF writer is checked line by line and against a VCF
 built from the restatement's sites."""
@@ -14,7 +14,7 @@ import pandas as pd
 import pytest
 
 import combo_cases as CC
-import emu_variants_harness as EV
+import emu_harness as E
 import limit_cases as LC
 from conftest import golden_input
 from fuzz_cases import random_case
@@ -23,7 +23,7 @@ from kindel_b200 import _ffi
 from kindel_b200 import kindel as K
 from oracle import coracle, py_voracle as V
 
-needs_emu = pytest.mark.skipif(not EV.available(), reason="needs g++ and the CUDA headers")
+needs_emu = pytest.mark.skipif(not E.available(), reason="needs g++ and the CUDA headers")
 NAN = float("nan")
 ABS = (-5, -1, 0, 1, 2, 2 ** 31, 10 ** 12, 1.5)
 REL = (-0.5, 0.0, 0.01, 0.25, 0.5, 1.0, NAN)
@@ -189,7 +189,7 @@ def test_planted_slots_are_never_sites():
 
 # ----------------------------------------------------------------------------------------------- K6
 def _emulated(table, cs, cl, a, r):
-    return EV.variant_sites(table, cs, cl, engine.variant_abs_floor(a), r)
+    return E.variant_sites(table, cs, cl, engine.variant_abs_floor(a), r)
 
 
 @needs_emu
@@ -197,7 +197,7 @@ def _emulated(table, cs, cl, a, r):
 def test_emulated_k6_equals_restatement(schedule, seed, tmp_path):
     """K6 from its source under three thread orders == the loop: adversarial tables (not a multiple of the CTA span),
     planted slot-L / padding counts, a table with no site, and fuzz, limit and combo tables."""
-    EV.set_schedule(schedule, seed)
+    E.set_schedule(schedule, seed)
     try:
         tables = [("adversarial%d" % s,) + adversarial(s + seed) for s in (1, 2)]
         tables.append(("empty", np.zeros((19, 2052), dtype=np.int32), np.array([0, 1030]), np.array([1000, 1020])))
@@ -215,7 +215,7 @@ def test_emulated_k6_equals_restatement(schedule, seed, tmp_path):
         assert len(_emulated(*tables[2][1:], -1, -0.5)[0]) == 2020  # the empty table: every position at < 0
         assert len(_emulated(*tables[2][1:], 0, 0.0)[0]) == 0
     finally:
-        EV.set_schedule("forward")
+        E.set_schedule("forward")
 
 
 def _tables_small(tmp_path):
