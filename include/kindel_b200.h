@@ -347,6 +347,42 @@ int kdl_select_count(const kdl_batch* batch, const kdl_qmask* qmask, const uint8
 int kdl_select_scatter(const kdl_batch* batch, const kdl_qmask* qmask, const uint8_t* keep, const uint32_t* scratch,
                        const kdl_batch* out, const kdl_qmask* out_mask, void* stream);
 
+/* K9 (extension: `--primers scheme.bed`): masks the bases of every read that copy an amplicon primer, as
+ * min_base_quality masks a low-quality base (N in seq4, listed in the mask list for kdl_unmask), before the pileup.
+ * Per read on contig c with at least one M/=/X base: s and e are the walk cursors (the reference's r_pos, before the
+ * Python index wrap) of its first and its last M/=/X base.  Left: if a primer [a, b) of c has a <= s < b, B = the
+ * largest such b, and every M/=/X base with cursor in [s, B) is masked.  Right: if a primer has a <= e < b, A = the
+ * smallest such a, and every M/=/X base with cursor in [A, e] is masked.  Nothing else is masked (inserted and clipped
+ * bases, deletions, clip events are untouched), and only bases inside the read's SEQ.  The primers of contig c, two
+ * sorted views of the same intervals [contig_off[c], contig_off[c + 1]) (device pointers, int32 coordinates):
+ *   start_sorted / end_max   starts ascending, end_max[i] = the largest end of the intervals up to i in that order
+ *   end_sorted / start_min   ends ascending, start_min[i] = the smallest start of the intervals from i on in that order
+ * (end_max and start_min restart at every contig).  n_contigs must be the batch's.
+ *   kdl_primers_count  per-CTA counts and their scans.  scratch: device uint32[kdl_primers_scratch_words(n_reads)]; its
+ *                      last 8 words are the totals record, read back once: [0] reads in the new mask list, [1] bases in
+ *                      it, [2] reads with primer bases, [3] primer bases.
+ *   kdl_primers_apply  on the same stream after it: writes the new mask list into out_mask (arrays sized by the
+ *                      totals; NULL when totals[0] == 0) -- per read the sorted union of its entries in qmask (may be
+ *                      NULL or empty) and its primer bases, each base once -- and sets the primer bases' nibbles to N
+ *                      (15) in `seq4`: the batch's own seq4 (in place) or a copy of it.
+ * One thread per 4 consecutive reads; a read owns whole words of seq4, so no atomics. */
+typedef struct kdl_primers {
+    int32_t n_contigs;
+    int32_t reserved;
+    int64_t n_intervals;
+    const int64_t* contig_off; /* [n_contigs + 1] */
+    const int32_t* start_sorted;
+    const int32_t* end_max;
+    const int32_t* end_sorted;
+    const int32_t* start_min;
+} kdl_primers;
+
+int64_t kdl_primers_scratch_words(int64_t n_reads);
+int kdl_primers_count(const kdl_batch* batch, const kdl_qmask* qmask, const kdl_primers* primers, uint32_t* scratch,
+                      void* stream);
+int kdl_primers_apply(const kdl_batch* batch, const kdl_qmask* qmask, const kdl_primers* primers,
+                      const uint32_t* scratch, uint32_t* seq4, const kdl_qmask* out_mask, void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced

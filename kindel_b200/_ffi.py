@@ -69,6 +69,19 @@ class KdlQmask(C.Structure):
     ]
 
 
+class KdlPrimers(C.Structure):
+    _fields_ = [
+        ("n_contigs", C.c_int32),
+        ("reserved", C.c_int32),
+        ("n_intervals", C.c_int64),
+        ("contig_off", C.c_void_p),
+        ("start_sorted", C.c_void_p),
+        ("end_max", C.c_void_p),
+        ("end_sorted", C.c_void_p),
+        ("start_min", C.c_void_p),
+    ]
+
+
 class KdlExchange(C.Structure):
     _fields_ = [
         ("n_ranks", C.c_int32),
@@ -135,6 +148,11 @@ _PROTOTYPES = {
     "kdl_select_count": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_select_scatter": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_void_p,
                                      C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p]),
+    "kdl_primers_scratch_words": (C.c_int64, [C.c_int64]),
+    "kdl_primers_count": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.POINTER(KdlPrimers), C.c_void_p,
+                                    C.c_void_p]),
+    "kdl_primers_apply": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.POINTER(KdlPrimers), C.c_void_p,
+                                    C.c_void_p, C.POINTER(KdlQmask), C.c_void_p]),
     "kdl_vote_peers":(C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,

@@ -6,7 +6,8 @@ extension one FASTQ record per contig instead),
 `weights` / `features` write TSV to stdout (cli.py:44,50), `version` prints `kindel <version>`;
 `variants` (in the reference's README only) is an extension, see kindel.variants; its `--vcf` writes a sites-only VCF
 (kindel.variants_vcf), against a FASTA with `--reference`, with per-strand counts and a strand odds ratio with
-`--strand` / `--max-sor`.
+`--strand` / `--max-sor`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
+bases of every read before the pileup (kindel_b200/primers.py).
 argh derived the flags from the function signatures (first letter as short option unless two
 parameters share it); argparse spells the same set out.  Note the CLI default `--min-overlap 7`
 (cli.py:13) differs from the API default 9 (kindel.py:492), as in the reference.
@@ -95,6 +96,10 @@ def _add_filters(p):
     p.add_argument("--min-mapq", type=int, default=0, help="skip records with mapping quality below this value")
     p.add_argument("--exclude-flags", type=_flags, default=0,
                    help="skip records with any of these FLAG bits set (decimal or 0x...)")
+    # extension: amplicon primer masking, off by default
+    p.add_argument("--primers", default=None, metavar="BED",
+                   help="mask the bases of each read that lie in an amplicon primer of this BED (plain or gzip): read "
+                        "as N, not counted")
 
 
 def _iupac_threshold(text: str) -> float:
@@ -110,7 +115,10 @@ def _max_sor(text: str) -> float:
 
 
 def _filters(a) -> dict:
-    return dict(min_base_quality=a.min_base_quality, min_mapq=a.min_mapq, exclude_flags=a.exclude_flags)
+    out = dict(min_base_quality=a.min_base_quality, min_mapq=a.min_mapq, exclude_flags=a.exclude_flags)
+    if a.primers is not None:  # (the keyword only when given: every call without it stays as it was)
+        out["primers"] = a.primers
+    return out
 
 
 def build_parser() -> argparse.ArgumentParser:

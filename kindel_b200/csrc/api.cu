@@ -14,6 +14,7 @@
 #include "assemble.cu"
 #include "variants.cu"
 #include "select.cu"
+#include "primers.cu"
 
 namespace {
 
@@ -595,6 +596,58 @@ int kdl_select_scatter(const kdl_batch* batch, const kdl_qmask* qmask, const uin
     const long long n_blocks = select_blocks(batch->n_reads);
     KDL_LAUNCH(kdl::select_scatter_kernel, (unsigned)n_blocks, kdl::S_THREADS, 0, (cudaStream_t)stream,
                *batch, q, keep, scratch, *out, const_cast<int64_t*>(out->contig_read_off), om);
+    return check_launch();
+}
+
+static long long primer_blocks(int64_t n_reads) { return n_reads / kdl::P_BLOCK + 1; }
+
+static int primer_args(const kdl_batch* batch, const kdl_qmask* qmask, const kdl_primers* primers, kdl_qmask* q) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if ((rc = select_qmask(qmask, q)) != KDL_OK) return rc;
+    if (!primers || primers->n_contigs != batch->n_contigs || primers->n_intervals < 0 ||
+        primers->n_intervals >= (int64_t)INT32_MAX || !primers->contig_off || batch->n_reads >= (int64_t)UINT32_MAX ||
+        (primers->n_intervals > 0 && (!primers->start_sorted || !primers->end_max || !primers->end_sorted ||
+                                      !primers->start_min)))
+        return KDL_ERR_INVALID_ARG;
+    return KDL_OK;
+}
+
+int64_t kdl_primers_scratch_words(int64_t n_reads) {
+    return n_reads < 0 ? 0 : (int64_t)kdl::P_NROW * (primer_blocks(n_reads) + 1) + kdl::P_TOTALS;
+}
+
+int kdl_primers_count(const kdl_batch* batch, const kdl_qmask* qmask, const kdl_primers* primers, uint32_t* scratch,
+                      void* stream) {
+    kdl_qmask q;
+    int rc = primer_args(batch, qmask, primers, &q);
+    if (rc != KDL_OK) return rc;
+    if (!scratch) return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = primer_blocks(batch->n_reads);
+    cudaStream_t st = (cudaStream_t)stream;
+    KDL_LAUNCH(kdl::primers_sums_kernel, (unsigned)n_blocks, kdl::P_THREADS, 0, st, *batch, q, *primers, scratch,
+               n_blocks);
+    if ((rc = check_launch()) != KDL_OK) return rc;
+    for (int k = kdl::P_MBASES; k <= kdl::P_MREADS; ++k) {
+        KDL_LAUNCH(kdl::assemble_scan_sums_kernel, 1, kdl::A_THREADS, 0, st, scratch + (size_t)k * (n_blocks + 1),
+                   n_blocks);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+    }
+    KDL_LAUNCH(kdl::primers_totals_kernel, 1, kdl::P_THREADS, 0, st, scratch, n_blocks);
+    return check_launch();
+}
+
+int kdl_primers_apply(const kdl_batch* batch, const kdl_qmask* qmask, const kdl_primers* primers,
+                      const uint32_t* scratch, uint32_t* seq4, const kdl_qmask* out_mask, void* stream) {
+    kdl_qmask q, om;
+    int rc = primer_args(batch, qmask, primers, &q);
+    if (rc != KDL_OK) return rc;
+    if ((rc = select_qmask(out_mask, &om)) != KDL_OK) return rc;
+    if (!scratch || (batch->n_reads > 0 && !seq4) || (om.n_reads > 0 && om.n_bases > 0 && !om.qpos))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = primer_blocks(batch->n_reads);
+    KDL_LAUNCH(kdl::primers_scatter_kernel, (unsigned)n_blocks, kdl::P_THREADS, 0, (cudaStream_t)stream, *batch, q,
+               *primers, scratch, n_blocks, seq4, om);
     return check_launch();
 }
 

@@ -29,6 +29,7 @@ import os
 import numpy as np
 
 from . import _ffi, bamio
+from .primers import load_arrays, save_arrays
 
 
 select_reads = bamio.select_reads
@@ -260,9 +261,13 @@ class ShardedConsensus:
     neighbour whose footprint reaches into it (the core of a slice waits for nobody), and the gather K2g waits for
     each peer's slice.  Nothing of step n has to finish before K1 of step n+1 starts overwriting the other
     table.  "peer": the same vote kernel behind an NCCL barrier + all_gather.  "allreduce": NCCL all_reduce of
-    the 7 vote columns, vote replicated (what the north star words literally; the baseline)."""
+    the 7 vote columns, vote replicated (what the north star words literally; the baseline).
 
-    def __init__(self, shard: bamio.ReadBatch, device, mode: str = "fused", group=None):
+    primers (extension): a primers.PrimerArrays over the shard's contigs; K9 then masks the shard's primer bases on
+    the device right after the upload, before the first pileup (the rule is per read: every shard's masks are those
+    of the whole batch)."""
+
+    def __init__(self, shard: bamio.ReadBatch, device, mode: str = "fused", group=None, primers=None):
         import torch
         import torch.distributed as dist
 
@@ -274,6 +279,8 @@ class ShardedConsensus:
         self.rank = dist.get_rank(group)
         self.n_slots = shard.n_slots
         self.dbatch = engine.upload(shard, device)
+        if primers is not None:
+            self.dbatch = engine.mask_primers(self.dbatch, primers)
         self.lib = _ffi.load()
         self.epoch = 0
         if mode in ("peer", "fused"):
@@ -424,7 +431,8 @@ def _free_port() -> int:
 
 def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode: str, plan: str,
                 iupac_threshold=None):
-    """One process per GPU: pile this rank's shard, exchange, vote; rank 0 leaves the job's results in workdir."""
+    """One process per GPU: pile this rank's shard (its primer bases masked first when workdir holds primer arrays),
+    exchange, vote; rank 0 leaves the job's results in workdir."""
     import json
     import os
     import traceback
@@ -444,7 +452,9 @@ def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode:
         batch = bamio.load_batch(os.path.join(workdir, "batch"))
         idx = shard_indices(batch, rank, world, plan)
         shard = select_reads(batch, idx)
-        sc = ShardedConsensus(shard, dev, mode=mode)
+        pth = os.path.join(workdir, "primers.npz")
+        primers = load_arrays(pth) if os.path.exists(pth) else None
+        sc = ShardedConsensus(shard, dev, mode=mode, primers=primers)
         calls = sc.step(min_depth, iupac_threshold=iupac_threshold)
         # data errors: the reference raises at the FIRST offending record in iteration order -- every rank
         # reports its first one (global read number), the parent re-raises the smallest
@@ -484,13 +494,14 @@ def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode:
 
 
 def run_sharded(batch: bamio.ReadBatch, devices: int, min_depth=1, mode: str = "fused", plan: str = None,
-                iupac_threshold=None):
+                iupac_threshold=None, primers=None):
     """Pileup + vote of `batch` over `devices` GPUs of this node: one process per GPU (torch.distributed, NCCL for
     the plumbing, the fused peer-memory exchange on the data path), whole contigs per rank when there are enough
     of them, else contiguous blocks of every contig's sorted reads.  Returns (calls uint8[n_slots], counts
     int32[19, n_slots], derived int32[5, n_slots], events int32[n_events, 4]) in host memory -- bit-identical to
     one GPU -- or raises the reference's IndexError / KeyError.  iupac_threshold (extension): the IUPAC vote, see
-    kindel.bam_to_consensus."""
+    kindel.bam_to_consensus.  primers (extension): primers.PrimerArrays of the batch's contigs, saved beside the batch;
+    every rank masks its shard's primer bases (ShardedConsensus)."""
     import json
     import shutil
     import tempfile
@@ -512,6 +523,8 @@ def run_sharded(batch: bamio.ReadBatch, devices: int, min_depth=1, mode: str = "
     workdir = tempfile.mkdtemp(prefix="kindel_b200_", dir=base)
     try:
         bamio.save_batch(os.path.join(workdir, "batch"), batch)
+        if primers is not None:
+            save_arrays(os.path.join(workdir, "primers.npz"), primers)
         try:
             mp.spawn(_api_worker, args=(devices, workdir, _free_port(), min_depth, mode, plan, iupac_threshold),
                      nprocs=devices, join=True)

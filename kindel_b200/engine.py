@@ -15,6 +15,7 @@ implementation behind these functions: without a CUDA device they raise.
     variant_sites_ref(...)     K6r: the SNV and insertion-candidate sites against a reference (extension)
     deletion_alleles(dbatch, counts, ...)  K7 + grouping: the deletion alleles against a reference (extension)
     select_reads(dbatch, keep) K8: the sub-batch of the kept reads, built on the device (extension)
+    mask_primers(dbatch, arrays)  K9: the batch with its amplicon primer bases masked (extension)
 """
 from __future__ import annotations
 
@@ -50,6 +51,7 @@ class DeviceBatch:
     tensors: dict
     struct: _ffi.KdlBatch
     qmask: _ffi.KdlQmask = None  # the batch's masked bases (min_base_quality); None when there are none
+    primer_masked: tuple = (0, 0)  # (reads, bases) K9 masked in it (mask_primers)
 
     @property
     def n_slots(self) -> int:
@@ -531,6 +533,59 @@ def select_reads(dbatch: DeviceBatch, keep: torch.Tensor) -> DeviceBatch:
         rc = lib.kdl_select_scatter(*args, C.byref(s), C.byref(q) if q is not None else None, _stream_ptr(dev))
         _ffi.check(rc, "kdl_select_scatter")
     return DeviceBatch(host=host, device=dev, tensors=t, struct=s, qmask=q)
+
+
+_PRIMER_TOTALS = 8  # words of K9's totals record (include/kindel_b200.h)
+
+
+def primers_struct(arrays, ptr: dict) -> _ffi.KdlPrimers:
+    """kdl_primers over the pointers `ptr` of a primers.PrimerArrays' fields."""
+    p = _ffi.KdlPrimers()
+    p.n_contigs, p.n_intervals = arrays.n_contigs, arrays.n_intervals
+    for f in ("contig_off", "start_sorted", "end_max", "end_sorted", "start_min"):
+        setattr(p, f, ptr[f])
+    return p
+
+
+def mask_primers(dbatch: DeviceBatch, arrays) -> DeviceBatch:
+    """K9 (extension: `--primers`): the batch with every read's primer bases masked (include/kindel_b200.h has the
+    rule), as min_base_quality masks a base: N in seq4 and listed in the mask list, whose count K1q takes back.
+
+    `arrays`: primers.PrimerArrays over the batch's contigs.  The nibbles are written into the batch's own device seq4,
+    in place -- the upload of one run, which nothing else reads -- and the result shares every tensor with `dbatch`
+    except the mask list, the union of the batch's own and the primer bases.  So `dbatch` itself must not be piled
+    after this call.  One 32-byte read-back sizes the list; a batch without a primer base comes back as it is.  The
+    host ReadBatch is never touched.  `primer_masked` of the result = (reads, bases) masked by the primers."""
+    lib = _ffi.load()
+    dev = dbatch.device
+    n = int(dbatch.struct.n_reads)
+    if arrays.n_contigs != int(dbatch.struct.n_contigs):
+        raise ValueError("primer arrays for %d contigs, the batch has %d" % (arrays.n_contigs, dbatch.struct.n_contigs))
+    if arrays.n_intervals == 0 or n == 0:
+        return dbatch
+    with torch.cuda.device(dev):
+        t = {f: torch.from_numpy(np.ascontiguousarray(getattr(arrays, f))).to(dev)
+             for f in ("contig_off", "start_sorted", "end_max", "end_sorted", "start_min")}
+        p = primers_struct(arrays, {f: int(x.data_ptr()) for f, x in t.items()})
+        qmask = C.byref(dbatch.qmask) if dbatch.qmask is not None else None
+        scratch = torch.empty(int(lib.kdl_primers_scratch_words(n)), dtype=torch.int32, device=dev)
+        args = (C.byref(dbatch.struct), qmask, C.byref(p), scratch.data_ptr())
+        _ffi.check(lib.kdl_primers_count(*args, _stream_ptr(dev)), "kdl_primers_count")
+        tot = scratch[-_PRIMER_TOTALS:].cpu().numpy().view(np.uint32).astype(np.int64)
+        n_mr, n_mb, n_pr, n_pb = (int(x) for x in tot[:4])
+        if n_pb == 0:
+            return dbatch
+        tensors = dict(dbatch.tensors)
+        tensors.update(mask_read=torch.empty(n_mr, dtype=torch.int32, device=dev),
+                       mask_off=torch.empty(n_mr + 1, dtype=torch.int32, device=dev),
+                       mask_qpos=torch.empty(n_mb, dtype=torch.int32, device=dev))
+        q = _ffi.KdlQmask()
+        q.n_reads, q.n_bases = n_mr, n_mb
+        q.read_idx, q.off, q.qpos = (int(tensors[f].data_ptr()) for f in ("mask_read", "mask_off", "mask_qpos"))
+        rc = lib.kdl_primers_apply(*args, int(dbatch.tensors["seq4"].data_ptr()), C.byref(q), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_primers_apply")
+    return DeviceBatch(host=dbatch.host, device=dev, tensors=tensors, struct=dbatch.struct, qmask=q,
+                       primer_masked=(n_pr, n_pb))
 
 
 def download_fields(dbatch: DeviceBatch) -> dict:

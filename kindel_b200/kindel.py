@@ -22,6 +22,7 @@ from collections import OrderedDict, namedtuple
 import numpy as np
 
 from . import bamio, engine, quality
+from .primers import as_primer_set, primer_arrays
 from .insertions import InsertionTable, decode_events, dict_consensus
 from .views import Alignment, BaseCounts, Insertions
 
@@ -55,10 +56,12 @@ class PileupRun:
 
     _device = None   # (count table, DeviceBatch) of host tables, uploaded on demand (device_tables)
     _reverse = None  # (count table, DeviceBatch) of the reverse-strand reads (reverse_table)
+    primers = None   # the PrimerSet whose primer bases the pileup masked (extension), None when off
 
-    def __init__(self, batch: bamio.ReadBatch, device=None):
+    def __init__(self, batch: bamio.ReadBatch, device=None, primers=None):
         self.batch = batch
-        self.dbatch = engine.upload(batch, device)
+        self.primers = primers
+        self.dbatch = _upload(batch, device, primers)
         self.counts, self.events = engine.pileup(self.dbatch)
         self.calls_device = None
         self._host_counts = None
@@ -66,11 +69,13 @@ class PileupRun:
         self._ins = None
 
     @classmethod
-    def from_host_tables(cls, batch, counts, derived, events):
+    def from_host_tables(cls, batch, counts, derived, events, primers=None):
         """Wrap tables that already sit in host memory (results copied back by another path, e.g.
-        the kdl_ctx_* host-buffer call or a multi-GPU reduction).  Does no computation."""
+        the kdl_ctx_* host-buffer call or a multi-GPU reduction).  Does no computation.  primers: the PrimerSet the
+        tables were piled with (a re-upload of the batch masks the same bases)."""
         run = cls.__new__(cls)
         run.batch, run.dbatch, run.counts, run.events, run.calls_device = batch, None, None, None, None
+        run.primers = primers
         run._host_counts = np.ascontiguousarray(counts, dtype=np.int32)
         run._host_derived = np.ascontiguousarray(derived, dtype=np.int32)
         run._ins = InsertionTable(batch, events)
@@ -78,14 +83,14 @@ class PileupRun:
 
     def device_tables(self):
         """(count table, DeviceBatch) on a device.  Host tables (a multi-GPU result): the reduced table and the batch
-        go to this process's GPU, once."""
+        go to this process's GPU, once (its primer bases masked again, as the ranks masked them)."""
         if self.counts is not None:
             return self.counts, self.dbatch
         if self._device is None:
             import torch
 
             dev = engine.require_cuda()
-            self._device = (torch.from_numpy(self.host_counts).to(dev), engine.upload(self.batch, dev))
+            self._device = (torch.from_numpy(self.host_counts).to(dev), _upload(self.batch, dev, self.primers))
         return self._device
 
     def reverse_table(self):
@@ -140,6 +145,14 @@ class PileupRun:
         return OrderedDict((self.batch.contig_names[c], self.alignment(c)) for c in range(self.batch.n_contigs))
 
 
+def _upload(batch, device, primers):
+    """The batch on a device; with a PrimerSet (extension) its primer bases masked there by K9 (engine.mask_primers)."""
+    dbatch = engine.upload(batch, device)
+    if primers is None:
+        return dbatch
+    return engine.mask_primers(dbatch, primer_arrays(primers, batch.contig_names, batch.contig_len))
+
+
 def _op_word(length, op):
     code = bamio._OP_CODE.get(op, 15) if op is not None else 15
     return (int(length) << 4) | code
@@ -183,31 +196,38 @@ def _default_devices(devices):
 
 
 def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq=0, exclude_flags=0,
-               iupac_threshold=None, strand=False):
+               iupac_threshold=None, strand=False, primers=None):
     """(PileupRun, calls) of an alignment file on `devices` GPUs.  devices > 1: one process per GPU, reads (or whole
     contigs) sharded, counts exchanged over NVLink in front of the vote (distributed.run_sharded); the result is
     bit-identical to one GPU.  min_base_quality / min_mapq / exclude_flags (extension, all off by default): a record
     with MAPQ < min_mapq or FLAG & exclude_flags is treated as unmapped; a base with Phred quality < min_base_quality
     is read as N and not counted (kindel_b200/bamio.py).  iupac_threshold: the vote of the sharded job (extension,
     see bam_to_consensus); calls is None for one GPU, where the caller votes.  strand (extension): the batch keeps
-    the reads' strands (PileupRun.reverse_table)."""
+    the reads' strands (PileupRun.reverse_table).  primers (extension, default None = off): a BED path or a
+    primers.PrimerSet; the bases of every read that copy an amplicon primer are then read as N and not counted, as
+    min_base_quality does with a low-quality base (K9, kindel_b200/primers.py has the rule).  With several GPUs every
+    rank masks its own shard; the result is the same."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
+    primers = as_primer_set(primers)
     batch = bamio.read_alignment(bam_path, min_mapq=min_mapq, exclude_flags=exclude_flags,
                                  min_base_quality=min_base_quality, strand=strand)
+    arrays = primer_arrays(primers, batch.contig_names, batch.contig_len) if primers is not None else None
     devices = _default_devices(devices)
     if devices <= 1:
-        run = PileupRun(batch)
+        run = PileupRun(batch, primers=primers)
         return run, None
     from . import distributed
 
-    calls, counts, derived, events = distributed.run_sharded(batch, devices, min_depth, iupac_threshold=iupac_threshold)
-    return PileupRun.from_host_tables(batch, counts, derived, events), calls
+    calls, counts, derived, events = distributed.run_sharded(batch, devices, min_depth, iupac_threshold=iupac_threshold,
+                                                             primers=arrays)
+    return PileupRun.from_host_tables(batch, counts, derived, events, primers=primers), calls
 
 
-def parse_bam(bam_path, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0):
+def parse_bam(bam_path, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None):
     """Alignment information for each reference sequence, first-seen order
-    (reference kindel/kindel.py:131-153).  devices and the filters: extensions, see pileup_run."""
-    return pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags)[0].alignments()
+    (reference kindel/kindel.py:131-153).  devices, the filters and primers: extensions, see pileup_run."""
+    return pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags,
+                      primers=primers)[0].alignments()
 
 
 # --------------------------------------------------------------------------------- consensus
@@ -530,12 +550,13 @@ DepthRange = namedtuple("DepthRange", ["dmin", "dmax"])  # min / max ACGT depth 
 
 
 def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_depth, min_overlap,
-                 clip_decay_threshold, trim_ends, uppercase, filters=None, iupac_threshold=None):
+                 clip_decay_threshold, trim_ends, uppercase, filters=None, iupac_threshold=None, primers=None):
     """REPORT text block (reference kindel/kindel.py:437-485).  filters (extension): (min_base_quality, min_mapq,
     exclude_flags); when any is set, three option lines follow `- uppercase:`, otherwise the text is the reference's.
     iupac_threshold (extension): when set, `- iupac_threshold:` follows the option lines and `- iupac sites:` (the
     positions of multi-base calls, from the `iupac` list of a changes list this module built) follows
-    `- ambiguous sites:`."""
+    `- ambiguous sites:`.  primers (extension): the primer BED's file name; when set, `- primers:` follows the filter
+    lines."""
     if isinstance(weights, DepthRange):  # already reduced on the device: no table copy needed
         dmin, dmax = weights.dmin, weights.dmax
     elif isinstance(weights, BaseCounts):
@@ -566,6 +587,8 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
     if filters is not None and any(filters):
         lines += ["- min_base_quality: {}".format(filters[0]), "- min_mapq: {}".format(filters[1]),
                   "- exclude_flags: {:#x}".format(filters[2])]
+    if primers is not None:
+        lines.append("- primers: {}".format(primers))
     if iupac_threshold is not None:
         lines.append("- iupac_threshold: {}".format(iupac_threshold))
     lines += [
@@ -586,13 +609,13 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
 # --------------------------------------------------------------------------------- public API
 def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_decay_threshold=0.1,
                      mask_ends=50, trim_ends=False, uppercase=False, devices=None, min_base_quality=0, min_mapq=0,
-                     exclude_flags=0, iupac_threshold=None, qualities=False):
+                     exclude_flags=0, iupac_threshold=None, qualities=False, primers=None):
     """Consensus sequence(s) of an alignment file (reference kindel/kindel.py:488-555).
 
     Device work per file: one pileup (K1) and one vote (K2) over all contigs at once; only the
     call bytes, the insertion events and -- for --realign and the report -- count columns come
     back to the host.  `devices` (extension; default $KINDEL_GPUS or 1) shards the pileup over that many GPUs of
-    the node.  min_base_quality / min_mapq / exclude_flags: extension, see pileup_run.
+    the node.  min_base_quality / min_mapq / exclude_flags / primers: extension, see pileup_run.
 
     iupac_threshold (extension; default None = off, the reference's vote): t in [0, 1].  Where a base is emitted,
     the call is the smallest set of the most frequent bases (A, C, G, T; N is not an allele) that holds at least
@@ -604,7 +627,7 @@ def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_d
     qualities=False.  Off, `.qualities` is None and nothing else runs."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
     filters = (min_base_quality, min_mapq, exclude_flags)
-    run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold)
+    run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold, primers=primers)
     if calls is None:
         calls = run.vote(min_depth, iupac_threshold)
     return consensus_from_run(run, calls, bam_path, realign, min_depth, min_overlap,
@@ -712,6 +735,7 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
     see bam_to_consensus -- K2q (and, with the device text, K5q) on the device, the host assembly otherwise."""
     ins_table = run.ins_table
     consensuses, refs_changes, refs_reports = [], {}, {}
+    primers_name = getattr(getattr(run, "primers", None), "name", None)
     on_device = run.counts is not None
     device_text = on_device and not realign and run.calls_device is not None
     qual_all = ins_q = qtexts = None
@@ -761,7 +785,8 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
             cons, changes = assemble_consensus(calls_all[s:e - 1], lambda p, s=s: ins_table.consensus_at(s + p),
                                                cdr_patches, trim_ends, uppercase)
         report = build_report(ref_id, report_weights, changes, cdr_patches, bam_path, realign, min_depth,
-                              min_overlap, clip_decay_threshold, trim_ends, uppercase, filters, iupac_threshold)
+                              min_overlap, clip_decay_threshold, trim_ends, uppercase, filters, iupac_threshold,
+                              primers=primers_name)
         consensuses.append(consensus_seqrecord(cons, ref_id, quals))
         refs_reports[ref_id] = report
         refs_changes[ref_id] = changes
@@ -770,12 +795,12 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
 
 def weights(bam_path: "path to SAM/BAM file", relative: "output relative nucleotide frequencies" = False,
             confidence: "calculate confidence interval" = True, confidence_alpha: "confidence interval alpha" = 0.01,
-            devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0):
+            devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None):
     """DataFrame of per-site nucleotide frequencies, depth, consensus, clip starts/ends, confidence
     interval and entropy (reference kindel/kindel.py:558-630).  Integer columns come from the GPU
-    table; the float tail is the reference's arithmetic, vectorised.  devices and the filters: extensions, see
-    pileup_run."""
-    run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags)[0]
+    table; the float tail is the reference's arithmetic, vectorised.  devices, the filters and primers: extensions,
+    see pileup_run."""
+    run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers)[0]
     return weights_from_run(run, relative, confidence, confidence_alpha)
 
 
@@ -831,7 +856,7 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
              rel_threshold: "relative frequency (0.0-1.0) above which to call variants" = 0.01,
              only_variants: "exclude invariant sites from output" = False,
              absolute: "report absolute variant frequencies" = False, devices=None, min_base_quality=0, min_mapq=0,
-             exclude_flags=0):
+             exclude_flags=0, primers=None):
     """EXTENSION -- not in the reference snapshot.  The reference's README (README.md:106-107) lists a `variants`
     sub-command ("Output variants exceeding specified absolute and relative frequency thresholds") but its code
     (kindel/kindel.py, kindel/cli.py) has no such function, so there is nothing to be bit-exact with: parity
@@ -840,8 +865,9 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
     `abs_threshold` AND whose share of the depth (A+C+G+T+N+deletions, as in `weights`) exceeds `rel_threshold`
     (variant_alleles).  Columns: chrom, pos, depth, consensus (allele letter, `-` = deletion), then one column per
     allele holding its relative (default) or absolute frequency where it is a variant and 0 elsewhere.  With
-    only_variants the sites are selected on the device (K6, variant_sites) and only they are copied back."""
-    run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags)[0]
+    only_variants the sites are selected on the device (K6, variant_sites) and only they are copied back.  primers:
+    extension, see pileup_run."""
+    run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers)[0]
     return variants_from_run(run, abs_threshold, rel_threshold, only_variants, absolute)
 
 
@@ -939,7 +965,7 @@ _VCF_ALT = ((0, "A"), (1, "C"), (2, "G"), (3, "T"), (5, "*"))  # N (4) is not an
 
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
-                 exclude_flags=0, reference=None, strand=False, max_sor=None) -> str:
+                 exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -957,11 +983,14 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
 
     strand (extension: `--strand`): every record also carries ADF / ADR, the forward- and reverse-strand counts of REF
     and of each ALT, and SOR, the strand odds ratio of each ALT; max_sor (`--max-sor`, implies strand): FILTER `sor`
-    where some ALT's SOR exceeds it.  _strand_fields has the rules."""
+    where some ALT's SOR exceeds it.  _strand_fields has the rules.
+
+    primers (extension: `--primers`): see pileup_run; the records then count no primer base (the strand counts
+    neither), and the header gets `##kindelPrimers=<the BED's file name>`."""
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
     filters = (min_base_quality, min_mapq, exclude_flags)
-    run = pileup_run(bam_path, devices, 1, *filters, strand=strand)[0]
+    run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers)[0]
     return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference, strand=strand,
                                  max_sor=max_sor)
 
@@ -1010,6 +1039,9 @@ def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None,
     lines = ["##fileformat=VCFv4.2", "##source=kindel {}".format(__version__),
              "##kindelVariants=abs_threshold={};rel_threshold={};min_base_quality={};min_mapq={};exclude_flags={:#x}"
              .format(abs_threshold, rel_threshold, mbq, mapq, flags)]
+    primers = getattr(run, "primers", None)
+    if primers is not None:
+        lines.append("##kindelPrimers={}".format(primers.name))
     if strand:
         lines.append("##kindelStrand=max_sor={}".format("." if max_sor is None else max_sor))
     if reference_name is not None:
@@ -1043,7 +1075,7 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
     """Host half of variants_vcf (see there): the VCF text of a finished pileup.  filters: (min_base_quality,
     min_mapq, exclude_flags) as the pileup applied them, for the header.  reference, strand, max_sor: see variants_vcf;
     with a reference the records are _reference_records'.  Strand needs a run whose batch has `reverse`
-    (ValueError otherwise).
+    (ValueError otherwise).  A run piled with primers (extension) adds its `##kindelPrimers` line.
 
     Strand counts (ADF, ADR): without a reference they are the reverse table's counts of the record's AD columns and
     the total's minus those, so ADF + ADR == AD.  With one, an SNV's the same (REF 0 where the reference has no A, C,
@@ -1204,12 +1236,14 @@ def _indel_strand(dp, dp_rev, ao, ao_rev, max_sor):
     return _strand_fields([max(dp_fwd - ao_fwd, 0), ao_fwd], [max(dp_rev - ao_rev, 0), ao_rev], max_sor)
 
 
-def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0):
+def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0,
+             primers=None):
     """DataFrame of relative per-site nucleotide frequencies, indels and entropy
     (reference kindel/kindel.py:633-664), including its indexing of `i`/`d` by global row number
     into the LAST contig's tables (IndexError on most multi-contig files, SURVEY.md A-14).
-    devices and the filters: extensions, see pileup_run."""
-    return features_from_run(pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags)[0])
+    devices, the filters and primers: extensions, see pileup_run."""
+    return features_from_run(pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags,
+                                        primers=primers)[0])
 
 
 def features_from_run(run):

@@ -4,6 +4,8 @@
                          (configs 2, 4, 5: 30 kb x 2000x, 5 Mb x 200x, 64 x 100 kb x 500x)
     complex_reads(...)   indel- and soft-clip-heavy CIGARs plus a tail of edge-case reads (config 3)
     strands(...)         seeded strand bytes, with reads that must lie on one strand (alleles carried by one strand)
+    tiled_scheme(...)    a tiled amplicon primer scheme as BED rows (`--primers`)
+    amplicon_reads(...)  tiled-amplicon reads: every read starts or ends at an amplicon end, in a primer
 
 Reads copy the contig's bases on M segments with a substitution rate (to A/C/G/T/N uniformly);
 inserted and clipped bases are random.  Everything is vectorised numpy so the 5 Mb x 200x case
@@ -218,6 +220,52 @@ def mixed_reads(seed: int, contig_lens, depth: float, complex_frac: float, read_
                            start_frac=start_frac, read_seed=rs)
         parts.append(on_contig(cx, names, contig_lens, c))
     return bamio.merge_batches(parts)
+
+
+def tiled_scheme(seed: int, contig_names, contig_lens, spacing: int = 200, overlap: int = 50):
+    """A tiled amplicon primer scheme (ARTIC-like) as BED rows [(chrom, start, end)]: amplicon k of a contig spans
+    [k * spacing, k * spacing + spacing + overlap), with a left primer at its start and a right primer at its end, each
+    22-30 bp long; both rows of every pair."""
+    rng = np.random.default_rng(seed)
+    rows = []
+    for name, L in zip(contig_names, (int(x) for x in contig_lens)):
+        for a in range(0, L - spacing - overlap + 1, spacing):
+            b = a + spacing + overlap
+            rows.append((name, a, a + int(rng.integers(22, 31))))
+            rows.append((name, b - int(rng.integers(22, 31)), b))
+    return rows
+
+
+def amplicon_reads(seed: int, contig_len: int, depth: float, read_len: int = 150, spacing: int = 200,
+                   overlap: int = 50, sub_rate: float = 0.01):
+    """Tiled-amplicon sequencing of one random contig: (batch, scheme rows).  Every read starts at the start of an
+    amplicon of tiled_scheme(seed, ...) or ends at its end (half each), so every read begins or ends in a primer;
+    `read_len`M reads, sorted by start."""
+    rng = np.random.default_rng(seed)
+    rows = tiled_scheme(seed, ["ctg0"], [contig_len], spacing, overlap)
+    amp_lo = np.array([a for _, a, _ in rows[0::2]], dtype=np.int64)
+    amp_hi = np.array([b for _, _, b in rows[1::2]], dtype=np.int64)
+    n = int(round(depth * contig_len / read_len))
+    words = (read_len + 7) // 8
+    k = rng.integers(0, amp_lo.shape[0], size=n)
+    starts = np.sort(np.where(rng.random(n) < 0.5, amp_lo[k], amp_hi[k] - read_len))
+    ref = random_contig(rng, contig_len)
+    ref_pad = np.concatenate([ref, np.zeros(words * 8, dtype=np.uint8)])
+    rows_packed = []
+    for s0 in range(0, n, 1 << 18):
+        st = starts[s0:s0 + (1 << 18)]
+        nib = ref_pad[st[:, None] + np.arange(words * 8, dtype=np.int64)[None, :]]
+        nib[:, read_len:] = 0
+        n_sub = rng.binomial(st.shape[0] * read_len, sub_rate)
+        nib[rng.integers(0, st.shape[0], size=n_sub), rng.integers(0, read_len, size=n_sub)] = \
+            _CODE[rng.integers(0, 5, size=n_sub)]
+        rows_packed.append(_pack_rows(nib))
+    seq4 = np.concatenate(rows_packed).reshape(-1) if rows_packed else np.zeros(0, dtype=np.uint32)
+    batch = bamio.finalize(["ctg0"], np.array([contig_len]), np.array([0, n]), starts,
+                           np.arange(n, dtype=np.int64) * words, np.full(n, read_len, dtype=np.int64),
+                           np.arange(n + 1, dtype=np.int64), np.full(n, read_len << 4, dtype=np.int64), seq4,
+                           n_records=n)
+    return batch, rows
 
 
 def to_records(batch: bamio.ReadBatch):

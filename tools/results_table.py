@@ -52,6 +52,8 @@ def row(path: str, d: dict) -> str:
         work += ", + variants against a reference (K6r, K7)"
     if d.get("strand_ms"):
         work += ", + strand split (K8, reverse pileup)"
+    if d.get("primers_ms"):
+        work += ", + primer masking (K9, K1q)"
     if d.get("map_ab"):
         work += ", zeroing A/B (dirty-sector map)"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
