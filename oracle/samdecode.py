@@ -1,7 +1,8 @@
 """TEST INFRASTRUCTURE ONLY -- stdlib (gzip + struct) BAM/SAM decoder for the oracle side.
 
 Produces record objects with exactly the attributes the reference's pileup consumes
-(`.pos`, `.mapped`, `.seq`, `.cigars`: reference kindel/kindel.py:42-48; `.rname`: :145) and the
+(`.pos`, `.mapped`, `.seq`, `.cigars`: reference kindel/kindel.py:42-48; `.rname`: :145), plus `.flag`, `.mapq` and
+`.qual` for the oracles of the record and base filters, and the
 `header["@SQ"]` shape read at kindel/kindel.py:138-141. It is deliberately independent of the
 product decoder `kindel_b200/bamio.py` (record-at-a-time struct.unpack, no numpy) so that the two
 cross-check each other. Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may
@@ -20,15 +21,17 @@ _NIBBLES = "=ACMGRSVTWYHKDBN"
 class Record:
     """simplesam.Sam look-alike: only what reference kindel/kindel.py:42-48,145 touches."""
 
-    __slots__ = ("qname", "flag", "rname", "pos", "seq", "cigars")
+    __slots__ = ("qname", "flag", "rname", "pos", "seq", "cigars", "mapq", "qual")
 
-    def __init__(self, qname, flag, rname, pos, seq, cigars):
+    def __init__(self, qname, flag, rname, pos, seq, cigars, mapq=255, qual=None):
         self.qname = qname
         self.flag = flag
         self.rname = rname
         self.pos = pos  # 1-based, SAM convention
         self.seq = seq
         self.cigars = cigars
+        self.mapq = mapq
+        self.qual = qual  # Phred values, one per base (a list of ints), or None for QUAL `*`
 
     @property
     def mapped(self):
@@ -69,7 +72,8 @@ def read_sam(path):
             f = line.rstrip("\n").split("\t")
             if len(f) < 11:
                 continue
-            records.append(Record(f[0], int(f[1]), f[2], int(f[3]), f[9], _parse_cigar_text(f[5])))
+            qual = None if f[10] == "*" else [ord(c) - 33 for c in f[10]]
+            records.append(Record(f[0], int(f[1]), f[2], int(f[3]), f[9], _parse_cigar_text(f[5]), int(f[4]), qual))
     return _header_sq("\n".join(header_lines)), records
 
 
@@ -101,7 +105,7 @@ def read_bam(path):
         (block_size,) = struct.unpack_from("<i", data, off)
         off += 4
         end = off + block_size
-        ref_id, pos, l_read_name, _mapq, _bin, n_cigar, flag, l_seq, _nref, _npos, _tlen = struct.unpack_from(
+        ref_id, pos, l_read_name, mapq, _bin, n_cigar, flag, l_seq, _nref, _npos, _tlen = struct.unpack_from(
             "<iiBBHHHiiii", data, off
         )
         p = off + 32
@@ -119,8 +123,10 @@ def read_bam(path):
             seq = "".join(chars[:l_seq])
         else:
             seq = "*"
+        p += (l_seq + 1) // 2
+        qual = list(data[p : p + l_seq]) if l_seq and data[p] != 0xFF else None
         rname = names[ref_id] if ref_id >= 0 else "*"
-        records.append(Record(qname, flag, rname, pos + 1, seq, cigars))
+        records.append(Record(qname, flag, rname, pos + 1, seq, cigars, mapq, qual))
         off = end
     return header, records
 
