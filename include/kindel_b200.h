@@ -383,6 +383,48 @@ int kdl_primers_count(const kdl_batch* batch, const kdl_qmask* qmask, const kdl_
 int kdl_primers_apply(const kdl_batch* batch, const kdl_qmask* qmask, const kdl_primers* primers,
                       const uint32_t* scratch, uint32_t* seq4, const kdl_qmask* out_mask, void* stream);
 
+/* K10 (extension: `--mask-overlaps`): each read pair counted once where its mates overlap.  The decode gives every
+ * kept read name_hash (64-bit FNV-1a of QNAME, NUL excluded), mate_start (PNEXT - 1, in ref_start's coordinates) and
+ * pair_role: 1 for a first mate, 2 for a last mate, and 0 unless FLAG has 0x1, none of 0x8 / 0x100 / 0x800, exactly
+ * one of 0x40 / 0x80, and RNEXT is the read's own contig (kdl_bam_fill_mates).
+ *   Pair: two reads with roles 1 and 2 that are the only reads of the batch with pair_role != 0 and that name hash,
+ *   on one contig, each one's ref_start the other's mate_start, neither KDL_HARD.  R1 is the role-1 read, R2 the
+ *   role-2 read.  Anything else (singletons, groups of three or more, inconsistent coordinates) is left alone.
+ *   Covers: R1 covers cursor x (the walk of K7) when it has there an M/=/X base inside SEQ whose nibble is not N --
+ *   after the quality and primer masks, so a masked R1 base covers nothing -- or a D op.
+ *   Masking R2: every M/=/X base of R2 at a covered cursor is masked as min_base_quality masks a base (N in seq4,
+ *   listed in the mask list, its column-4 count taken back by kdl_unmask); a D op at [r, r + n) is dropped when R1
+ *   covers r (its n column-5 counts are taken back, and it is no K7 event); an I op at slot p is dropped when R1
+ *   covers p - 1 and p (its column-6 count is taken back, and its event row reaches no insertion string).  Clips
+ *   and clip columns 7-18 are untouched.  So at a position R1 covers a pair adds at most one count to columns 0-3
+ *   and 5, R1's, and where R1 covers nothing only R2 counts.  Exceptions where R1's information starts or stops: a
+ *   real N in R1 is counted in column 4 and hides nothing; a kept R2 deletion (R1 does not cover its first position)
+ *   also counts where R1 covers later positions of it; an R2 insertion next to an R1 end, N or masked base is kept
+ *   beside an R1 insertion at the same slot.
+ *   Order: decode, upload, K9, kdl_mates_pair, kdl_overlap_count / _apply, the pileup, kdl_unmask, kdl_overlap_untake.
+ *   kdl_mates_pair     K10p.  order[n_order]: the indices of the reads with pair_role != 0, sorted by name_hash
+ *                      (any order among equal hashes).  Writes mate[n_reads]: the R1 of every paired R2, -1 elsewhere.
+ *                      The device sees only the hash: two names that hash alike are one group.
+ *   kdl_overlap_count  K10's count.  scratch: device uint32[kdl_overlap_scratch_words(n_reads)]; its last 8 words are
+ *                      the totals record, read back once: [0] reads in the merged mask list, [1] bases in it, [2] drop
+ *                      rows, [3] pairs, [4] overlap bases, [5] dropped deletions, [6] dropped insertions.
+ *   kdl_overlap_apply  on the same stream after it: writes the merged mask list into out_mask (sized by the totals;
+ *                      NULL when totals[0] == 0) -- per read the sorted union of its entries in qmask (may be NULL)
+ *                      and its overlap bases --, sets R2's overlap nibbles to N in `seq4` (the batch's own, in place,
+ *                      or a copy), and writes drops[n_drops][4] int32 = (slot, len, read, evt) for every dropped op
+ *                      in read, then op order: evt = the I op's row in ins_events, -1 for a D.
+ *   kdl_overlap_untake K10u, after kdl_unmask on the same stream: subtracts each drop row's counts from column 5
+ *                      (slots [slot, slot + len)) or column 6 (slot) of the table.
+ * One thread per read (K10p: per sorted entry, K10u: per drop row); R1 is only read, so no atomics but K10u's. */
+int kdl_mates_pair(const kdl_batch* batch, const uint64_t* name_hash, const int32_t* mate_start,
+                   const uint8_t* pair_role, const int32_t* order, int64_t n_order, int32_t* mate, void* stream);
+int64_t kdl_overlap_scratch_words(int64_t n_reads);
+int kdl_overlap_count(const kdl_batch* batch, const kdl_qmask* qmask, const int32_t* mate, uint32_t* scratch,
+                      void* stream);
+int kdl_overlap_apply(const kdl_batch* batch, const kdl_qmask* qmask, const int32_t* mate, const uint32_t* scratch,
+                      uint32_t* seq4, const kdl_qmask* out_mask, int32_t* drops, int64_t n_drops, void* stream);
+int kdl_overlap_untake(const int32_t* drops, int64_t n_drops, int32_t* counts, int64_t n_slots, void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced
@@ -489,7 +531,8 @@ int kdl_ctx_last_timing(kdl_ctx* ctx, float* h2d_ms, float* kernel_ms, float* d2
  *                    text parser could not carry when the filter would read them.  prepare's info[13] = masked bases,
  *                    info[14] = reads with masked bases
  *   kdl_bam_fill_mask   after fill: the kdl_qmask arrays, read_idx [info[14]], off [info[14] + 1], qpos [info[13]]
- *   kdl_bam_fill_strand after fill (extension): reverse [n_kept], 1 where the kept read's FLAG has 0x10, in read order */
+ *   kdl_bam_fill_strand after fill (extension): reverse [n_kept], 1 where the kept read's FLAG has 0x10, in read order
+ *   kdl_bam_fill_mates  after fill (extension): name_hash / mate_start / pair_role [n_kept] of K10, in read order */
 typedef struct kdl_bam kdl_bam;
 int kdl_bam_open(const char* path, int threads, kdl_bam** out);
 void kdl_bam_close(kdl_bam* h);
@@ -505,6 +548,7 @@ int kdl_bam_fill(kdl_bam* h, int threads, const int64_t* contig_slot, int32_t* r
 int kdl_bam_set_filter(kdl_bam* h, int32_t min_mapq, int32_t exclude_flags, int32_t min_base_quality);
 int kdl_bam_fill_mask(kdl_bam* h, int threads, uint32_t* read_idx, uint32_t* off, uint32_t* qpos);
 int kdl_bam_fill_strand(kdl_bam* h, int threads, uint8_t* reverse);
+int kdl_bam_fill_mates(kdl_bam* h, int threads, uint64_t* name_hash, int32_t* mate_start, uint8_t* pair_role);
 
 #ifdef __cplusplus
 }

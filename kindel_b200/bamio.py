@@ -27,7 +27,8 @@ nibble becomes N (15) in `seq4` before the reads are classified, and its query o
 base column.  A record without qualities (SAM `*`, BAM 0xff) is never masked; with min_base_quality == 0 QUAL is not
 read at all.
 With `strand=True` the batch also keeps each kept read's strand (`reverse`, FLAG & 0x10), which `variants --vcf
---strand` splits the pileup by; it costs nothing when off.
+--strand` splits the pileup by; it costs nothing when off.  With `mates=True` it keeps what `--mask-overlaps` pairs the
+reads by (`name_hash`, `mate_start`, `pair_role`: include/kindel_b200.h K10 has the rule); nothing is decoded when off.
 
 The result is a `ReadBatch` (numpy arrays in host memory) described in include/kindel_b200.h.
 """
@@ -88,6 +89,16 @@ class ReadBatch:
     mask_qpos: np.ndarray = field(default=None)     # uint32 [n_masked]: query offsets, ascending per read
     # strand (extension; `strand=True` at decode): 1 where the read's FLAG has 0x10.  None = not asked for.
     reverse: np.ndarray = field(default=None)       # uint8 [n]
+    # mates (extension; `mates=True` at decode, K10): FNV-1a of QNAME, PNEXT - 1, 1 / 2 = first / last mate of a pair
+    # on one contig (0 otherwise).  None = not asked for.
+    name_hash: np.ndarray = field(default=None)     # uint64 [n]
+    mate_start: np.ndarray = field(default=None)    # int32 [n]
+    pair_role: np.ndarray = field(default=None)     # uint8 [n]
+
+    @property
+    def mates(self):
+        """(name_hash, mate_start, pair_role), or None when the batch was decoded without them."""
+        return None if self.pair_role is None else (self.name_hash, self.mate_start, self.pair_role)
 
     @property
     def n_reads(self) -> int:
@@ -228,7 +239,7 @@ def mask_bases(seq4: np.ndarray, seq_off: np.ndarray, counts: np.ndarray, qpos: 
 
 
 def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_seq, cig_off, cigar, seq4,
-             n_records=0, exotic=None, qual=None, min_base_quality=0, mask=None, reverse=None) -> ReadBatch:
+             n_records=0, exotic=None, qual=None, min_base_quality=0, mask=None, reverse=None, mates=None) -> ReadBatch:
     """Classify reads (simple / tile-eligible complex / hard), lay the complex reads' CIGARs behind their bases,
     detect coordinate order.  All vectorised numpy; shared by the BAM, SAM and synthetic paths.
 
@@ -237,7 +248,8 @@ def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_se
     qual + min_base_quality > 0: concatenated Phred qualities (one byte per base, 0xff = none); the bases below the
     threshold are masked (N in seq4, listed in the mask) BEFORE classification.  mask = (per-read counts, query
     offsets): a mask already applied to `seq4` (re-finalizing a masked batch), carried into the result.
-    reverse: the reads' strand bytes (1 = FLAG & 0x10), carried into the result."""
+    reverse: the reads' strand bytes (1 = FLAG & 0x10), carried into the result.  mates: (name_hash, mate_start,
+    pair_role) of the reads, carried into the result."""
     contig_len = np.ascontiguousarray(contig_len, dtype=np.int32)
     contig_read_off = np.ascontiguousarray(contig_read_off, dtype=np.int64)
     ref_start = np.ascontiguousarray(ref_start, dtype=np.int32)
@@ -350,7 +362,38 @@ def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_se
         n_records=int(n_records), max_simple_len=int(oplen[simple].max()) if simple.any() else 0,
         reach_right=reach_right, reach_left=reach_left, mask_read=mask_read, mask_off=mask_off, mask_qpos=mask_qpos,
         reverse=None if reverse is None else np.ascontiguousarray(reverse, dtype=np.uint8),
+        **_mate_fields(mates),
     )
+
+
+def _mate_fields(mates) -> dict:
+    if mates is None:
+        return {}
+    h, m, r = mates
+    return dict(name_hash=np.ascontiguousarray(h, dtype=np.uint64), mate_start=np.ascontiguousarray(m, dtype=np.int32),
+                pair_role=np.ascontiguousarray(r, dtype=np.uint8))
+
+
+def _mates_at(batch: ReadBatch, idx):
+    return None if batch.mates is None else tuple(a[idx] for a in batch.mates)
+
+
+_FNV_OFFSET, _FNV_PRIME = 0xCBF29CE484222325, 0x100000001B3
+
+
+def name_hash(qname) -> int:
+    """64-bit FNV-1a of a QNAME's bytes (str or bytes), the hash K10 pairs mates by."""
+    h = _FNV_OFFSET
+    for c in qname.encode() if isinstance(qname, str) else bytes(qname):
+        h = ((h ^ c) * _FNV_PRIME) & 0xFFFFFFFFFFFFFFFF
+    return h
+
+
+def pair_role(flag: int, same_contig: bool) -> int:
+    """1 / 2 for the first / last mate of a pair whose mates sit on one contig, else 0 (include/kindel_b200.h K10)."""
+    if not flag & 0x1 or flag & (0x8 | 0x100 | 0x800) or bool(flag & 0x40) == bool(flag & 0x80) or not same_contig:
+        return 0
+    return 1 if flag & 0x40 else 2
 
 
 def _mask_of(batch: ReadBatch, idx: np.ndarray):
@@ -372,7 +415,7 @@ def with_mask(batch: ReadBatch, counts: np.ndarray, qpos: np.ndarray) -> ReadBat
     seq4 = mask_bases(batch.seq4, batch.seq_off, counts, qpos)
     return finalize(batch.contig_names, batch.contig_len, batch.contig_read_off, batch.ref_start, batch.seq_off,
                     batch.seq_len, batch.cig_off, batch.cigar, seq4, n_records=batch.n_records, mask=(counts, qpos),
-                    reverse=batch.reverse)
+                    reverse=batch.reverse, mates=batch.mates)
 
 
 def select_reads(batch: ReadBatch, idx) -> ReadBatch:
@@ -396,7 +439,7 @@ def select_reads(batch: ReadBatch, idx) -> ReadBatch:
         np.arange(int(seq_off[-1])) - np.repeat(seq_off[:-1], words))
     return finalize(batch.contig_names, batch.contig_len, read_off, batch.ref_start[idx], seq_off[:-1], lseq,
                           cig_off, batch.cigar[cig_src], batch.seq4[seq_src], n_records=n, mask=_mask_of(batch, idx),
-                          reverse=None if batch.reverse is None else batch.reverse[idx])
+                          reverse=None if batch.reverse is None else batch.reverse[idx], mates=_mates_at(batch, idx))
 
 
 
@@ -410,8 +453,8 @@ def _ragged_gather(src: np.ndarray, starts: np.ndarray, lens: np.ndarray) -> np.
 
 def merge_batches(batches) -> ReadBatch:
     """All reads of several batches over the SAME contigs as one batch, coordinate-sorted inside every contig
-    (stable: ties keep batch order).  Used to mix synthetic read populations; not a hot path.  The strand bytes are
-    carried when every batch has them."""
+    (stable: ties keep batch order).  Used to mix synthetic read populations; not a hot path.  The strand bytes and the
+    mates are carried when every batch has them."""
     first = batches[0]
     for b in batches[1:]:
         if list(b.contig_names) != list(first.contig_names) or not np.array_equal(b.contig_len, first.contig_len):
@@ -439,9 +482,12 @@ def merge_batches(batches) -> ReadBatch:
     reverse = None
     if all(b.reverse is not None for b in batches):
         reverse = np.concatenate([b.reverse for b in batches])[order]
+    mates = None
+    if all(b.mates is not None for b in batches):
+        mates = tuple(np.concatenate([b.mates[k] for b in batches])[order] for k in range(3))
     return finalize(first.contig_names, first.contig_len, read_off, ref_start[order], base_at[order], lseq[order],
                     cig_off, _ragged_gather(cigar, cig_at[order], nco), bases, n_records=int(order.shape[0]), mask=mask,
-                    reverse=reverse)
+                    reverse=reverse, mates=mates)
 
 
 _SAVE_FIELDS = ("contig_len", "contig_read_off", "contig_slot", "ref_start", "seq_off", "l_seq", "seq_len", "cig_off",
@@ -450,6 +496,7 @@ _SAVE_SCALARS = ("n_slots", "n_events", "reads_sorted", "aligned_bases", "n_reco
                  "reach_left")
 _MASK_FIELDS = ("mask_read", "mask_off", "mask_qpos")  # saved only when the batch has masked bases
 _STRAND_FIELDS = ("reverse",)  # saved only when the batch has its strands
+_MATE_FIELDS = ("name_hash", "mate_start", "pair_role")  # saved only when the batch has its mates
 
 
 def save_batch(directory: str, batch: ReadBatch) -> None:
@@ -457,11 +504,11 @@ def save_batch(directory: str, batch: ReadBatch) -> None:
     import json
 
     os.makedirs(directory, exist_ok=True)
-    for f in _MASK_FIELDS + _STRAND_FIELDS:
+    for f in _MASK_FIELDS + _STRAND_FIELDS + _MATE_FIELDS:
         if os.path.exists(os.path.join(directory, f + ".npy")):
             os.remove(os.path.join(directory, f + ".npy"))
     for f in (_SAVE_FIELDS + (_MASK_FIELDS if batch.n_masked else ())
-              + (_STRAND_FIELDS if batch.reverse is not None else ())):
+              + (_STRAND_FIELDS if batch.reverse is not None else ()) + (_MATE_FIELDS if batch.mates is not None else ())):
         np.save(os.path.join(directory, f + ".npy"), np.ascontiguousarray(getattr(batch, f)))
     meta = {k: (bool(getattr(batch, k)) if k == "reads_sorted" else int(getattr(batch, k))) for k in _SAVE_SCALARS}
     meta["contig_names"] = list(batch.contig_names)
@@ -475,7 +522,7 @@ def load_batch(directory: str, mmap: bool = True) -> ReadBatch:
     with open(os.path.join(directory, "batch.json")) as fh:
         meta = json.load(fh)
     arrays = {f: np.load(os.path.join(directory, f + ".npy"), mmap_mode="r" if mmap else None) for f in _SAVE_FIELDS}
-    for f in _MASK_FIELDS + _STRAND_FIELDS:
+    for f in _MASK_FIELDS + _STRAND_FIELDS + _MATE_FIELDS:
         if os.path.exists(os.path.join(directory, f + ".npy")):
             arrays[f] = np.load(os.path.join(directory, f + ".npy"), mmap_mode="r" if mmap else None)
     return ReadBatch(contig_names=meta.pop("contig_names"), **arrays, **meta)
@@ -563,12 +610,13 @@ def decode_threads() -> int:
 
 
 def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0, exclude_flags: int = 0,
-             min_base_quality: int = 0, strand: bool = False) -> ReadBatch:
+             min_base_quality: int = 0, strand: bool = False, mates: bool = False) -> ReadBatch:
     """.bam -> ReadBatch through the C++ decoder (bam_host.cpp): BGZF inflate, filter, classification and the
     device layout (inline CIGAR blocks included) in threads, no Python per-record or per-array work.
     pinned=True puts the arrays the device consumes into page-locked memory (needs torch + CUDA).
     min_mapq / exclude_flags / min_base_quality: the filters of this module's docstring (extension).  strand=True
-    (extension): also the kept reads' strands, `reverse` (kdl_bam_fill_strand)."""
+    (extension): also the kept reads' strands, `reverse` (kdl_bam_fill_strand).  mates=True (extension): also
+    `name_hash`, `mate_start` and `pair_role` (kdl_bam_fill_mates)."""
     import ctypes as C
 
     filters = check_filters(min_mapq, exclude_flags, min_base_quality)
@@ -634,6 +682,11 @@ def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0,
             mask["reverse"] = np.zeros(n, dtype=np.uint8)
             _ffi.check(lib.kdl_bam_fill_strand(h, threads, mask["reverse"].ctypes.data if n else None),
                        "kdl_bam_fill_strand")
+        if mates:
+            mask.update(name_hash=np.zeros(n, dtype=np.uint64), mate_start=np.zeros(n, dtype=np.int32),
+                        pair_role=np.zeros(n, dtype=np.uint8))
+            ptrs = [mask[f].ctypes.data if n else None for f in _MATE_FIELDS]
+            _ffi.check(lib.kdl_bam_fill_mates(h, threads, *ptrs), "kdl_bam_fill_mates")
     finally:
         lib.kdl_bam_close(h)
     return ReadBatch(
@@ -703,10 +756,10 @@ def _sam_qual(text: str, seq: str) -> bytes:
 
 
 def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0,
-             strand: bool = False) -> ReadBatch:
+             strand: bool = False, mates: bool = False) -> ReadBatch:
     min_mapq, exclude_flags, min_base_quality = check_filters(min_mapq, exclude_flags, min_base_quality)
     header = []
-    groups = {}  # rname -> list of (pos0, cigar words, seq, qualities, reverse)
+    groups = {}  # rname -> list of (pos0, cigar words, seq, qualities, reverse, (name hash, PNEXT - 1, role))
     n_records = 0
     with open(path, "rt") as fh:
         for line in fh:
@@ -733,7 +786,15 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
                 if mapq < min_mapq:
                     continue
             qual = _sam_qual(f[10], seq) if min_base_quality else None
-            g.append((int(f[3]) - 1, parse_cigar_text(f[5]), seq, qual, 1 if flag & 0x10 else 0))
+            mate = None
+            if mates:
+                try:
+                    pnext = int(f[7])
+                except ValueError:
+                    pnext = -1
+                mate = (name_hash(f[0]), pnext - 1 if 0 <= pnext < (1 << 31) else -1,
+                        pair_role(flag, f[6] == "=" or f[6] == rname))
+            g.append((int(f[3]) - 1, parse_cigar_text(f[5]), seq, qual, 1 if flag & 0x10 else 0, mate))
     groups.pop("*", None)  # kindel.py:147-148
     names, lens = _sq_from_text("\n".join(header))
     sq = dict(zip(names, lens))
@@ -741,11 +802,11 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
     for nm in contig_names:
         if nm not in sq:
             raise KeyError(nm)  # refs_lens[ref_id], kindel.py:151
-    ref_start, l_seq, cig_off, cigar, seq_off, seq_parts, quals, rev = [], [], [0], [], [], [], [], []
+    ref_start, l_seq, cig_off, cigar, seq_off, seq_parts, quals, rev, mate_rows = [], [], [0], [], [], [], [], [], []
     read_off = [0]
     words = 0
     for nm in contig_names:
-        for pos0, cig, seq, qual, is_rev in groups[nm]:
+        for pos0, cig, seq, qual, is_rev, mate in groups[nm]:
             ref_start.append(pos0)
             l_seq.append(len(seq))
             cigar.extend(cig)
@@ -756,6 +817,7 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
             seq_parts.append(enc)
             quals.append(qual)
             rev.append(is_rev)
+            mate_rows.append(mate)
         read_off.append(len(ref_start))
     seq4 = np.concatenate(seq_parts) if seq_parts else np.zeros(0, dtype=np.uint32)
     qual = np.frombuffer(b"".join(quals), dtype=np.uint8) if min_base_quality else None
@@ -764,16 +826,20 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
                     np.array(seq_off, dtype=np.int64), np.array(l_seq, dtype=np.int64),
                     np.array(cig_off, dtype=np.int64), np.array(cigar, dtype=np.int64), seq4,
                     n_records=n_records, qual=qual, min_base_quality=min_base_quality,
-                    reverse=np.array(rev, dtype=np.uint8) if strand else None)
+                    reverse=np.array(rev, dtype=np.uint8) if strand else None,
+                    mates=tuple(np.array([m[k] for m in mate_rows], dtype=dt) for k, dt in
+                                enumerate((np.uint64, np.int64, np.uint8))) if mates else None)
 
 
 def read_alignment(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0,
-                   strand: bool = False) -> ReadBatch:
-    """.bam or .sam (by content, not by suffix) -> ReadBatch.  The filters and strand (extensions): see the module
-    docstring."""
+                   strand: bool = False, mates: bool = False) -> ReadBatch:
+    """.bam or .sam (by content, not by suffix) -> ReadBatch.  The filters, strand and mates (extensions): see the
+    module docstring."""
     path = os.fspath(path)
     filters = dict(zip(("min_mapq", "exclude_flags", "min_base_quality"),
                        check_filters(min_mapq, exclude_flags, min_base_quality)), strand=bool(strand))
+    if mates:  # (the keyword only when asked: a reader without it stays as it was)
+        filters["mates"] = True
     with open(path, "rb") as fh:
         magic = fh.read(4)
     if magic[:2] == b"\x1f\x8b" or magic == b"BAM\x01":
@@ -792,8 +858,9 @@ def write_bam(path, contigs, records, header_text=None, level=6):
     """Minimal BAM writer (used for synthetic inputs and test fixtures).
 
     contigs: list of (name, length).  records: iterable of tuples
-    (ref_id, pos0, flag, cigar_words, seq_text[, qname[, mapq[, qual]]]): mapq defaults to 60, qual (Phred values,
-    bytes or a sequence of ints, one per base; None = none, stored as 0xff) to none.  One BGZF block per ~60 KB + EOF
+    (ref_id, pos0, flag, cigar_words, seq_text[, qname[, mapq[, qual[, next_ref_id, next_pos0]]]]): mapq defaults to
+    60, qual (Phred values, bytes or a sequence of ints, one per base; None = none, stored as 0xff) to none, RNEXT /
+    PNEXT (the mate's reference id and 0-based position) to -1.  One BGZF block per ~60 KB + EOF
     block.
     """
     if header_text is None:
@@ -817,7 +884,10 @@ def write_bam(path, contigs, records, header_text=None, level=6):
         qual = bytes(rec[7]) if len(rec) > 7 and rec[7] is not None else b"\xff" * l_seq
         if len(qual) != l_seq:
             raise ValueError("record %d: %d qualities for %d bases" % (k, len(qual), l_seq))
-        core = struct.pack("<iiBBHHHiiii", ref_id, pos0, len(qname), mapq, 4680, len(cig), flag, l_seq, -1, -1, 0)
+        next_ref = int(rec[8]) if len(rec) > 8 and rec[8] is not None else -1
+        next_pos = int(rec[9]) if len(rec) > 9 and rec[9] is not None else -1
+        core = struct.pack("<iiBBHHHiiii", ref_id, pos0, len(qname), mapq, 4680, len(cig), flag, l_seq, next_ref, next_pos,
+                           0)
         data = core + qname + struct.pack("<%dI" % len(cig), *cig) + packed + qual
         body += struct.pack("<i", len(data)) + data
     with open(path, "wb") as fh:

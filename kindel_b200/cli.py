@@ -7,7 +7,8 @@ extension one FASTQ record per contig instead),
 `variants` (in the reference's README only) is an extension, see kindel.variants; its `--vcf` writes a sites-only VCF
 (kindel.variants_vcf), against a FASTA with `--reference`, with per-strand counts and a strand odds ratio with
 `--strand` / `--max-sor`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
-bases of every read before the pileup (kindel_b200/primers.py).
+bases of every read before the pileup (kindel_b200/primers.py); `--mask-overlaps` counts each read pair once where
+its mates overlap (include/kindel_b200.h K10).
 argh derived the flags from the function signatures (first letter as short option unless two
 parameters share it); argparse spells the same set out.  Note the CLI default `--min-overlap 7`
 (cli.py:13) differs from the API default 9 (kindel.py:492), as in the reference.
@@ -100,6 +101,10 @@ def _add_filters(p):
     p.add_argument("--primers", default=None, metavar="BED",
                    help="mask the bases of each read that lie in an amplicon primer of this BED (plain or gzip): read "
                         "as N, not counted")
+    # extension: each read pair counted once where its mates overlap, off by default
+    p.add_argument("--mask-overlaps", action="store_true",
+                   help="count each read pair once where its mates overlap: the second mate's bases, deletions and "
+                        "insertions there are not counted where the first mate has information")
 
 
 def _iupac_threshold(text: str) -> float:
@@ -118,6 +123,8 @@ def _filters(a) -> dict:
     out = dict(min_base_quality=a.min_base_quality, min_mapq=a.min_mapq, exclude_flags=a.exclude_flags)
     if a.primers is not None:  # (the keyword only when given: every call without it stays as it was)
         out["primers"] = a.primers
+    if a.mask_overlaps:
+        out["mask_overlaps"] = True
     return out
 
 

@@ -15,6 +15,7 @@
 #include "variants.cu"
 #include "select.cu"
 #include "primers.cu"
+#include "mates.cu"
 
 namespace {
 
@@ -648,6 +649,80 @@ int kdl_primers_apply(const kdl_batch* batch, const kdl_qmask* qmask, const kdl_
     const long long n_blocks = primer_blocks(batch->n_reads);
     KDL_LAUNCH(kdl::primers_scatter_kernel, (unsigned)n_blocks, kdl::P_THREADS, 0, (cudaStream_t)stream, *batch, q,
                *primers, scratch, n_blocks, seq4, om);
+    return check_launch();
+}
+
+static long long overlap_blocks(int64_t n_reads) { return n_reads / kdl::M_THREADS + 1; }
+
+int kdl_mates_pair(const kdl_batch* batch, const uint64_t* name_hash, const int32_t* mate_start,
+                   const uint8_t* pair_role, const int32_t* order, int64_t n_order, int32_t* mate, void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (n_order < 0 || n_order > batch->n_reads || batch->n_reads >= (int64_t)INT32_MAX ||
+        (batch->n_reads > 0 && !mate) || (n_order > 0 && (!name_hash || !mate_start || !pair_role || !order)))
+        return KDL_ERR_INVALID_ARG;
+    if (batch->n_reads == 0) return KDL_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const long long n = batch->n_reads;
+    const long long grid = (n + kdl::M_THREADS - 1) / kdl::M_THREADS;
+    KDL_LAUNCH(kdl::mates_clear_kernel, (unsigned)(grid < 4096 ? grid : 4096), kdl::M_THREADS, 0, st, mate, n);
+    if ((rc = check_launch()) != KDL_OK || n_order < 2) return rc;
+    KDL_LAUNCH(kdl::mates_pair_kernel, (unsigned)((n_order + kdl::M_THREADS - 1) / kdl::M_THREADS), kdl::M_THREADS, 0,
+               st, *batch, name_hash, mate_start, pair_role, order, n_order, mate);
+    return check_launch();
+}
+
+static int overlap_args(const kdl_batch* batch, const kdl_qmask* qmask, const int32_t* mate, kdl_qmask* q) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if ((rc = select_qmask(qmask, q)) != KDL_OK) return rc;
+    if ((batch->n_reads > 0 && !mate) || batch->n_reads >= (int64_t)INT32_MAX) return KDL_ERR_INVALID_ARG;
+    return KDL_OK;
+}
+
+int64_t kdl_overlap_scratch_words(int64_t n_reads) {
+    return n_reads < 0 ? 0 : (int64_t)kdl::M_NROW * (overlap_blocks(n_reads) + 1) + kdl::M_TOTALS;
+}
+
+int kdl_overlap_count(const kdl_batch* batch, const kdl_qmask* qmask, const int32_t* mate, uint32_t* scratch,
+                      void* stream) {
+    kdl_qmask q;
+    int rc = overlap_args(batch, qmask, mate, &q);
+    if (rc != KDL_OK) return rc;
+    if (!scratch) return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = overlap_blocks(batch->n_reads);
+    cudaStream_t st = (cudaStream_t)stream;
+    KDL_LAUNCH(kdl::overlap_sums_kernel, (unsigned)n_blocks, kdl::M_THREADS, 0, st, *batch, q, mate, scratch, n_blocks);
+    if ((rc = check_launch()) != KDL_OK) return rc;
+    for (int k = 0; k < kdl::M_NSCAN; ++k) {
+        KDL_LAUNCH(kdl::assemble_scan_sums_kernel, 1, kdl::A_THREADS, 0, st, scratch + (size_t)k * (n_blocks + 1),
+                   n_blocks);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+    }
+    KDL_LAUNCH(kdl::overlap_totals_kernel, 1, kdl::M_THREADS, 0, st, scratch, n_blocks);
+    return check_launch();
+}
+
+int kdl_overlap_apply(const kdl_batch* batch, const kdl_qmask* qmask, const int32_t* mate, const uint32_t* scratch,
+                      uint32_t* seq4, const kdl_qmask* out_mask, int32_t* drops, int64_t n_drops, void* stream) {
+    kdl_qmask q, om;
+    int rc = overlap_args(batch, qmask, mate, &q);
+    if (rc != KDL_OK) return rc;
+    if ((rc = select_qmask(out_mask, &om)) != KDL_OK) return rc;
+    if (!scratch || (batch->n_reads > 0 && !seq4) || (om.n_reads > 0 && om.n_bases > 0 && !om.qpos) || n_drops < 0 ||
+        (n_drops > 0 && !drops))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = overlap_blocks(batch->n_reads);
+    KDL_LAUNCH(kdl::overlap_scatter_kernel, (unsigned)n_blocks, kdl::M_THREADS, 0, (cudaStream_t)stream, *batch, q,
+               mate, scratch, n_blocks, seq4, om, drops, n_drops);
+    return check_launch();
+}
+
+int kdl_overlap_untake(const int32_t* drops, int64_t n_drops, int32_t* counts, int64_t n_slots, void* stream) {
+    if (n_drops < 0 || n_slots <= 0 || !counts || (n_drops > 0 && !drops)) return KDL_ERR_INVALID_ARG;
+    if (n_drops == 0) return KDL_OK;
+    KDL_LAUNCH(kdl::overlap_untake_kernel, (unsigned)((n_drops + kdl::M_THREADS - 1) / kdl::M_THREADS),
+               kdl::M_THREADS, 0, (cudaStream_t)stream, drops, n_drops, counts, n_slots);
     return check_launch();
 }
 

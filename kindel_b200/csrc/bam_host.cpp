@@ -493,27 +493,37 @@ int sam_text_to_bam(const uint8_t* p, size_t n, Pool& pool, int threads, std::ve
                     else odd_fields |= 2;
                 }
             }
+            // QNAME, RNEXT and PNEXT travel as BAM keeps them (the mates of `--mask-overlaps` read them); an RNEXT
+            // without @SQ line or a PNEXT that is no integer in 0..2^31-1 says "no mate on this contig": -1
+            const int64_t l_name = fe(0) - f[0];
+            if (l_name > 254) { failed = 1; return; }
+            int32_t next_ref = -1, next_pos = -1;
+            if (fe(6) - f[6] == 1 && *f[6] == '=') next_ref = ref_id;
+            else if (ref_id_of(f[6], fe(6)) >= 0) next_ref = ref_id_of(f[6], fe(6));
+            int64_t pnext;
+            if (parse_int(f[7], fe(7), &pnext) && pnext >= 0 && pnext <= INT32_MAX) next_pos = (int32_t)(pnext - 1);
             const int64_t seq_bytes = (l_seq + 1) / 2;
-            const int64_t block_size = 32 + 1 + 4 * (int64_t)ops.size() + seq_bytes + l_seq;
+            const int64_t block_size = 32 + (l_name + 1) + 4 * (int64_t)ops.size() + seq_bytes + l_seq;
             if (block_size > (1ll << 28)) { failed = 1; return; }
             const size_t base = o.size();
             o.resize(base + 4 + (size_t)block_size);
             uint8_t* w = o.data() + base;
-            const int32_t bs32 = (int32_t)block_size, pos0 = (int32_t)(pos - 1), lseq32 = (int32_t)l_seq, m1 = -1, zero = 0;
+            const int32_t bs32 = (int32_t)block_size, pos0 = (int32_t)(pos - 1), lseq32 = (int32_t)l_seq, zero = 0;
             const uint16_t ncig = (uint16_t)ops.size(), flag16 = (uint16_t)flag, bin = 4680;
             std::memcpy(w, &bs32, 4);
             std::memcpy(w + 4, &ref_id, 4);
             std::memcpy(w + 8, &pos0, 4);
-            w[12] = 1; w[13] = (uint8_t)mapq;           // l_read_name (the NUL only), mapq
+            w[12] = (uint8_t)(l_name + 1); w[13] = (uint8_t)mapq;  // l_read_name (with its NUL), mapq
             std::memcpy(w + 14, &bin, 2);
             std::memcpy(w + 16, &ncig, 2);
             std::memcpy(w + 18, &flag16, 2);
             std::memcpy(w + 20, &lseq32, 4);
-            std::memcpy(w + 24, &m1, 4);
-            std::memcpy(w + 28, &m1, 4);
+            std::memcpy(w + 24, &next_ref, 4);
+            std::memcpy(w + 28, &next_pos, 4);
             std::memcpy(w + 32, &zero, 4);
-            w[36] = 0;                                  // read name ""
-            uint8_t* q = w + 37;
+            if (l_name) std::memcpy(w + 36, f[0], (size_t)l_name);
+            w[36 + l_name] = 0;                                   // read name
+            uint8_t* q = w + 37 + l_name;
             if (!ops.empty()) std::memcpy(q, ops.data(), 4 * ops.size());
             q += 4 * ops.size();
             for (int64_t k = 0; k < l_seq; k += 2) {
@@ -1100,6 +1110,37 @@ int kdl_bam_fill_strand(kdl_bam* h, int threads, uint8_t* reverse) {
             const int64_t off_i = h->rec_off[(size_t)i];
             parse_record(d + off_i, h->rec_off[(size_t)i + 1] - off_i, &r);
             reverse[cr[(size_t)r.ref_id]++] = (r.flag & 0x10u) ? 1 : 0;
+        }
+    });
+    return KDL_OK;
+}
+
+// The mates of the last prepare's kept reads, in read order (K10, include/kindel_b200.h): name_hash[k] = 64-bit FNV-1a
+// of QNAME (NUL excluded), mate_start[k] = PNEXT - 1 (BAM next_pos), pair_role[k] = 1 / 2 for a first / last mate of a
+// pair whose FLAG has 0x1, none of 0x8 / 0x100 / 0x800, exactly one of 0x40 / 0x80 and next_refID == refID, else 0.
+int kdl_bam_fill_mates(kdl_bam* h, int threads, uint64_t* name_hash, int32_t* mate_start, uint8_t* pair_role) {
+    if (!h || !h->prepared || (h->n_kept > 0 && (!name_hash || !mate_start || !pair_role))) return KDL_ERR_INVALID_ARG;
+    const uint8_t* d = h->dptr;
+    const int32_t n_ref = (int32_t)h->ref_name.size();
+    const int64_t n_tasks = (int64_t)h->chunk_lo.size() - 1;
+    h->pool->run(n_tasks, threads, [&](int64_t t, int) {
+        std::vector<int64_t> cr(h->cur_read.begin() + t * n_ref, h->cur_read.begin() + (t + 1) * n_ref);
+        RecView r;
+        for (int64_t i = h->chunk_lo[(size_t)t]; i < h->chunk_lo[(size_t)t + 1]; ++i) {
+            if (h->cls[(size_t)i].cls == CLS_DROP) continue;
+            const int64_t off_i = h->rec_off[(size_t)i];
+            parse_record(d + off_i, h->rec_off[(size_t)i + 1] - off_i, &r);
+            const int64_t k = cr[(size_t)r.ref_id]++;
+            const uint8_t* q = d + off_i + 4;  // the record behind block_size
+            const uint32_t l_name = q[8];
+            uint64_t hv = 0xcbf29ce484222325ull;
+            for (uint32_t c = 0; c < l_name && q[32 + c]; ++c) hv = (hv ^ q[32 + c]) * 0x100000001b3ull;
+            name_hash[k] = hv;
+            mate_start[k] = rd_i32(q + 24);
+            const uint32_t f = r.flag;
+            const bool ends = ((f & 0x40u) != 0) != ((f & 0x80u) != 0);
+            const bool ok = (f & 0x1u) && !(f & (0x8u | 0x100u | 0x800u)) && ends && rd_i32(q + 20) == r.ref_id;
+            pair_role[k] = ok ? ((f & 0x40u) ? 1 : 2) : 0;
         }
     });
     return KDL_OK;

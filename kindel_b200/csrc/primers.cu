@@ -159,6 +159,64 @@ __device__ __forceinline__ void own_mask(const kdl_qmask& q, long long r, uint32
     }
 }
 
+// The merge of a read's run [m0, m1) of the batch's own mask list with new bases given as ascending, disjoint query
+// ranges -- the sorted union, each base once.  Shared by K9 (primer bases) and K10 (mates.cu: overlap bases).
+// MergeCount sizes it: after the ranges, merged() = the bases of the union.
+struct MergeCount {
+    const uint32_t* __restrict__ own;
+    uint32_t m0, k, m1, added, same;
+
+    __device__ __forceinline__ MergeCount(const kdl_qmask& q, uint32_t b0, uint32_t b1)
+        : own(q.qpos), m0(b0), k(b0), m1(b1), added(0), same(0) {}
+    __device__ __forceinline__ void add(long long q0, long long q1) {
+        added += (uint32_t)(q1 - q0);
+        while (k < m1 && (long long)own[k] < q0) ++k;
+        while (k < m1 && (long long)own[k] < q1) { ++same; ++k; }
+    }
+    __device__ __forceinline__ uint32_t merged() const { return added + (m1 - m0) - same; }
+};
+
+// MergeWrite writes it from qpos[o] on (writes bounded by cap) and sets the new bases' nibbles to N in `words`, the
+// read's own words of seq4; finish() after the last range.
+struct MergeWrite {
+    const uint32_t* __restrict__ own;
+    uint32_t k, m1;
+    uint32_t* __restrict__ qpos;
+    long long o, cap;
+
+    __device__ __forceinline__ MergeWrite(const kdl_qmask& q, uint32_t b0, uint32_t b1, uint32_t* out, long long at,
+                                          long long n_out)
+        : own(q.qpos), k(b0), m1(b1), qpos(out), o(at), cap(n_out) {}
+    __device__ __forceinline__ void put(long long qq) {
+        if (o < cap) qpos[o] = (uint32_t)qq;
+        ++o;
+    }
+    __device__ __forceinline__ void add(long long q0, long long q1, uint32_t* words) {
+        while (k < m1 && (long long)own[k] < q0) put(own[k++]);
+        for (long long qq = q0; qq < q1; ++qq) {
+            put(qq);
+            words[qq >> 3] |= 0xFu << (28 - 4 * (int)(qq & 7));  // N
+        }
+        while (k < m1 && (long long)own[k] < q1) ++k;  // already listed
+    }
+    __device__ __forceinline__ void finish() {
+        while (k < m1) put(own[k++]);
+    }
+};
+
+// read r's entry orr of the merged list `om`, its bases from ob on: read_idx / off written, the writer returned.
+// Writes are bounded by om's counts (the totals), so a wrong count stays in bounds.
+__device__ __forceinline__ MergeWrite merged_list_entry(const kdl_qmask& q, const kdl_qmask& om, long long r,
+                                                        long long orr, long long ob) {
+    if (orr < om.n_reads) {
+        const_cast<uint32_t*>(om.read_idx)[orr] = (uint32_t)r;
+        const_cast<uint32_t*>(om.off)[orr] = (uint32_t)ob;
+    }
+    uint32_t m0, m1;
+    own_mask(q, r, &m0, &m1);
+    return MergeWrite(q, m0, m1, const_cast<uint32_t*>(om.qpos), ob, om.n_bases);
+}
+
 // read r's share of the four rows
 __device__ __forceinline__ void primer_item(const kdl_batch& b, const kdl_qmask& q, const kdl_primers& p, long long r,
                                             uint32_t (&v)[P_NROW]) {
@@ -167,13 +225,10 @@ __device__ __forceinline__ void primer_item(const kdl_batch& b, const kdl_qmask&
     if (r >= b.n_reads) return;
     uint32_t m0, m1;
     own_mask(q, r, &m0, &m1);
-    uint32_t n_p = 0, overlap = 0, k = m0;
-    primer_ranges(b, p, r, [&](long long q0, long long q1) {
-        n_p += (uint32_t)(q1 - q0);
-        while (k < m1 && (long long)q.qpos[k] < q0) ++k;
-        while (k < m1 && (long long)q.qpos[k] < q1) { ++overlap; ++k; }
-    });
-    v[P_MBASES] = n_p + (m1 - m0) - overlap;
+    MergeCount mc(q, m0, m1);
+    primer_ranges(b, p, r, [&](long long q0, long long q1) { mc.add(q0, q1); });
+    const uint32_t n_p = mc.added;
+    v[P_MBASES] = mc.merged();
     v[P_MREADS] = v[P_MBASES] ? 1u : 0u;
     v[P_PREADS] = n_p ? 1u : 0u;
     v[P_PBASES] = n_p;
@@ -240,36 +295,15 @@ primers_scatter_kernel(kdl_batch b, kdl_qmask q, kdl_primers p, const uint32_t* 
     cta_scan_vec(t, tot);
     long long ob = (long long)t[0] + scratch[(size_t)P_MBASES * (n_blocks + 1) + blockIdx.x];
     long long orr = (long long)t[1] + scratch[(size_t)P_MREADS * (n_blocks + 1) + blockIdx.x];
-    uint32_t* __restrict__ read_idx = const_cast<uint32_t*>(om.read_idx);
-    uint32_t* __restrict__ off = const_cast<uint32_t*>(om.off);
-    uint32_t* __restrict__ qpos = const_cast<uint32_t*>(om.qpos);
-    if (blockIdx.x == 0 && threadIdx.x == 0 && om.n_reads > 0) off[om.n_reads] = (uint32_t)om.n_bases;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && om.n_reads > 0) const_cast<uint32_t*>(om.off)[om.n_reads] = (uint32_t)om.n_bases;
 #pragma unroll
     for (int j = 0; j < P_PER; ++j) {
         if (!n[j]) continue;
         const long long r = r0 + j;
-        if (orr < om.n_reads) {
-            read_idx[orr] = (uint32_t)r;
-            off[orr] = (uint32_t)ob;
-        }
-        uint32_t m0, m1;
-        own_mask(q, r, &m0, &m1);
-        uint32_t k = m0;
-        long long o = ob;
-        auto out = [&](long long qq) {
-            if (o < om.n_bases) qpos[o] = (uint32_t)qq;
-            ++o;
-        };
+        MergeWrite mw = merged_list_entry(q, om, r, orr, ob);
         uint32_t* words = seq4 + (size_t)b.seq_off[r];  // (may be b.seq4 itself: the CIGAR words are only read)
-        primer_ranges(b, p, r, [&](long long q0, long long q1) {
-            while (k < m1 && (long long)q.qpos[k] < q0) out(q.qpos[k++]);
-            for (long long qq = q0; qq < q1; ++qq) {
-                out(qq);
-                words[qq >> 3] |= 0xFu << (28 - 4 * (int)(qq & 7));  // N
-            }
-            while (k < m1 && (long long)q.qpos[k] < q1) ++k;  // already listed
-        });
-        while (k < m1) out(q.qpos[k++]);
+        primer_ranges(b, p, r, [&](long long q0, long long q1) { mw.add(q0, q1, words); });
+        mw.finish();
         ob += n[j];
         ++orr;
     }

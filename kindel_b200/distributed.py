@@ -102,6 +102,18 @@ def merge_events(per_rank_events, per_rank_index) -> np.ndarray:
     return allrows[np.argsort(allrows[:, 1], kind="stable")]
 
 
+def shard_drops(drops, idx) -> np.ndarray:
+    """The rows of K10's drop list (int32 [m, 4] = slot, len, read, event row; global read numbers) whose read is in
+    the shard `idx` (ascending global indices), with the shard's own read numbers."""
+    drops = np.asarray(drops, dtype=np.int32).reshape(-1, 4)
+    idx = np.asarray(idx, dtype=np.int64)
+    at = np.searchsorted(idx, drops[:, 2].astype(np.int64)).clip(max=max(idx.shape[0] - 1, 0))
+    mine = (idx.shape[0] > 0) & (idx[at] == drops[:, 2]) if idx.shape[0] else np.zeros(drops.shape[0], dtype=bool)
+    out = drops[mine].copy()
+    out[:, 2] = at[mine]
+    return out
+
+
 def footprint(batch: bamio.ReadBatch, align: int = 4):
     """[lo, hi) slot range outside of which this shard's count table is certainly zero.
     Conservative: every read may touch from (start - its soft clips) to (start + reference span +
@@ -265,9 +277,10 @@ class ShardedConsensus:
 
     primers (extension): a primers.PrimerArrays over the shard's contigs; K9 then masks the shard's primer bases on
     the device right after the upload, before the first pileup (the rule is per read: every shard's masks are those
-    of the whole batch)."""
+    of the whole batch).  drops (extension: `--mask-overlaps`): the shard's rows of K10's drop list (shard_drops),
+    whose deletion and insertion counts every pileup takes back; the shard's overlap bases are already masked."""
 
-    def __init__(self, shard: bamio.ReadBatch, device, mode: str = "fused", group=None, primers=None):
+    def __init__(self, shard: bamio.ReadBatch, device, mode: str = "fused", group=None, primers=None, drops=None):
         import torch
         import torch.distributed as dist
 
@@ -281,6 +294,11 @@ class ShardedConsensus:
         self.dbatch = engine.upload(shard, device)
         if primers is not None:
             self.dbatch = engine.mask_primers(self.dbatch, primers)
+        if drops is not None:  # K10's drop rows of this shard's R2 reads: every pileup takes them back (K10u)
+            import dataclasses
+
+            self.dbatch = dataclasses.replace(self.dbatch, drops=torch.from_numpy(
+                np.ascontiguousarray(drops, dtype=np.int32).reshape(-1, 4)).to(device))
         self.lib = _ffi.load()
         self.epoch = 0
         if mode in ("peer", "fused"):
@@ -454,7 +472,9 @@ def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode:
         shard = select_reads(batch, idx)
         pth = os.path.join(workdir, "primers.npz")
         primers = load_arrays(pth) if os.path.exists(pth) else None
-        sc = ShardedConsensus(shard, dev, mode=mode, primers=primers)
+        pth = os.path.join(workdir, "drops.npy")
+        drops = shard_drops(np.load(pth), idx) if os.path.exists(pth) else None
+        sc = ShardedConsensus(shard, dev, mode=mode, primers=primers, drops=drops)
         calls = sc.step(min_depth, iupac_threshold=iupac_threshold)
         # data errors: the reference raises at the FIRST offending record in iteration order -- every rank
         # reports its first one (global read number), the parent re-raises the smallest
@@ -494,14 +514,16 @@ def _api_worker(rank: int, world: int, workdir: str, port: int, min_depth, mode:
 
 
 def run_sharded(batch: bamio.ReadBatch, devices: int, min_depth=1, mode: str = "fused", plan: str = None,
-                iupac_threshold=None, primers=None):
+                iupac_threshold=None, primers=None, drops=None):
     """Pileup + vote of `batch` over `devices` GPUs of this node: one process per GPU (torch.distributed, NCCL for
     the plumbing, the fused peer-memory exchange on the data path), whole contigs per rank when there are enough
     of them, else contiguous blocks of every contig's sorted reads.  Returns (calls uint8[n_slots], counts
     int32[19, n_slots], derived int32[5, n_slots], events int32[n_events, 4]) in host memory -- bit-identical to
     one GPU -- or raises the reference's IndexError / KeyError.  iupac_threshold (extension): the IUPAC vote, see
     kindel.bam_to_consensus.  primers (extension): primers.PrimerArrays of the batch's contigs, saved beside the batch;
-    every rank masks its shard's primer bases (ShardedConsensus)."""
+    every rank masks its shard's primer bases (ShardedConsensus).  drops (extension: `--mask-overlaps`): K10's drop rows
+    of the batch (int32 [m, 4], global read numbers), its overlap bases already masked in `batch`; every rank takes back
+    its own rows after its pileup."""
     import json
     import shutil
     import tempfile
@@ -525,6 +547,8 @@ def run_sharded(batch: bamio.ReadBatch, devices: int, min_depth=1, mode: str = "
         bamio.save_batch(os.path.join(workdir, "batch"), batch)
         if primers is not None:
             save_arrays(os.path.join(workdir, "primers.npz"), primers)
+        if drops is not None:
+            np.save(os.path.join(workdir, "drops.npy"), np.ascontiguousarray(drops, dtype=np.int32).reshape(-1, 4))
         try:
             mp.spawn(_api_worker, args=(devices, workdir, _free_port(), min_depth, mode, plan, iupac_threshold),
                      nprocs=devices, join=True)

@@ -16,10 +16,13 @@ implementation behind these functions: without a CUDA device they raise.
     deletion_alleles(dbatch, counts, ...)  K7 + grouping: the deletion alleles against a reference (extension)
     select_reads(dbatch, keep) K8: the sub-batch of the kept reads, built on the device (extension)
     mask_primers(dbatch, arrays)  K9: the batch with its amplicon primer bases masked (extension)
+    mask_overlaps(dbatch)      K10p + K10: the batch with its read pairs' second mates masked where the first covers
+                               (extension); pileup then runs K10u
 """
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import math
 from dataclasses import dataclass
 
@@ -52,6 +55,10 @@ class DeviceBatch:
     struct: _ffi.KdlBatch
     qmask: _ffi.KdlQmask = None  # the batch's masked bases (min_base_quality); None when there are none
     primer_masked: tuple = (0, 0)  # (reads, bases) K9 masked in it (mask_primers)
+    # K10 (mask_overlaps): the dropped R2 ops, int32 [m, 4] = (slot, len, read, event row or -1 for a D), whose counts
+    # pileup takes back (K10u); None when off
+    drops: torch.Tensor = None
+    overlap_masked: tuple = None  # (pairs, bases, deletions, insertions) K10 masked in it; None when off
 
     @property
     def n_slots(self) -> int:
@@ -205,7 +212,7 @@ def _tile_align(lo: int, hi: int, n_slots: int):
 
 def pileup(dbatch: DeviceBatch, counts: torch.Tensor = None, check: bool = True, table: CountTable = None,
            slot_range=None):
-    """K1 (+ K1q when the batch has masked bases).  Returns (counts int32[19, n_slots], events int32[n_events, 4]) on
+    """K1 (+ K1q when the batch has masked bases, + K10u when it has dropped mate ops).  Returns (counts int32[19, n_slots], events int32[n_events, 4]) on
     the device.
 
     counts=<tensor>  accumulate into a table the caller zeroed (several batches / shards may add up).
@@ -251,6 +258,11 @@ def pileup(dbatch: DeviceBatch, counts: torch.Tensor = None, check: bool = True,
             rc = lib.kdl_unmask(C.byref(dbatch.struct), C.byref(dbatch.qmask), counts.data_ptr(), n_slots,
                                 _stream_ptr(dev))
             _ffi.check(rc, "kdl_unmask")
+        if dbatch.drops is not None and dbatch.drops.shape[0]:
+            # K10u: only columns 5 and 6 of complex reads, whose sectors the pileup already marked dirty
+            rc = lib.kdl_overlap_untake(dbatch.drops.data_ptr(), int(dbatch.drops.shape[0]), counts.data_ptr(), n_slots,
+                                        _stream_ptr(dev))
+            _ffi.check(rc, "kdl_overlap_untake")
         if check and int(flag[0].item()) != 0:
             diagnose_and_raise(dbatch)
     return counts, events[: dbatch.host.n_events]
@@ -532,7 +544,12 @@ def select_reads(dbatch: DeviceBatch, keep: torch.Tensor) -> DeviceBatch:
         q = make_qmask(host, ptr) if n_mr else None
         rc = lib.kdl_select_scatter(*args, C.byref(s), C.byref(q) if q is not None else None, _stream_ptr(dev))
         _ffi.check(rc, "kdl_select_scatter")
-    return DeviceBatch(host=host, device=dev, tensors=t, struct=s, qmask=q)
+        drops = None
+        if dbatch.drops is not None:  # the kept reads' drop rows, their read numbers those of the sub-batch
+            kept = keep[dbatch.drops[:, 2].long()] != 0
+            drops = dbatch.drops[kept].clone()
+            drops[:, 2] = (torch.cumsum(keep.to(torch.int64), 0) - 1).index_select(0, drops[:, 2].long()).to(torch.int32)
+    return DeviceBatch(host=host, device=dev, tensors=t, struct=s, qmask=q, drops=drops)
 
 
 _PRIMER_TOTALS = 8  # words of K9's totals record (include/kindel_b200.h)
@@ -555,7 +572,8 @@ def mask_primers(dbatch: DeviceBatch, arrays) -> DeviceBatch:
     in place -- the upload of one run, which nothing else reads -- and the result shares every tensor with `dbatch`
     except the mask list, the union of the batch's own and the primer bases.  So `dbatch` itself must not be piled
     after this call.  One 32-byte read-back sizes the list; a batch without a primer base comes back as it is.  The
-    host ReadBatch is never touched.  `primer_masked` of the result = (reads, bases) masked by the primers."""
+    host ReadBatch is never touched.  `primer_masked` of the result = (reads, bases) masked by the primers.  A batch
+    that already carries drop rows (mask_overlaps) keeps them."""
     lib = _ffi.load()
     dev = dbatch.device
     n = int(dbatch.struct.n_reads)
@@ -585,7 +603,86 @@ def mask_primers(dbatch: DeviceBatch, arrays) -> DeviceBatch:
         rc = lib.kdl_primers_apply(*args, int(dbatch.tensors["seq4"].data_ptr()), C.byref(q), _stream_ptr(dev))
         _ffi.check(rc, "kdl_primers_apply")
     return DeviceBatch(host=dbatch.host, device=dev, tensors=tensors, struct=dbatch.struct, qmask=q,
-                       primer_masked=(n_pr, n_pb))
+                       primer_masked=(n_pr, n_pb), drops=dbatch.drops, overlap_masked=dbatch.overlap_masked)
+
+
+_OVERLAP_TOTALS = 8  # words of K10's totals record (include/kindel_b200.h)
+
+
+def pair_mates(dbatch: DeviceBatch, order: torch.Tensor = None) -> torch.Tensor:
+    """K10p (extension: `--mask-overlaps`): int32[n_reads] on the device, the R1 of every paired R2 and -1 elsewhere
+    (include/kindel_b200.h has the rule).  The reads with pair_role != 0 are compacted and sorted by name hash here
+    (torch, on the device); `order` gives that sorted index list instead.  Needs a host batch decoded with mates."""
+    h = dbatch.host
+    if getattr(h, "mates", None) is None:
+        raise ValueError("mask_overlaps needs the reads' mates: decode the batch with mates=True")
+    lib = _ffi.load()
+    dev = dbatch.device
+    n = h.n_reads
+    with torch.cuda.device(dev):
+        t_hash = torch.from_numpy(np.ascontiguousarray(h.name_hash, dtype=np.uint64).view(np.int64)).to(dev)
+        t_mate = torch.from_numpy(np.ascontiguousarray(h.mate_start, dtype=np.int32)).to(dev)
+        t_role = torch.from_numpy(np.ascontiguousarray(h.pair_role, dtype=np.uint8)).to(dev)
+        if order is None:
+            idx = torch.nonzero(t_role, as_tuple=True)[0]
+            order = idx.index_select(0, torch.sort(t_hash.index_select(0, idx), stable=True)[1])
+        order = order.to(dev, torch.int32).contiguous()
+        mate = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        rc = lib.kdl_mates_pair(C.byref(dbatch.struct), t_hash.data_ptr(), t_mate.data_ptr(), t_role.data_ptr(),
+                                order.data_ptr(), int(order.numel()), mate.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_mates_pair")
+    return mate[:n]
+
+
+def mask_overlaps(dbatch: DeviceBatch, mate: torch.Tensor = None) -> DeviceBatch:
+    """K10 (extension: `--mask-overlaps`): the batch with every read pair's second mate (R2) masked where the first
+    (R1) covers it, as min_base_quality masks a base, and the drop rows of R2's deletions and insertions there, whose
+    counts pileup takes back after K1q (K10u).  include/kindel_b200.h has the rule.
+
+    mate: K10p's result (pair_mates runs when it is None).  Like mask_primers, the nibbles are written into the batch's
+    own device seq4 -- run it after mask_primers, so that primer-masked R1 bases cover nothing -- and the result shares
+    every tensor with `dbatch` but the mask list; `dbatch` must not be piled after this call.  One 32-byte read-back
+    sizes the outputs.  `overlap_masked` of the result = (pairs, bases, deletions, insertions)."""
+    lib = _ffi.load()
+    dev = dbatch.device
+    n = int(dbatch.struct.n_reads)
+    if mate is None:
+        mate = pair_mates(dbatch)
+    with torch.cuda.device(dev):
+        mate = mate.to(dev, torch.int32).contiguous()
+        qmask = C.byref(dbatch.qmask) if dbatch.qmask is not None else None
+        scratch = torch.empty(int(lib.kdl_overlap_scratch_words(n)), dtype=torch.int32, device=dev)
+        args = (C.byref(dbatch.struct), qmask, mate.data_ptr() if n else None, scratch.data_ptr())
+        _ffi.check(lib.kdl_overlap_count(*args, _stream_ptr(dev)), "kdl_overlap_count")
+        tot = scratch[-_OVERLAP_TOTALS:].cpu().numpy().view(np.uint32).astype(np.int64)
+        n_mr, n_mb, n_drops, n_pairs, n_ob, n_od, n_oi = (int(x) for x in tot[:7])
+        drops = torch.empty((n_drops, 4), dtype=torch.int32, device=dev)
+        stats = (n_pairs, n_ob, n_od, n_oi)
+        if n_ob == 0 and n_drops == 0:
+            return dataclasses.replace(dbatch, drops=drops, overlap_masked=stats)
+        tensors = dict(dbatch.tensors)
+        q = dbatch.qmask
+        if n_ob:
+            tensors.update(mask_read=torch.empty(n_mr, dtype=torch.int32, device=dev),
+                           mask_off=torch.empty(n_mr + 1, dtype=torch.int32, device=dev),
+                           mask_qpos=torch.empty(n_mb, dtype=torch.int32, device=dev))
+            q = _ffi.KdlQmask()
+            q.n_reads, q.n_bases = n_mr, n_mb
+            q.read_idx, q.off, q.qpos = (int(tensors[f].data_ptr()) for f in ("mask_read", "mask_off", "mask_qpos"))
+        # (no overlap base: the merged list is the batch's own, and only the drop rows are written)
+        out = C.byref(q) if n_ob and n_mr else None
+        rc = lib.kdl_overlap_apply(*args, int(dbatch.tensors["seq4"].data_ptr()), out,
+                                   drops.data_ptr() if n_drops else None, n_drops, _stream_ptr(dev))
+        _ffi.check(rc, "kdl_overlap_apply")
+    return dataclasses.replace(dbatch, tensors=tensors, qmask=q, drops=drops, overlap_masked=stats)
+
+
+def dropped_event_rows(dbatch: DeviceBatch) -> np.ndarray:
+    """The insertion-event rows K10 dropped (int64, ascending) -- the rows no insertion string may read."""
+    if dbatch.drops is None or dbatch.drops.shape[0] == 0:
+        return np.zeros(0, dtype=np.int64)
+    evt = dbatch.drops[:, 3].cpu().numpy().astype(np.int64)
+    return np.sort(evt[evt >= 0])
 
 
 def download_fields(dbatch: DeviceBatch) -> dict:
@@ -628,17 +725,36 @@ def deletion_events(dbatch: DeviceBatch):
 _LEN_BITS = 28  # a CIGAR op length has 28 bits
 
 
+def _deletion_groups(dbatch: DeviceBatch):
+    """K7's events grouped by (slot, length) on the device: (key = slot << 28 | length, count), keys ascending.  The
+    deletions K10 dropped (mask_overlaps) are subtracted by the same key, and groups left empty are removed."""
+    ev_slot, ev_len = deletion_events(dbatch)
+    with torch.cuda.device(dbatch.device):
+        key, cnt = torch.unique((ev_slot << _LEN_BITS) | ev_len.to(torch.int64), sorted=True, return_counts=True)
+        d = dbatch.drops
+        if d is None or key.numel() == 0:
+            return key, cnt
+        d = d[d[:, 3] < 0]
+        if d.shape[0] == 0:
+            return key, cnt
+        dk, dc = torch.unique((d[:, 0].to(torch.int64) << _LEN_BITS) | d[:, 1].to(torch.int64), return_counts=True)
+        at = torch.searchsorted(key, dk).clamp(max=key.numel() - 1)
+        cnt = cnt.clone()
+        cnt.index_add_(0, at, torch.where(key[at] == dk, -dc, torch.zeros_like(dc)))  # (each is one of the events)
+        live = cnt > 0
+        return key[live], cnt[live]
+
+
 def deletion_alleles(dbatch: DeviceBatch, counts: torch.Tensor, abs_threshold, rel_threshold):
     """The deletion alleles of `variants --vcf --reference` (extension): K7's events grouped by (slot, length) on the
     device, each with its count c and the six-allele depth D of its first slot (columns 0-5 of `counts`, a device
     table of the same batch); kept when c > abs_threshold and c / D > rel_threshold (0 at D = 0).  Only the kept
     groups leave the device: (slot, length, count, depth), int64 numpy arrays sorted by slot, then length."""
-    ev_slot, ev_len = deletion_events(dbatch)
-    if ev_slot.numel() == 0:
+    key, cnt = _deletion_groups(dbatch)
+    if key.numel() == 0:
         z = np.zeros(0, dtype=np.int64)
         return z, z.copy(), z.copy(), z.copy()
     with torch.cuda.device(counts.device):
-        key, cnt = torch.unique((ev_slot << _LEN_BITS) | ev_len.to(torch.int64), sorted=True, return_counts=True)
         slot = key >> _LEN_BITS
         length = key & ((1 << _LEN_BITS) - 1)
         depth = counts[0:6].index_select(1, slot).to(torch.int64).sum(dim=0)
@@ -654,11 +770,10 @@ def deletion_counts(dbatch: DeviceBatch, slot, length) -> np.ndarray:
     q = (np.asarray(slot, dtype=np.int64) << _LEN_BITS) | np.asarray(length, dtype=np.int64)
     if q.size == 0:
         return np.zeros(0, dtype=np.int64)
-    ev_slot, ev_len = deletion_events(dbatch)
-    if ev_slot.numel() == 0:
+    key, cnt = _deletion_groups(dbatch)
+    if key.numel() == 0:
         return np.zeros(q.shape[0], dtype=np.int64)
     with torch.cuda.device(dbatch.device):
-        key, cnt = torch.unique((ev_slot << _LEN_BITS) | ev_len.to(torch.int64), sorted=True, return_counts=True)
         tq = torch.from_numpy(q).to(key.device)
         at = torch.searchsorted(key, tq).clamp(max=key.numel() - 1)
         return torch.where(key[at] == tq, cnt[at], torch.zeros_like(cnt[at])).cpu().numpy().astype(np.int64)

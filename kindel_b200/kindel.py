@@ -57,11 +57,15 @@ class PileupRun:
     _device = None   # (count table, DeviceBatch) of host tables, uploaded on demand (device_tables)
     _reverse = None  # (count table, DeviceBatch) of the reverse-strand reads (reverse_table)
     primers = None   # the PrimerSet whose primer bases the pileup masked (extension), None when off
+    mask_overlaps = False  # the pileup counted each read pair once where its mates overlap (extension, K10)
+    _dropped_events = None  # K10's dropped insertion-event rows of host tables
+    _overlap_stats = None   # K10's (pairs, bases, deletions, insertions) of host tables
 
-    def __init__(self, batch: bamio.ReadBatch, device=None, primers=None):
+    def __init__(self, batch: bamio.ReadBatch, device=None, primers=None, mask_overlaps=False):
         self.batch = batch
         self.primers = primers
-        self.dbatch = _upload(batch, device, primers)
+        self.mask_overlaps = bool(mask_overlaps)
+        self.dbatch = _upload(batch, device, primers, self.mask_overlaps)
         self.counts, self.events = engine.pileup(self.dbatch)
         self.calls_device = None
         self._host_counts = None
@@ -69,34 +73,45 @@ class PileupRun:
         self._ins = None
 
     @classmethod
-    def from_host_tables(cls, batch, counts, derived, events, primers=None):
+    def from_host_tables(cls, batch, counts, derived, events, primers=None, mask_overlaps=False, dropped_events=None,
+                         overlap_stats=None):
         """Wrap tables that already sit in host memory (results copied back by another path, e.g.
         the kdl_ctx_* host-buffer call or a multi-GPU reduction).  Does no computation.  primers: the PrimerSet the
-        tables were piled with (a re-upload of the batch masks the same bases)."""
+        tables were piled with (a re-upload of the batch masks the same bases).  mask_overlaps: the tables count each
+        read pair once (a re-upload masks the same mates again); dropped_events: K10's dropped insertion-event rows,
+        which the insertion table leaves out; overlap_stats: K10's (pairs, bases, deletions, insertions) for the
+        REPORT."""
         run = cls.__new__(cls)
         run.batch, run.dbatch, run.counts, run.events, run.calls_device = batch, None, None, None, None
         run.primers = primers
+        run.mask_overlaps = bool(mask_overlaps)
+        run._dropped_events = dropped_events
+        run._overlap_stats = None if overlap_stats is None else tuple(int(x) for x in overlap_stats)
         run._host_counts = np.ascontiguousarray(counts, dtype=np.int32)
         run._host_derived = np.ascontiguousarray(derived, dtype=np.int32)
-        run._ins = InsertionTable(batch, events)
+        run._ins = None
+        run._ins = run._insertion_table(events)
         return run
 
     def device_tables(self):
         """(count table, DeviceBatch) on a device.  Host tables (a multi-GPU result): the reduced table and the batch
-        go to this process's GPU, once (its primer bases masked again, as the ranks masked them)."""
+        go to this process's GPU, once (its primer bases and mate overlaps masked again, as the ranks saw them)."""
         if self.counts is not None:
             return self.counts, self.dbatch
         if self._device is None:
             import torch
 
             dev = engine.require_cuda()
-            self._device = (torch.from_numpy(self.host_counts).to(dev), _upload(self.batch, dev, self.primers))
+            self._device = (torch.from_numpy(self.host_counts).to(dev),
+                            _upload(self.batch, dev, self.primers, self.mask_overlaps))
         return self._device
 
     def reverse_table(self):
         """(count table, DeviceBatch) of the reverse-strand reads alone (extension: `variants --vcf --strand`), built
         once: K8 selects the reads whose `reverse` byte is set into a device batch, and the unchanged pileup counts
-        them.  The forward table is the total minus this one.  Needs a batch decoded with strand=True."""
+        them.  The forward table is the total minus this one.  Needs a batch decoded with strand=True.  K8 carries the
+        merged mask list, and the sub-batch keeps the drop rows of its reverse R2 reads (mask_overlaps), which its
+        pileup takes back."""
         if self._reverse is None:
             import torch
 
@@ -117,8 +132,27 @@ class PileupRun:
     @property
     def ins_table(self) -> InsertionTable:
         if self._ins is None:
-            self._ins = InsertionTable(self.batch, self.events.cpu().numpy())
+            self._ins = self._insertion_table(self.events.cpu().numpy())
         return self._ins
+
+    def _insertion_table(self, events) -> InsertionTable:
+        """The one place the run's event rows become its insertion table: without the rows K10 dropped
+        (mask_overlaps), so that no insertion string, VCF record or `alignment` view reads them."""
+        dropped = self._dropped_events
+        if dropped is None and self.dbatch is not None:
+            dropped = engine.dropped_event_rows(self.dbatch)
+        if dropped is not None and len(dropped):
+            events = np.delete(np.asarray(events).reshape(-1, 4), np.asarray(dropped, dtype=np.int64), axis=0)
+        return InsertionTable(self.batch, events)
+
+    @property
+    def overlap_stats(self):
+        """(pairs, bases, deletions, insertions) K10 masked (mask_overlaps), None when off."""
+        if not self.mask_overlaps:
+            return None
+        if self._overlap_stats is not None:
+            return self._overlap_stats
+        return (self.dbatch if self.dbatch is not None else self.device_tables()[1]).overlap_masked
 
     @property
     def host_counts(self) -> np.ndarray:
@@ -145,12 +179,36 @@ class PileupRun:
         return OrderedDict((self.batch.contig_names[c], self.alignment(c)) for c in range(self.batch.n_contigs))
 
 
-def _upload(batch, device, primers):
-    """The batch on a device; with a PrimerSet (extension) its primer bases masked there by K9 (engine.mask_primers)."""
+def _upload(batch, device, primers, mask_overlaps=False):
+    """The batch on a device; with a PrimerSet (extension) its primer bases masked there by K9 (engine.mask_primers),
+    then with mask_overlaps (extension) each pair's second mate masked where the first covers it, K10p + K10
+    (engine.mask_overlaps): after K9, so that a primer-masked base of R1 covers nothing."""
     dbatch = engine.upload(batch, device)
-    if primers is None:
-        return dbatch
-    return engine.mask_primers(dbatch, primer_arrays(primers, batch.contig_names, batch.contig_len))
+    if primers is not None:
+        dbatch = engine.mask_primers(dbatch, primer_arrays(primers, batch.contig_names, batch.contig_len))
+    if mask_overlaps:
+        dbatch = engine.mask_overlaps(dbatch)
+    return dbatch
+
+
+def _masked_for_shards(batch, primers, mask_overlaps):
+    """(host batch, drop rows, K10's (pairs, bases, deletions, insertions)) of a sharded job with mask_overlaps: mates
+    may land on different ranks, so K9 and K10 run once here, on this process's GPU; the merged mask list comes back
+    and is applied to the host batch (the ranks pile it without primers), and each rank takes back its own R2s' drop
+    rows (distributed.shard_drops)."""
+    dbatch = _upload(batch, engine.require_cuda(), primers, True)
+    drops = dbatch.drops.cpu().numpy().astype(np.int32).reshape(-1, 4)
+    stats = dbatch.overlap_masked
+    q = dbatch.qmask
+    if q is None:
+        return batch, drops, stats
+    n_mr, n_mb = int(q.n_reads), int(q.n_bases)
+    read = dbatch.tensors["mask_read"][:n_mr].cpu().numpy().view(np.uint32).astype(np.int64)
+    off = dbatch.tensors["mask_off"][:n_mr + 1].cpu().numpy().view(np.uint32).astype(np.int64)
+    qpos = dbatch.tensors["mask_qpos"][:n_mb].cpu().numpy().view(np.uint32)
+    counts = np.zeros(batch.n_reads, dtype=np.int64)
+    counts[read] = np.diff(off)
+    return bamio.with_mask(batch, counts, qpos), drops, stats
 
 
 def _op_word(length, op):
@@ -196,7 +254,7 @@ def _default_devices(devices):
 
 
 def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq=0, exclude_flags=0,
-               iupac_threshold=None, strand=False, primers=None):
+               iupac_threshold=None, strand=False, primers=None, mask_overlaps=False):
     """(PileupRun, calls) of an alignment file on `devices` GPUs.  devices > 1: one process per GPU, reads (or whole
     contigs) sharded, counts exchanged over NVLink in front of the vote (distributed.run_sharded); the result is
     bit-identical to one GPU.  min_base_quality / min_mapq / exclude_flags (extension, all off by default): a record
@@ -206,28 +264,42 @@ def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq
     the reads' strands (PileupRun.reverse_table).  primers (extension, default None = off): a BED path or a
     primers.PrimerSet; the bases of every read that copy an amplicon primer are then read as N and not counted, as
     min_base_quality does with a low-quality base (K9, kindel_b200/primers.py has the rule).  With several GPUs every
-    rank masks its own shard; the result is the same."""
+    rank masks its own shard; the result is the same.  mask_overlaps (extension, default False = off): each read pair
+    is counted once where its mates overlap -- the second mate's bases, deletions and insertions there are masked or
+    dropped where the first mate has information (K10p / K10 / K10u, include/kindel_b200.h has the rule); the batch is
+    then decoded with its mates.  With several GPUs the pairing and the masking run once on this process's GPU, and
+    every rank takes back its own second mates' drops; the result is the same."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
     primers = as_primer_set(primers)
-    batch = bamio.read_alignment(bam_path, min_mapq=min_mapq, exclude_flags=exclude_flags,
-                                 min_base_quality=min_base_quality, strand=strand)
+    decode = dict(min_mapq=min_mapq, exclude_flags=exclude_flags, min_base_quality=min_base_quality, strand=strand)
+    if mask_overlaps:  # (the keyword only when on: the decode stays as it was otherwise)
+        decode["mates"] = True
+    batch = bamio.read_alignment(bam_path, **decode)
     arrays = primer_arrays(primers, batch.contig_names, batch.contig_len) if primers is not None else None
     devices = _default_devices(devices)
     if devices <= 1:
-        run = PileupRun(batch, primers=primers)
+        run = PileupRun(batch, primers=primers, mask_overlaps=mask_overlaps)
         return run, None
     from . import distributed
 
-    calls, counts, derived, events = distributed.run_sharded(batch, devices, min_depth, iupac_threshold=iupac_threshold,
-                                                             primers=arrays)
-    return PileupRun.from_host_tables(batch, counts, derived, events, primers=primers), calls
+    shards, drops, stats = batch, None, None
+    if mask_overlaps:
+        shards, drops, stats = _masked_for_shards(batch, primers, True)
+        arrays = None  # (the primer bases are in the merged mask list already)
+    calls, counts, derived, events = distributed.run_sharded(shards, devices, min_depth, iupac_threshold=iupac_threshold,
+                                                             primers=arrays, drops=drops)
+    dropped = None if drops is None else np.sort(drops[drops[:, 3] >= 0, 3].astype(np.int64))
+    return PileupRun.from_host_tables(batch, counts, derived, events, primers=primers, mask_overlaps=mask_overlaps,
+                                      dropped_events=dropped, overlap_stats=stats), calls
 
 
-def parse_bam(bam_path, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None):
+def parse_bam(bam_path, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None,
+              mask_overlaps=False):
     """Alignment information for each reference sequence, first-seen order
-    (reference kindel/kindel.py:131-153).  devices, the filters and primers: extensions, see pileup_run."""
+    (reference kindel/kindel.py:131-153).  devices, the filters, primers and mask_overlaps: extensions, see
+    pileup_run."""
     return pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags,
-                      primers=primers)[0].alignments()
+                      primers=primers, mask_overlaps=mask_overlaps)[0].alignments()
 
 
 # --------------------------------------------------------------------------------- consensus
@@ -550,13 +622,15 @@ DepthRange = namedtuple("DepthRange", ["dmin", "dmax"])  # min / max ACGT depth 
 
 
 def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_depth, min_overlap,
-                 clip_decay_threshold, trim_ends, uppercase, filters=None, iupac_threshold=None, primers=None):
+                 clip_decay_threshold, trim_ends, uppercase, filters=None, iupac_threshold=None, primers=None,
+                 overlaps=None):
     """REPORT text block (reference kindel/kindel.py:437-485).  filters (extension): (min_base_quality, min_mapq,
     exclude_flags); when any is set, three option lines follow `- uppercase:`, otherwise the text is the reference's.
     iupac_threshold (extension): when set, `- iupac_threshold:` follows the option lines and `- iupac sites:` (the
     positions of multi-base calls, from the `iupac` list of a changes list this module built) follows
     `- ambiguous sites:`.  primers (extension): the primer BED's file name; when set, `- primers:` follows the filter
-    lines."""
+    lines.  overlaps (extension: mask_overlaps): K10's (pairs, bases, deletions, insertions); when set,
+    `- mate overlaps:` follows the filter and primer lines."""
     if isinstance(weights, DepthRange):  # already reduced on the device: no table copy needed
         dmin, dmax = weights.dmin, weights.dmax
     elif isinstance(weights, BaseCounts):
@@ -589,6 +663,8 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
                   "- exclude_flags: {:#x}".format(filters[2])]
     if primers is not None:
         lines.append("- primers: {}".format(primers))
+    if overlaps is not None:
+        lines.append("- mate overlaps: {} pairs, {} bases, {} deletions, {} insertions masked".format(*overlaps))
     if iupac_threshold is not None:
         lines.append("- iupac_threshold: {}".format(iupac_threshold))
     lines += [
@@ -609,13 +685,13 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
 # --------------------------------------------------------------------------------- public API
 def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_decay_threshold=0.1,
                      mask_ends=50, trim_ends=False, uppercase=False, devices=None, min_base_quality=0, min_mapq=0,
-                     exclude_flags=0, iupac_threshold=None, qualities=False, primers=None):
+                     exclude_flags=0, iupac_threshold=None, qualities=False, primers=None, mask_overlaps=False):
     """Consensus sequence(s) of an alignment file (reference kindel/kindel.py:488-555).
 
     Device work per file: one pileup (K1) and one vote (K2) over all contigs at once; only the
     call bytes, the insertion events and -- for --realign and the report -- count columns come
     back to the host.  `devices` (extension; default $KINDEL_GPUS or 1) shards the pileup over that many GPUs of
-    the node.  min_base_quality / min_mapq / exclude_flags / primers: extension, see pileup_run.
+    the node.  min_base_quality / min_mapq / exclude_flags / primers / mask_overlaps: extension, see pileup_run.
 
     iupac_threshold (extension; default None = off, the reference's vote): t in [0, 1].  Where a base is emitted,
     the call is the smallest set of the most frequent bases (A, C, G, T; N is not an allele) that holds at least
@@ -627,7 +703,8 @@ def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_d
     qualities=False.  Off, `.qualities` is None and nothing else runs."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
     filters = (min_base_quality, min_mapq, exclude_flags)
-    run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold, primers=primers)
+    run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold, primers=primers,
+                            mask_overlaps=mask_overlaps)
     if calls is None:
         calls = run.vote(min_depth, iupac_threshold)
     return consensus_from_run(run, calls, bam_path, realign, min_depth, min_overlap,
@@ -736,6 +813,7 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
     ins_table = run.ins_table
     consensuses, refs_changes, refs_reports = [], {}, {}
     primers_name = getattr(getattr(run, "primers", None), "name", None)
+    overlaps = run.overlap_stats if getattr(run, "mask_overlaps", False) else None
     on_device = run.counts is not None
     device_text = on_device and not realign and run.calls_device is not None
     qual_all = ins_q = qtexts = None
@@ -786,7 +864,7 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
                                                cdr_patches, trim_ends, uppercase)
         report = build_report(ref_id, report_weights, changes, cdr_patches, bam_path, realign, min_depth,
                               min_overlap, clip_decay_threshold, trim_ends, uppercase, filters, iupac_threshold,
-                              primers=primers_name)
+                              primers=primers_name, overlaps=overlaps)
         consensuses.append(consensus_seqrecord(cons, ref_id, quals))
         refs_reports[ref_id] = report
         refs_changes[ref_id] = changes
@@ -795,12 +873,13 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
 
 def weights(bam_path: "path to SAM/BAM file", relative: "output relative nucleotide frequencies" = False,
             confidence: "calculate confidence interval" = True, confidence_alpha: "confidence interval alpha" = 0.01,
-            devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None):
+            devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None, mask_overlaps=False):
     """DataFrame of per-site nucleotide frequencies, depth, consensus, clip starts/ends, confidence
     interval and entropy (reference kindel/kindel.py:558-630).  Integer columns come from the GPU
-    table; the float tail is the reference's arithmetic, vectorised.  devices, the filters and primers: extensions,
-    see pileup_run."""
-    run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers)[0]
+    table; the float tail is the reference's arithmetic, vectorised.  devices, the filters, primers and
+    mask_overlaps: extensions, see pileup_run."""
+    run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers,
+                     mask_overlaps=mask_overlaps)[0]
     return weights_from_run(run, relative, confidence, confidence_alpha)
 
 
@@ -856,7 +935,7 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
              rel_threshold: "relative frequency (0.0-1.0) above which to call variants" = 0.01,
              only_variants: "exclude invariant sites from output" = False,
              absolute: "report absolute variant frequencies" = False, devices=None, min_base_quality=0, min_mapq=0,
-             exclude_flags=0, primers=None):
+             exclude_flags=0, primers=None, mask_overlaps=False):
     """EXTENSION -- not in the reference snapshot.  The reference's README (README.md:106-107) lists a `variants`
     sub-command ("Output variants exceeding specified absolute and relative frequency thresholds") but its code
     (kindel/kindel.py, kindel/cli.py) has no such function, so there is nothing to be bit-exact with: parity
@@ -865,9 +944,10 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
     `abs_threshold` AND whose share of the depth (A+C+G+T+N+deletions, as in `weights`) exceeds `rel_threshold`
     (variant_alleles).  Columns: chrom, pos, depth, consensus (allele letter, `-` = deletion), then one column per
     allele holding its relative (default) or absolute frequency where it is a variant and 0 elsewhere.  With
-    only_variants the sites are selected on the device (K6, variant_sites) and only they are copied back.  primers:
-    extension, see pileup_run."""
-    run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers)[0]
+    only_variants the sites are selected on the device (K6, variant_sites) and only they are copied back.  primers,
+    mask_overlaps: extensions, see pileup_run."""
+    run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers,
+                     mask_overlaps=mask_overlaps)[0]
     return variants_from_run(run, abs_threshold, rel_threshold, only_variants, absolute)
 
 
@@ -965,7 +1045,7 @@ _VCF_ALT = ((0, "A"), (1, "C"), (2, "G"), (3, "T"), (5, "*"))  # N (4) is not an
 
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
-                 exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None) -> str:
+                 exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None, mask_overlaps=False) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -986,11 +1066,14 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     where some ALT's SOR exceeds it.  _strand_fields has the rules.
 
     primers (extension: `--primers`): see pileup_run; the records then count no primer base (the strand counts
-    neither), and the header gets `##kindelPrimers=<the BED's file name>`."""
+    neither), and the header gets `##kindelPrimers=<the BED's file name>`.
+
+    mask_overlaps (extension: `--mask-overlaps`): see pileup_run; DP, AD, AO and the strand counts then count each
+    read pair once where its mates overlap, and the header gets `##kindelMateOverlaps=R2 masked where R1 covers`."""
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
     filters = (min_base_quality, min_mapq, exclude_flags)
-    run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers)[0]
+    run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers, mask_overlaps=mask_overlaps)[0]
     return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference, strand=strand,
                                  max_sor=max_sor)
 
@@ -1042,6 +1125,8 @@ def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None,
     primers = getattr(run, "primers", None)
     if primers is not None:
         lines.append("##kindelPrimers={}".format(primers.name))
+    if getattr(run, "mask_overlaps", False):
+        lines.append("##kindelMateOverlaps=R2 masked where R1 covers")
     if strand:
         lines.append("##kindelStrand=max_sor={}".format("." if max_sor is None else max_sor))
     if reference_name is not None:
@@ -1075,7 +1160,8 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
     """Host half of variants_vcf (see there): the VCF text of a finished pileup.  filters: (min_base_quality,
     min_mapq, exclude_flags) as the pileup applied them, for the header.  reference, strand, max_sor: see variants_vcf;
     with a reference the records are _reference_records'.  Strand needs a run whose batch has `reverse`
-    (ValueError otherwise).  A run piled with primers (extension) adds its `##kindelPrimers` line.
+    (ValueError otherwise).  A run piled with primers (extension) adds its `##kindelPrimers` line, one piled with
+    mask_overlaps its `##kindelMateOverlaps` line.
 
     Strand counts (ADF, ADR): without a reference they are the reverse table's counts of the record's AD columns and
     the total's minus those, so ADF + ADR == AD.  With one, an SNV's the same (REF 0 where the reference has no A, C,
@@ -1237,13 +1323,13 @@ def _indel_strand(dp, dp_rev, ao, ao_rev, max_sor):
 
 
 def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0,
-             primers=None):
+             primers=None, mask_overlaps=False):
     """DataFrame of relative per-site nucleotide frequencies, indels and entropy
     (reference kindel/kindel.py:633-664), including its indexing of `i`/`d` by global row number
     into the LAST contig's tables (IndexError on most multi-contig files, SURVEY.md A-14).
-    devices, the filters and primers: extensions, see pileup_run."""
+    devices, the filters, primers and mask_overlaps: extensions, see pileup_run."""
     return features_from_run(pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags,
-                                        primers=primers)[0])
+                                        primers=primers, mask_overlaps=mask_overlaps)[0])
 
 
 def features_from_run(run):

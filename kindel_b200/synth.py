@@ -6,6 +6,10 @@
     strands(...)         seeded strand bytes, with reads that must lie on one strand (alleles carried by one strand)
     tiled_scheme(...)    a tiled amplicon primer scheme as BED rows (`--primers`)
     amplicon_reads(...)  tiled-amplicon reads: every read starts or ends at an amplicon end, in a primer
+    paired_reads(...)    Illumina-style read pairs (`--mask-overlaps`): both mates of every fragment, names, flags and
+                         mate positions, both orientations, some fragments with an indel the mates share
+    amplicon_pairs(...)  read pairs of tiled amplicons: both mates of a fragment start or end in its primers
+    simple_pairs(...)    paired_reads / amplicon_pairs at the sizes of the bench lines, vectorised, without indels
 
 Reads copy the contig's bases on M segments with a substitution rate (to A/C/G/T/N uniformly);
 inserted and clipped bases are random.  Everything is vectorised numpy so the 5 Mb x 200x case
@@ -283,9 +287,12 @@ def to_records(batch: bamio.ReadBatch):
     return contigs, recs
 
 
-def write_simple_bam(path, batch: bamio.ReadBatch, level: int = 1, threads: int = 8):
+def write_simple_bam(path, batch: bamio.ReadBatch, level: int = 1, threads: int = 8, names=None, flag=None,
+                     next_pos=None):
     """Vectorised BAM writer for an all-simple, uniform-read-length batch (the config 2/4/5 shapes):
-    lets tests and tools push 10^5..10^7 synthetic reads through the real decode path quickly."""
+    lets tests and tools push 10^5..10^7 synthetic reads through the real decode path quickly.  names (uint8 [n, k]
+    fixed-width QNAMEs), flag (per read) and next_pos (PNEXT - 1 per read, RNEXT then the read's own contig): paired
+    reads (write_paired_bam); by default every read is "r", FLAG 0 or 16 by strand, RNEXT / PNEXT -1."""
     import struct
     from concurrent.futures import ThreadPoolExecutor
 
@@ -296,7 +303,7 @@ def write_simple_bam(path, batch: bamio.ReadBatch, level: int = 1, threads: int 
     L = int(lens[0])
     words = (L + 7) // 8
     n_seq = (L + 1) // 2
-    name = b"r\x00"
+    name = b"r\x00" if names is None else b"\x00" * (names.shape[1] + 1)
     rec_len = 32 + len(name) + 4 + n_seq + L
     rec = np.zeros((n, 4 + rec_len), dtype=np.uint8)
 
@@ -312,12 +319,18 @@ def write_simple_bam(path, batch: bamio.ReadBatch, level: int = 1, threads: int 
     rec[:, 13] = 60
     put(14, np.full(n, 4680), "<u2")
     put(16, np.ones(n), "<u2")            # n_cigar_op
-    put(18, np.zeros(n) if batch.reverse is None else 16 * batch.reverse.astype(np.int64), "<u2")  # flag
+    if flag is None:
+        flag = np.zeros(n) if batch.reverse is None else 16 * batch.reverse.astype(np.int64)
+    put(18, flag, "<u2")  # flag
     put(20, np.full(n, L), "<i4")
-    put(24, np.full(n, -1), "<i4")
-    put(28, np.full(n, -1), "<i4")
+    put(24, np.full(n, -1) if next_pos is None else ref_id, "<i4")
+    put(28, np.full(n, -1) if next_pos is None else next_pos, "<i4")
     put(32, np.zeros(n), "<i4")
-    rec[:, 36:36 + len(name)] = np.frombuffer(name, dtype=np.uint8)
+    if names is None:
+        rec[:, 36:36 + len(name)] = np.frombuffer(name, dtype=np.uint8)
+    else:
+        rec[:, 36:36 + names.shape[1]] = names
+        rec[:, 36 + names.shape[1]] = 0
     put(36 + len(name), np.full(n, L << 4), "<u4")
     seq_be = batch.seq4.reshape(n, words).astype(">u4").view(np.uint8).reshape(n, words * 4)[:, :n_seq]
     rec[:, 40 + len(name):40 + len(name) + n_seq] = seq_be
@@ -394,3 +407,228 @@ def with_qualities(batch: bamio.ReadBatch, seed: int, min_base_quality: int = 20
     qual = qualities(seed, batch.seq_len, low_frac)
     counts, qpos = bamio.low_quality_mask(qual, batch.seq_len, min_base_quality)
     return bamio.with_mask(batch, counts, qpos), qual
+
+
+_NAME_DIGITS = 9  # paired read names: "p" + the fragment number, zero-padded
+
+
+def pair_names(frag) -> np.ndarray:
+    """The QNAMEs of fragments `frag` as fixed-width bytes rows (uint8 [n, 1 + _NAME_DIGITS])."""
+    frag = np.asarray(frag, dtype=np.int64)
+    digits = (frag[:, None] // (10 ** np.arange(_NAME_DIGITS - 1, -1, -1, dtype=np.int64))[None, :]) % 10
+    return np.concatenate([np.full((frag.shape[0], 1), ord("p"), dtype=np.uint8),
+                           (digits + ord("0")).astype(np.uint8)], axis=1)
+
+
+def _fnv_rows(rows: np.ndarray) -> np.ndarray:
+    """64-bit FNV-1a of every bytes row (bamio.name_hash, vectorised)."""
+    h = np.full(rows.shape[0], 0xCBF29CE484222325, dtype=np.uint64)
+    with np.errstate(over="ignore"):
+        for k in range(rows.shape[1]):
+            h = (h ^ rows[:, k].astype(np.uint64)) * np.uint64(0x100000001B3)
+    return h
+
+
+def _pair_batch(names, contig_lens, contig_of, starts, mate_starts, flags, cigars, seqs, frag):
+    """ReadBatch (mates included) of reads given one by one: contig, start, CIGAR words, nibble codes."""
+    order = np.lexsort((starts, contig_of))
+    n = len(order)
+    seq_len = np.array([len(seqs[i]) for i in order], dtype=np.int64)
+    words = (seq_len + 7) // 8
+    seq4 = np.concatenate([_pack_rows(np.concatenate([seqs[i], np.zeros((-len(seqs[i])) % 8, np.uint8)])[None, :])
+                           .reshape(-1) for i in order]) if n else np.zeros(0, dtype=np.uint32)
+    cig = [cigars[i] for i in order]
+    cig_off = np.concatenate(([0], np.cumsum([len(c) for c in cig]))).astype(np.int64)
+    read_off = np.concatenate(([0], np.cumsum(np.bincount(np.asarray(contig_of)[order], minlength=len(names)))))
+    flag = np.asarray(flags)[order]
+    same = np.ones(n, dtype=bool)
+    roles = np.array([bamio.pair_role(int(f), bool(x)) for f, x in zip(flag, same)], dtype=np.uint8)
+    mates = (_fnv_rows(pair_names(np.asarray(frag)[order])), np.asarray(mate_starts)[order], roles)
+    batch = bamio.finalize(names, np.asarray(contig_lens), read_off, np.asarray(starts)[order],
+                           np.cumsum(words) - words, seq_len, cig_off,
+                           np.array([w for c in cig for w in c], dtype=np.int64), seq4, n_records=n,
+                           reverse=((flag & 0x10) != 0).astype(np.uint8), mates=mates)
+    return batch, flag.astype(np.uint16), np.asarray(frag)[order]
+
+
+def paired_reads(seed: int, contig_lens, depth: float, read_len: int = 150, insert_mean: float = 300,
+                 insert_sd: float = 40, indel_frac: float = 0.05, sub_rate: float = 0.01, names=None, refs=None):
+    """Paired-end reads of random contigs: (batch, flag uint16[n], frag int64[n]).  Every fragment of length
+    ~N(insert_mean, insert_sd) (at least read_len) gives two `read_len` reads, one from each end: the left mate
+    forward, the right one reverse, and which of them is the first mate (FLAG 0x40) is random.  A share indel_frac of
+    the fragments carries one insertion or deletion that both mates read where they cover it, so pairs with I / D in
+    their overlap occur.  The batch has its mates (name_hash of "p<fragment>", mate_start, pair_role) and strands;
+    write_paired_bam writes it with QNAME, RNEXT and PNEXT.  refs: a dict that receives each contig's sequence."""
+    rng = np.random.default_rng(seed)
+    names = names or ["ctg%d" % i for i in range(len(contig_lens))]
+    contig_of, starts, mstarts, flags, cigars, seqs, frag = [], [], [], [], [], [], []
+    nf = 0
+    for c, L in enumerate(contig_lens):
+        ref = random_contig(rng, int(L))
+        if refs is not None:
+            refs[names[c]] = "".join("ACGTN"[int(x).bit_length() - 1] if x != 15 else "N" for x in ref)
+        n_frag = int(round(depth * L / (2 * read_len)))
+        ins = np.clip(np.round(rng.normal(insert_mean, insert_sd, n_frag)), read_len, L - 2).astype(np.int64)
+        fs = rng.integers(1, np.maximum(L - ins, 2))
+        kind = np.where(rng.random(n_frag) < indel_frac, rng.integers(1, 3, n_frag), 0)  # 1 = D, 2 = I
+        first_left = rng.random(n_frag) < 0.5
+        for k in range(n_frag):
+            s0, ln = int(fs[k]), int(ins[k])
+            mol = ref[s0:s0 + ln].copy()
+            ops_pos = None
+            if kind[k]:  # an indel in the middle of the fragment, where the mates most likely overlap
+                at = ln // 2 + int(rng.integers(-10, 11))
+                size = int(rng.integers(1, 6))
+                if kind[k] == 1 and at + size < ln - 1:
+                    mol = np.concatenate([mol[:at], mol[at + size:]])
+                    ops_pos = ("D", at, size)
+                elif kind[k] == 2:
+                    mol = np.concatenate([mol[:at], random_contig(rng, size), mol[at:]])
+                    ops_pos = ("I", at, size)
+            sub = rng.random(mol.shape[0]) < sub_rate
+            mol[sub] = _CODE[rng.integers(0, 5, int(sub.sum()))]
+            m = mol.shape[0]
+            rl = min(read_len, m)
+            for left in (True, False):
+                q0 = 0 if left else m - rl  # the read's bases mol[q0 : q0 + rl]
+                cig, r0 = _window_cigar(q0, rl, ops_pos)
+                contig_of.append(c)
+                starts.append(s0 + r0)
+                seqs.append(mol[q0:q0 + rl])
+                cigars.append(cig)
+                frag.append(nf + k)
+                first = left == bool(first_left[k])
+                flags.append(0x1 | 0x2 | (0x40 if first else 0x80) | (0x20 if left else 0x10))
+            # each mate's PNEXT is the other's start
+            mstarts += [starts[-1], starts[-2]]
+        nf += n_frag
+    return _pair_batch(names, contig_lens, contig_of, starts, mstarts, flags, cigars, seqs, frag)
+
+
+def _window_cigar(q0: int, n: int, event):
+    """(CIGAR words, reference offset of its start within the fragment) of the molecule bases [q0, q0 + n) when the
+    molecule is the fragment with `event` = None, ("D", at, size) or ("I", at, size) at molecule offset `at`."""
+    M, I, D = 0, 1, 2
+    if event is None:
+        return [n << 4 | M], q0
+    kind, at, size = event
+    if kind == "D":  # molecule offset x >= at sits at fragment offset x + size
+        r0 = q0 if q0 < at else q0 + size
+        if q0 < at < q0 + n:
+            return [(at - q0) << 4 | M, size << 4 | D, (q0 + n - at) << 4 | M], r0
+        return [n << 4 | M], r0
+    # insertion: molecule [at, at + size) is inserted; x >= at + size sits at fragment offset x - size
+    lo, hi = max(q0, at), min(q0 + n, at + size)
+    if lo >= hi:
+        return [n << 4 | M], q0 if q0 < at else q0 - size
+    ops = []
+    if lo > q0:
+        ops.append((lo - q0) << 4 | M)
+    ops.append((hi - lo) << 4 | (I if (lo > q0 and hi < q0 + n) else 4))  # at a read end the inserted bases are a clip
+    if hi < q0 + n:
+        ops.append((q0 + n - hi) << 4 | M)
+    r0 = q0 if q0 < at else at
+    return ops, r0
+
+
+def amplicon_pairs(seed: int, contig_len: int, depth: float, read_len: int = 150, spacing: int = 200,
+                   overlap: int = 50, sub_rate: float = 0.01):
+    """Tiled-amplicon read pairs of one random contig: (batch, flag, frag, scheme rows).  Each fragment is one whole
+    amplicon of tiled_scheme(seed, ...), so one mate starts in its left primer and the other ends in its right
+    primer; the mates overlap in the amplicon's middle when it is shorter than two reads."""
+    rng = np.random.default_rng(seed)
+    rows = tiled_scheme(seed, ["ctg0"], [contig_len], spacing, overlap)
+    amp_lo = np.array([a for _, a, _ in rows[0::2]], dtype=np.int64)
+    amp_hi = np.array([b for _, _, b in rows[1::2]], dtype=np.int64)
+    ref = random_contig(rng, contig_len)
+    n_frag = int(round(depth * contig_len / (2 * read_len)))
+    k = rng.integers(0, amp_lo.shape[0], size=n_frag)
+    first_left = rng.random(n_frag) < 0.5
+    contig_of, starts, mstarts, flags, cigars, seqs, frag = [], [], [], [], [], [], []
+    for j in range(n_frag):
+        a, b = int(amp_lo[k[j]]), int(amp_hi[k[j]])
+        rl = min(read_len, b - a)
+        for left in (True, False):
+            s0 = a if left else b - rl
+            bases = ref[s0:s0 + rl].copy()
+            sub = rng.random(rl) < sub_rate
+            bases[sub] = _CODE[rng.integers(0, 5, int(sub.sum()))]
+            contig_of.append(0)
+            starts.append(s0)
+            seqs.append(bases)
+            cigars.append([rl << 4])
+            frag.append(j)
+            first = left == bool(first_left[j])
+            flags.append(0x1 | 0x2 | (0x40 if first else 0x80) | (0x20 if left else 0x10))
+        mstarts += [starts[-1], starts[-2]]
+    batch, flag, fr = _pair_batch(["ctg0"], [contig_len], contig_of, starts, mstarts, flags, cigars, seqs, frag)
+    return batch, flag, fr, rows
+
+
+def paired_records(batch: bamio.ReadBatch, flag, frag):
+    """(contigs, records) for bamio.write_bam of a paired batch: QNAME "p<fragment>", its FLAG, RNEXT = its own
+    contig and PNEXT = mate_start -- small batches only (Python loop)."""
+    contigs, recs = to_records(batch)
+    names = pair_names(frag)
+    out = []
+    for r, (ref_id, pos0, _, words, seq) in enumerate(recs):
+        out.append((ref_id, pos0, int(flag[r]), words, seq, names[r].tobytes().decode(), 60, None, ref_id,
+                    int(batch.mate_start[r])))
+    return contigs, out
+
+
+def write_paired_bam(path, batch: bamio.ReadBatch, flag, frag, level: int = 1, threads: int = 8):
+    """A paired batch as a BAM file with QNAME, FLAG, RNEXT and PNEXT: vectorised for an all-simple batch of one read
+    length (write_simple_bam), record by record otherwise."""
+    if batch.n_complex == 0 and np.unique(batch.l_seq).shape[0] == 1:
+        write_simple_bam(path, batch, level, threads, names=pair_names(frag), flag=flag,
+                         next_pos=batch.mate_start)
+        return
+    bamio.write_bam(path, *paired_records(batch, flag, frag), level=level)
+
+
+def simple_pairs(seed: int, contig_len: int, depth: float, read_len: int = 150, insert_mean: float = 300,
+                 insert_sd: float = 40, sub_rate: float = 0.01, amplicons=None):
+    """paired_reads for large sizes, vectorised: one contig, `read_len`M mates without indels, sorted by start.
+    amplicons: scheme rows (tiled_scheme); each fragment is then one whole amplicon, so one mate starts in its left
+    primer and the other ends in its right one.  Returns (batch, flag, frag)."""
+    rng = np.random.default_rng(seed)
+    n_frag = int(round(depth * contig_len / (2 * read_len)))
+    if amplicons is None:
+        ins = np.clip(np.round(rng.normal(insert_mean, insert_sd, n_frag)), read_len, contig_len - 2).astype(np.int64)
+        lo = rng.integers(1, np.maximum(contig_len - ins, 2))
+    else:
+        a = np.array([x for _, x, _ in amplicons[0::2]], dtype=np.int64)
+        b = np.array([y for _, _, y in amplicons[1::2]], dtype=np.int64)
+        k = rng.integers(0, a.shape[0], size=n_frag)
+        lo, ins = a[k], np.maximum(b[k] - a[k], read_len)
+    first_left = rng.random(n_frag) < 0.5
+    frag = np.repeat(np.arange(n_frag, dtype=np.int64), 2)
+    left = np.tile(np.array([True, False]), n_frag)
+    start = np.where(left, np.repeat(lo, 2), np.repeat(lo + ins - read_len, 2))
+    mate_start = np.where(left, np.repeat(lo + ins - read_len, 2), np.repeat(lo, 2))
+    first = left == np.repeat(first_left, 2)
+    flag = (0x1 | 0x2 | np.where(first, 0x40, 0x80) | np.where(left, 0x20, 0x10)).astype(np.uint16)
+    order = np.argsort(start, kind="stable")
+    start, mate_start, flag, frag = start[order], mate_start[order], flag[order], frag[order]
+    n = start.shape[0]
+    words = (read_len + 7) // 8
+    ref = random_contig(rng, contig_len)
+    ref_pad = np.concatenate([ref, np.zeros(words * 8, dtype=np.uint8)])
+    parts = []
+    for s0 in range(0, n, 1 << 18):
+        st = start[s0:s0 + (1 << 18)]
+        nib = ref_pad[st[:, None] + np.arange(words * 8, dtype=np.int64)[None, :]]
+        nib[:, read_len:] = 0
+        n_sub = rng.binomial(st.shape[0] * read_len, sub_rate)
+        nib[rng.integers(0, st.shape[0], size=n_sub), rng.integers(0, read_len, size=n_sub)] = \
+            _CODE[rng.integers(0, 5, size=n_sub)]
+        parts.append(_pack_rows(nib))
+    seq4 = np.concatenate(parts).reshape(-1) if parts else np.zeros(0, dtype=np.uint32)
+    roles = np.where((flag & 0x40) != 0, 1, 2).astype(np.uint8)
+    mates = (_fnv_rows(pair_names(frag)), mate_start, roles)
+    batch = bamio.finalize(["ctg0"], np.array([contig_len]), np.array([0, n]), start,
+                           np.arange(n, dtype=np.int64) * words, np.full(n, read_len, dtype=np.int64),
+                           np.arange(n + 1, dtype=np.int64), np.full(n, read_len << 4, dtype=np.int64), seq4,
+                           n_records=n, reverse=((flag & 0x10) != 0).astype(np.uint8), mates=mates)
+    return batch, flag, frag

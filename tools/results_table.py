@@ -54,6 +54,8 @@ def row(path: str, d: dict) -> str:
         work += ", + strand split (K8, reverse pileup)"
     if d.get("primers_ms"):
         work += ", + primer masking (K9, K1q)"
+    if d.get("mates_ms"):
+        work += ", + mate-overlap masking (K10p, K10, K10u)"
     if d.get("map_ab"):
         work += ", zeroing A/B (dirty-sector map)"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
