@@ -310,6 +310,28 @@ int kdl_variant_ref_scatter(const int32_t* counts, int64_t n_slots, const int64_
                             double rel_threshold, const uint32_t* block_sums, int64_t n_sites, int64_t* site_slot,
                             int32_t* site_counts, int64_t* site_dpa, uint8_t* site_mask, void* stream);
 
+/* K6m -- the sites of several samples at once (`variants --vcf a.bam b.bam ...`, extension): K6's passes over the
+ * samples' tables stacked on one shared layout.  counts: int32 [n_samples][7][n_slots] (sample i's columns 0-6 at
+ * counts + i * 7 * n_slots), n_samples >= 1.  Per slot, with t^i sample i's columns and depth^i = t^i[0] + ... +
+ * t^i[5]:
+ *   pooled mode (ref == NULL), only at positions (0 <= p < L): P = sum over the samples of t^i[0..5] in 64-bit,
+ *     top = the first maximum of P; bit k (k = 0..5, k != top) is set when some sample has t^i[k] > abs_floor and
+ *     (double)t^i[k] / (double)depth^i > rel_threshold (0 at depth 0).
+ *   reference mode (ref as for K6r): bits 0-3 are K6r's SNV test of each sample against g, bit 6 K6r's
+ *     insertion-candidate test with each sample's own DPa (depth^i(s - 1) for p >= 1, depth^i(s) for p = 0); each
+ *     ORed over the samples, at K6r's positions.
+ * At n_samples = 1 the bits are K6's (pooled) and K6r's (reference).  abs_floor / rel_threshold as for K6; counting,
+ * scratch (kdl_variant_scratch_words) and the site total as for kdl_variant_count.  kdl_variant_multi_scatter writes,
+ * in ascending slot order, site_slot[i] and site_mask[i] (the OR); the samples' rows are not written: the caller
+ * gathers them from counts at the sites.  All pointers are device pointers. */
+int kdl_variant_multi_count(const int32_t* counts, int32_t n_samples, int64_t n_slots, const int64_t* contig_slot,
+                            const int32_t* contig_len, int32_t n_contigs, const uint8_t* ref, int64_t abs_floor,
+                            double rel_threshold, uint32_t* block_sums, void* stream);
+int kdl_variant_multi_scatter(const int32_t* counts, int32_t n_samples, int64_t n_slots, const int64_t* contig_slot,
+                              const int32_t* contig_len, int32_t n_contigs, const uint8_t* ref, int64_t abs_floor,
+                              double rel_threshold, const uint32_t* block_sums, int64_t n_sites, int64_t* site_slot,
+                              uint8_t* site_mask, void* stream);
+
 /* K7 -- the deletion events of a batch (extension, for `variants --vcf --reference`).  Every read's CIGAR is walked
  * with the reference's cursor (kindel.py:40-81: M/=/X and D advance; an S that is op #0 does not; any later S advances
  * while the cursor is below the contig length L; I, N, H, P do not); simple reads have no D op.  A D of length n >= 1

@@ -140,6 +140,11 @@ _PROTOTYPES = {
     "kdl_variant_ref_scatter": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                           C.c_int64, C.c_double, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_variant_multi_count": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
+                                          C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p]),
+    "kdl_variant_multi_scatter": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
+                                            C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_int64, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
     "kdl_deletion_scratch_words": (C.c_int64, [C.c_int64]),
     "kdl_deletion_count": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p]),
     "kdl_deletion_scatter": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,

@@ -178,7 +178,9 @@ def build_parser() -> argparse.ArgumentParser:
 
     # `variants` is listed by the reference's README (README.md:106-107) but absent from its code: an extension here
     p = sub.add_parser("variants", help=variants.__doc__, description=variants.__doc__, formatter_class=fmt)
-    p.add_argument("bam_path", help="path to SAM/BAM file")
+    # extension: several files (with --vcf) give one VCF with a column per sample
+    p.add_argument("bam_path", nargs="+",
+                   help="path to SAM/BAM file; with --vcf several files give one VCF with a column per sample")
     p.add_argument("-a", "--abs-threshold", type=int, default=1, help="absolute frequency above which to call variants")
     p.add_argument("-r", "--rel-threshold", type=float, default=0.01,
                    help="relative frequency (0.0-1.0) above which to call variants")
@@ -198,8 +200,9 @@ def build_parser() -> argparse.ArgumentParser:
                    help="with --vcf: add ADF / ADR (per-strand allele counts) and SOR (strand odds ratio) to INFO")
     p.add_argument("--max-sor", type=_max_sor, default=None, metavar="X",
                    help="with --vcf: FILTER `sor` where an ALT's strand odds ratio is above X (implies --strand)")
-    p.set_defaults(func=lambda a: variants(a.bam_path, a.abs_threshold, a.rel_threshold, a.only_variants, a.absolute,
-                                           a.gpus, a.vcf, a.reference, a.strand, a.max_sor, **_filters(a)))
+    p.set_defaults(func=lambda a: variants(a.bam_path[0] if len(a.bam_path) == 1 else a.bam_path, a.abs_threshold,
+                                           a.rel_threshold, a.only_variants, a.absolute, a.gpus, a.vcf, a.reference,
+                                           a.strand, a.max_sor, **_filters(a)))
 
     p = sub.add_parser("plot", help=plot.__doc__, description=plot.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")
@@ -212,6 +215,12 @@ def build_parser() -> argparse.ArgumentParser:
 
 def _check_variants_args(parser, args):
     # --absolute and --only-variants shape the table; the VCF always holds the variant sites alone
+    paths = getattr(args, "bam_path", None)
+    if getattr(args, "command", None) == "variants" and len(paths) > 1:
+        if not args.vcf:
+            parser.error("variants: several alignment files need --vcf (the table has no sample columns)")
+        if args.strand or args.max_sor is not None:
+            parser.error("variants: --strand and --max-sor take one alignment file")
     if getattr(args, "vcf", False):
         for flag, on in (("--absolute", args.absolute), ("--only-variants", args.only_variants)):
             if on:

@@ -523,6 +523,59 @@ int kdl_variant_ref_scatter(const int32_t* counts, int64_t n_slots, const int64_
     return check_launch();
 }
 
+static int variant_multi_args(const int32_t* counts, int32_t n_samples, int64_t n_slots, const int64_t* contig_slot,
+                              const int32_t* contig_len, int32_t n_contigs, const uint8_t* ref, int64_t abs_floor,
+                              double rel_threshold, kdl::VariantArgs* v) {
+    int rc = variant_args(counts, n_slots, contig_slot, contig_len, n_contigs, abs_floor, rel_threshold, v);
+    if (rc != KDL_OK) return rc;
+    if (n_samples < 1 || (ref && (reinterpret_cast<uintptr_t>(ref) & 3))) return KDL_ERR_INVALID_ARG;
+    return KDL_OK;
+}
+
+int kdl_variant_multi_count(const int32_t* counts, int32_t n_samples, int64_t n_slots, const int64_t* contig_slot,
+                            const int32_t* contig_len, int32_t n_contigs, const uint8_t* ref, int64_t abs_floor,
+                            double rel_threshold, uint32_t* block_sums, void* stream) {
+    kdl::VariantArgs v;
+    int rc = variant_multi_args(counts, n_samples, n_slots, contig_slot, contig_len, n_contigs, ref, abs_floor,
+                                rel_threshold, &v);
+    if (rc != KDL_OK) return rc;
+    if (!block_sums) return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (ref) {
+        KDL_LAUNCH(kdl::variant_multi_sums_kernel<true>, (unsigned)n_blocks, kdl::A_THREADS, 0, st,
+                   kdl::MultiVariantArgs<true>::make(v, n_samples, ref), block_sums);
+    } else {
+        KDL_LAUNCH(kdl::variant_multi_sums_kernel<false>, (unsigned)n_blocks, kdl::A_THREADS, 0, st,
+                   kdl::MultiVariantArgs<false>::make(v, n_samples, ref), block_sums);
+    }
+    if ((rc = check_launch()) != KDL_OK) return rc;
+    KDL_LAUNCH(kdl::assemble_scan_sums_kernel, 1, kdl::A_THREADS, 0, st, block_sums, n_blocks);
+    return check_launch();
+}
+
+int kdl_variant_multi_scatter(const int32_t* counts, int32_t n_samples, int64_t n_slots, const int64_t* contig_slot,
+                              const int32_t* contig_len, int32_t n_contigs, const uint8_t* ref, int64_t abs_floor,
+                              double rel_threshold, const uint32_t* block_sums, int64_t n_sites, int64_t* site_slot,
+                              uint8_t* site_mask, void* stream) {
+    kdl::VariantArgs v;
+    int rc = variant_multi_args(counts, n_samples, n_slots, contig_slot, contig_len, n_contigs, ref, abs_floor,
+                                rel_threshold, &v);
+    if (rc != KDL_OK) return rc;
+    if (!block_sums || n_sites < 0 || n_sites > n_slots || (n_sites > 0 && (!site_slot || !site_mask)))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_slots + kdl::A_BLOCK - 1) / kdl::A_BLOCK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (ref) {
+        KDL_LAUNCH(kdl::variant_multi_scatter_kernel<true>, (unsigned)n_blocks, kdl::A_THREADS, 0, st,
+                   kdl::MultiVariantArgs<true>::make(v, n_samples, ref), block_sums, n_sites, site_slot, site_mask);
+    } else {
+        KDL_LAUNCH(kdl::variant_multi_scatter_kernel<false>, (unsigned)n_blocks, kdl::A_THREADS, 0, st,
+                   kdl::MultiVariantArgs<false>::make(v, n_samples, ref), block_sums, n_sites, site_slot, site_mask);
+    }
+    return check_launch();
+}
+
 int64_t kdl_deletion_scratch_words(int64_t n_reads) {
     return n_reads < 0 ? 0 : (n_reads + kdl::A_THREADS - 1) / kdl::A_THREADS + 1;
 }

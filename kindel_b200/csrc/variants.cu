@@ -263,6 +263,172 @@ variant_ref_scatter_kernel(RefVariantArgs a, const uint32_t* __restrict__ block_
     variant_scatter(a, block_sums, n_sites, RefVariantArgs::Out{site_slot, site_counts, site_dpa, site_mask});
 }
 
+// ---- K6m: the sites of several samples at once (`variants --vcf a.bam b.bam ...`) ----------------------------
+// counts = T, the samples' tables stacked over one shared layout: int32 [n_samples][7][n_slots].  Per slot, with t^i
+// sample i's columns and depth^i = t0^i + ... + t5^i:
+//   pooled (ref == NULL): P = sum_i t^i over columns 0-5 in int64, top = the first maximum of P; bit k (k = 0..5,
+//     k != top) when some sample has t_k^i > abs_floor and t_k^i / depth^i > rel (0 at depth 0); positions only.
+//   reference: bits 0-3 are K6r's SNV test of each sample against g, bit 6 K6r's insertion test with each sample's
+//     own DPa; both ORed over the samples, at K6r's positions.
+// The test of each sample does not depend on top, so one read of every sample's columns serves both halves of the
+// pooled rule: the per-sample bits are ORed, P is summed beside them, and top's bit is cleared at the end.  The
+// whole rule runs in `load` (every thread of the CTA), because the loop over samples holds DPa's shuffle: lanes past
+// n_slots join it with zeros.  Only (slot, OR-ed mask) is written; the host gathers the samples' rows at the sites.
+// Each pass reads 24 B (pooled) or 28 B + 1 B of reference (reference mode) per slot and sample.
+template <bool kRef>
+struct MultiVariantArgs {
+    const int32_t* counts;  // [n_samples][7][n_slots]
+    long long n_slots;
+    int n_samples;
+    AssembleArgs layout;    // contig_slot / contig_len / n_contigs of the shared layout
+    const uint8_t* ref;     // [n_slots] codes (reference mode)
+    long long abs_floor;
+    double rel_threshold;
+
+    static constexpr int kCols = kRef ? 7 : 6;
+    static MultiVariantArgs make(const VariantArgs& v, int n_samples, const uint8_t* ref) {
+        MultiVariantArgs a{};
+        a.counts = v.counts; a.n_slots = v.n_slots; a.n_samples = n_samples; a.layout = v.layout; a.ref = ref;
+        a.abs_floor = v.abs_floor; a.rel_threshold = v.rel_threshold;
+        return a;
+    }
+    struct Quad { unsigned bits[4]; };
+    struct Out { int64_t* slot; uint8_t* mask; };
+    __device__ __forceinline__ void load(long long s, Quad& q) const;
+    __device__ __forceinline__ void eval(long long, Quad& q, unsigned (&bits)[4]) const {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) bits[j] = q.bits[j];
+    }
+    __device__ __forceinline__ void write(const Out& out, const Quad& q, int j, long long o, long long,
+                                          long long slot, unsigned bits) const {
+        out.slot[o] = slot;
+        out.mask[o] = (uint8_t)bits;
+    }
+};
+
+// where each of the 4 slots from s lies: bit 0 = a position (0 <= p < L), bit 1 = an insertion slot (0 <= p <= L),
+// bit 2 = the first slot of its contig (p = 0); 3 bits per slot, slot s + j at bit 3j
+__device__ __forceinline__ unsigned quad_places(const AssembleArgs& l, long long s) {
+    int lo = 0, hi = l.n_contigs;  // the last contig with contig_slot <= s
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (l.contig_slot[mid] <= s) lo = mid + 1; else hi = mid;
+    }
+    int c = lo - 1;
+    unsigned w = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        while (c + 1 < l.n_contigs && l.contig_slot[c + 1] <= s + j) ++c;  // (contigs of length 0 own one slot)
+        if (c < 0) continue;
+        const long long p = s + j - l.contig_slot[c], L = l.contig_len[c];
+        w |= ((p < L ? 1u : 0u) | (p <= L ? 2u : 0u) | (p == 0 ? 4u : 0u)) << (3 * j);
+    }
+    return w;
+}
+
+template <bool kRef>
+__device__ __forceinline__ void MultiVariantArgs<kRef>::load(long long s, Quad& q) const {
+    const bool in = s < n_slots;
+    const unsigned places = in ? quad_places(layout, s) : 0u;
+    const uint32_t g = (kRef && in) ? __ldg(reinterpret_cast<const uint32_t*>(ref + s)) : 0u;
+    unsigned acc[4] = {0u, 0u, 0u, 0u};
+    long long pool[4][6];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int k = 0; k < 6; ++k) pool[j][k] = 0;
+    const double rel = rel_threshold;
+#pragma unroll 1
+    for (int i = 0; i < n_samples; ++i) {  // uniform over the warp: every lane runs every sample
+        const int32_t* __restrict__ tab = counts + (long long)i * 7 * n_slots;
+        int t[4][kCols];
+        long long depth[4] = {0, 0, 0, 0};
+        if (in) {
+#pragma unroll
+            for (int k = 0; k < kCols; ++k) {
+                const int4 v = __ldg(reinterpret_cast<const int4*>(tab + (long long)k * n_slots + s));
+                t[0][k] = v.x; t[1][k] = v.y; t[2][k] = v.z; t[3][k] = v.w;
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int k = 0; k < 6; ++k) depth[j] += t[j][k];
+        }
+        if (kRef) {
+            long long prev = __shfl_up_sync(0xffffffffu, depth[3], 1);  // depth(s - 1) of this sample
+            if ((threadIdx.x & 31) == 0) {
+                prev = 0;
+                if (s > 0 && in) {
+#pragma unroll
+                    for (int k = 0; k < 6; ++k) prev += __ldg(tab + (long long)k * n_slots + s - 1);
+                }
+            }
+            if (!in) continue;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const unsigned gj = (g >> (8 * j)) & 0xFFu;
+                const double d = (double)depth[j];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    if ((unsigned)k != gj && (long long)t[j][k] > abs_floor) {
+                        const double share = depth[j] > 0 ? (double)t[j][k] / d : 0.0;
+                        if (share > rel) acc[j] |= 1u << k;
+                    }
+                }
+                if ((long long)t[j][6] > abs_floor) {
+                    const long long da = (places >> (3 * j)) & 4u ? depth[j] : (j == 0 ? prev : depth[j - 1]);
+                    const double share = da > 0 ? (double)t[j][6] / (double)da : 0.0;
+                    if (share > rel) acc[j] |= 1u << 6;
+                }
+            }
+        } else if (in) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const double d = (double)depth[j];
+#pragma unroll
+                for (int k = 0; k < 6; ++k) {
+                    pool[j][k] += t[j][k];
+                    if ((long long)t[j][k] > abs_floor) {
+                        const double share = depth[j] > 0 ? (double)t[j][k] / d : 0.0;
+                        if (share > rel) acc[j] |= 1u << k;
+                    }
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const unsigned pl = (places >> (3 * j)) & 7u;
+        unsigned b = acc[j];
+        if (kRef) {
+            b = (pl & 1u ? (b & 15u) : 0u) | (pl & 2u ? (b & 64u) : 0u);
+        } else {
+            int top = 0;
+            long long best = pool[j][0];
+#pragma unroll
+            for (int k = 1; k < 6; ++k)
+                if (pool[j][k] > best) { best = pool[j][k]; top = k; }  // first maximum
+            b = pl & 1u ? b & ~(1u << top) : 0u;
+        }
+        q.bits[j] = b;
+    }
+}
+
+template <bool kRef>
+__global__ void __launch_bounds__(A_THREADS, 2)
+variant_multi_sums_kernel(MultiVariantArgs<kRef> a, uint32_t* __restrict__ block_sums) {
+    variant_sums(a, block_sums);
+}
+
+// Records: site_slot[i], site_mask[i] (pooled: bits 0-5 = alleles A, C, G, T, N, deletions; reference: bits 0-3 SNV
+// alleles, bit 6 the insertion candidate), in ascending slot order.
+template <bool kRef>
+__global__ void __launch_bounds__(A_THREADS, 2)
+variant_multi_scatter_kernel(MultiVariantArgs<kRef> a, const uint32_t* __restrict__ block_sums, long long n_sites,
+                             int64_t* __restrict__ site_slot, uint8_t* __restrict__ site_mask) {
+    variant_scatter(a, block_sums, n_sites, typename MultiVariantArgs<kRef>::Out{site_slot, site_mask});
+}
+
 // ---- K7: deletion events -------------------------------------------------------------------------------------
 // One thread per read.  Simple reads (l_seq bit 31 clear) have no D op.  A complex read's CIGAR block sits behind its
 // bases in seq4: [n_ops][evt_off][ops...].  The reference cursor moves as in kindel.py:40-81 (K1g restates it): M / = /

@@ -496,6 +496,42 @@ def variant_sites_ref(counts: torch.Tensor, contig_slot, contig_len, ref, abs_th
                 site_mask.cpu().numpy())
 
 
+def variant_sites_multi(counts: torch.Tensor, contig_slot, contig_len, ref, abs_threshold, rel_threshold):
+    """K6m (extension): the sites of several samples at once in a stacked device table (int32[S, 7, n_slots],
+    contiguous, n_slots % 4 == 0; sample s's columns 0-6 over one shared layout).  ref None: the pooled mode (bits
+    0-5, the alleles of kindel.variant_alleles tested in each sample, the pooled top left out); else reference codes
+    as for variant_sites_ref (bits 0-3 SNV alleles, bit 6 the insertion candidate, each sample tested against its own
+    DPa).  Each bit is ORed over the samples (include/kindel_b200.h has the rule).  Returns (slot int64[n], mask
+    uint8[n]) as device tensors in ascending slot order; the samples' rows stay in `counts`."""
+    lib = _ffi.load()
+    dev = counts.device
+    if counts.dim() != 3 or counts.shape[1] != 7 or counts.dtype != torch.int32 or not counts.is_contiguous():
+        raise ValueError("the stacked table must be a contiguous int32[S, 7, n_slots], got %s %s"
+                         % (counts.dtype, tuple(counts.shape)))
+    n_samples, n_slots = int(counts.shape[0]), int(counts.shape[2])
+    a, r = variant_abs_floor(abs_threshold), float(rel_threshold)
+    with torch.cuda.device(dev):
+        ref_ptr = None
+        if ref is not None:
+            if not isinstance(ref, torch.Tensor):
+                ref = torch.from_numpy(np.ascontiguousarray(ref, dtype=np.uint8))
+            ref = ref.to(dev).contiguous()
+            if ref.dtype != torch.uint8 or ref.numel() != n_slots:
+                raise ValueError("reference codes must be uint8[%d], got %s[%d]" % (n_slots, ref.dtype, ref.numel()))
+            ref_ptr = ref.data_ptr()
+        t_slot, t_len, n_contigs = _device_layout(contig_slot, contig_len, dev)
+        sums = torch.empty(int(lib.kdl_variant_scratch_words(n_slots)), dtype=torch.int32, device=dev)
+        args = (counts.data_ptr(), n_samples, n_slots, t_slot.data_ptr(), t_len.data_ptr(), n_contigs, ref_ptr, a, r,
+                sums.data_ptr())
+        _ffi.check(lib.kdl_variant_multi_count(*args, _stream_ptr(dev)), "kdl_variant_multi_count")
+        n = int(sums[-1].item()) & 0xFFFFFFFF
+        site_slot = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+        site_mask = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        rc = lib.kdl_variant_multi_scatter(*args, n, site_slot.data_ptr(), site_mask.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_variant_multi_scatter")
+    return site_slot[:n], site_mask[:n]
+
+
 _SELECT_TOTALS = 16  # words of K8's totals record (include/kindel_b200.h)
 
 

@@ -1045,7 +1045,8 @@ _VCF_ALT = ((0, "A"), (1, "C"), (2, "G"), (3, "T"), (5, "*"))  # N (4) is not an
 
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
-                 exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None, mask_overlaps=False) -> str:
+                 exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None, mask_overlaps=False,
+                 samples=None) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -1069,9 +1070,27 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     neither), and the header gets `##kindelPrimers=<the BED's file name>`.
 
     mask_overlaps (extension: `--mask-overlaps`): see pileup_run; DP, AD, AO and the strand counts then count each
-    read pair once where its mates overlap, and the header gets `##kindelMateOverlaps=R2 masked where R1 covers`."""
+    read pair once where its mates overlap, and the header gets `##kindelMateOverlaps=R2 masked where R1 covers`.
+
+    bam_path a list or tuple of paths (extension: `kindel variants --vcf a.bam b.bam ...`): one VCF of all the
+    samples, one FORMAT column each (DP:AD:AF), named by `samples` (unique, non-empty, no whitespace) or else by the
+    files' names without their directories.  A record is written where some sample passes; INFO holds the values
+    pooled over the samples, and without a reference REF is the pooled most frequent allele.  The options apply to
+    every sample as they would to that sample alone; strand / max_sor are not available with a list (ValueError).
+    kindel_b200/cohort.py has the layout and the union rules; a list of one path gives the data lines of that path
+    alone in columns 1-8."""
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
+    if isinstance(bam_path, (list, tuple)):
+        if strand:
+            raise ValueError("strand and max_sor are not available with several samples")
+        from . import cohort
+
+        return cohort.variants_vcf(bam_path, abs_threshold, rel_threshold, devices, min_base_quality, min_mapq,
+                                   exclude_flags, reference=reference, primers=primers, mask_overlaps=mask_overlaps,
+                                   samples=samples)
+    if samples is not None:
+        raise ValueError("samples= names the columns of several samples: pass the alignment files as a list")
     filters = (min_base_quality, min_mapq, exclude_flags)
     run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers, mask_overlaps=mask_overlaps)[0]
     return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference, strand=strand,

@@ -56,6 +56,8 @@ def row(path: str, d: dict) -> str:
         work += ", + primer masking (K9, K1q)"
     if d.get("mates_ms"):
         work += ", + mate-overlap masking (K10p, K10, K10u)"
+    if d.get("cohort_ms"):
+        work += ", multi-sample VCF (%d samples, K6m)" % cfg.get("samples", 0)
     if d.get("map_ab"):
         work += ", zeroing A/B (dirty-sector map)"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
