@@ -447,6 +447,23 @@ int kdl_overlap_apply(const kdl_batch* batch, const kdl_qmask* qmask, const int3
                       uint32_t* seq4, const kdl_qmask* out_mask, int32_t* drops, int64_t n_drops, void* stream);
 int kdl_overlap_untake(const int32_t* drops, int64_t n_drops, int32_t* counts, int64_t n_slots, void* stream);
 
+/* K11 (extension: `variants --vcf --qual`): the base qualities of the counted bases, summed per slot.  The counted
+ * bases are exactly those the pileup counts in columns 0-3: M/=/X bases whose nibble in seq4 is A, C, G or T (so a base
+ * masked by quality, primer or mate overlap -- an N nibble -- counts nowhere; clipped and inserted bases, N and
+ * deletions add nothing), along K1g's walk for KDL_HARD reads (Python index wrap included).
+ *   qual8[8 * seq4_words]  uint8, 8-byte aligned: the Phred quality of base k of read r at byte 8 * seq_off[r] + k
+ *                          (kdl_bam_fill_qual); a tile's qualities are the bytes [8 * wa, 8 * wend) of its words
+ *   qsum[4][n_slots]       uint32, 16-byte aligned: the summed Phred of the counted A / C / G / T bases of each slot
+ *   emass[n_slots]         uint64, 16-byte aligned: the summed EPS[min(q, 93)] of each slot's counted bases, EPS[q] the
+ *                          integer nearest to 2^32 * 10^(-q / 10)
+ * Both tables are written whole (no zeroing needed); the sums are integers, so the result is independent of order.
+ * With constant qualities q, qsum[k][s] == q * counts[k][s].  A coordinate-sorted batch with tile_index takes K0 (into
+ * tile_index, so no ordering dependency on kdl_pileup) + K11 (one CTA per tile, plain stores) + K11g (KDL_HARD reads,
+ * global atomics); any other batch a zeroing pass + K11g over every read.  Reads the batch's seq4 as it is: after K9 /
+ * K10 when they run.  n_slots % 4 == 0.  Device pointers. */
+int kdl_quality_pileup(const kdl_batch* batch, const uint8_t* qual8, uint32_t* qsum, uint64_t* emass, int64_t n_slots,
+                       void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced
@@ -554,7 +571,10 @@ int kdl_ctx_last_timing(kdl_ctx* ctx, float* h2d_ms, float* kernel_ms, float* d2
  *                    info[14] = reads with masked bases
  *   kdl_bam_fill_mask   after fill: the kdl_qmask arrays, read_idx [info[14]], off [info[14] + 1], qpos [info[13]]
  *   kdl_bam_fill_strand after fill (extension): reverse [n_kept], 1 where the kept read's FLAG has 0x10, in read order
- *   kdl_bam_fill_mates  after fill (extension): name_hash / mate_start / pair_role [n_kept] of K10, in read order */
+ *   kdl_bam_fill_mates  after fill (extension): name_hash / mate_start / pair_role [n_kept] of K10, in read order
+ *   kdl_bam_fill_qual   after fill (extension): qual8 [8 * words of seq4], the Phred quality of base k of read r at byte
+ *                    8 * seq_off[r] + k, 0xff for a complex read's trailer words and the padding.  prepare's info[15] =
+ *                    kept reads without qualities (BAM 0xff, SAM `*`): their bytes are 0xff too */
 typedef struct kdl_bam kdl_bam;
 int kdl_bam_open(const char* path, int threads, kdl_bam** out);
 void kdl_bam_close(kdl_bam* h);
@@ -571,6 +591,7 @@ int kdl_bam_set_filter(kdl_bam* h, int32_t min_mapq, int32_t exclude_flags, int3
 int kdl_bam_fill_mask(kdl_bam* h, int threads, uint32_t* read_idx, uint32_t* off, uint32_t* qpos);
 int kdl_bam_fill_strand(kdl_bam* h, int threads, uint8_t* reverse);
 int kdl_bam_fill_mates(kdl_bam* h, int threads, uint64_t* name_hash, int32_t* mate_start, uint8_t* pair_role);
+int kdl_bam_fill_qual(kdl_bam* h, int threads, uint8_t* qual8);
 
 #ifdef __cplusplus
 }

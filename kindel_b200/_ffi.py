@@ -165,6 +165,7 @@ _PROTOTYPES = {
     "kdl_overlap_apply": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.POINTER(KdlQmask), C.c_void_p, C.c_int64, C.c_void_p]),
     "kdl_overlap_untake": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
+    "kdl_quality_pileup": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "kdl_vote_peers":(C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,
@@ -200,6 +201,7 @@ _PROTOTYPES = {
     "kdl_bam_fill_mask": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_bam_fill_strand": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "kdl_bam_fill_mates": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_bam_fill_qual": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -29,6 +29,8 @@ read at all.
 With `strand=True` the batch also keeps each kept read's strand (`reverse`, FLAG & 0x10), which `variants --vcf
 --strand` splits the pileup by; it costs nothing when off.  With `mates=True` it keeps what `--mask-overlaps` pairs the
 reads by (`name_hash`, `mate_start`, `pair_role`: include/kindel_b200.h K10 has the rule); nothing is decoded when off.
+With `qual=True` it keeps every base's quality beside its bases (`qual8`, which K11 sums for `variants --vcf --qual`);
+a kept read without qualities is then a ValueError naming the file: nothing is guessed.
 
 The result is a `ReadBatch` (numpy arrays in host memory) described in include/kindel_b200.h.
 """
@@ -94,6 +96,9 @@ class ReadBatch:
     name_hash: np.ndarray = field(default=None)     # uint64 [n]
     mate_start: np.ndarray = field(default=None)    # int32 [n]
     pair_role: np.ndarray = field(default=None)     # uint8 [n]
+    # base qualities (extension; `qual=True` at decode, K11): base k of read r at byte 8 * seq_off[r] + k, 0xff for the
+    # padding and a complex read's trailer words.  None = not asked for; select_reads and the shards leave it behind.
+    qual8: np.ndarray = field(default=None)         # uint8 [8 * words of seq4]
 
     @property
     def mates(self):
@@ -610,13 +615,14 @@ def decode_threads() -> int:
 
 
 def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0, exclude_flags: int = 0,
-             min_base_quality: int = 0, strand: bool = False, mates: bool = False) -> ReadBatch:
+             min_base_quality: int = 0, strand: bool = False, mates: bool = False, qual: bool = False) -> ReadBatch:
     """.bam -> ReadBatch through the C++ decoder (bam_host.cpp): BGZF inflate, filter, classification and the
     device layout (inline CIGAR blocks included) in threads, no Python per-record or per-array work.
     pinned=True puts the arrays the device consumes into page-locked memory (needs torch + CUDA).
     min_mapq / exclude_flags / min_base_quality: the filters of this module's docstring (extension).  strand=True
     (extension): also the kept reads' strands, `reverse` (kdl_bam_fill_strand).  mates=True (extension): also
-    `name_hash`, `mate_start` and `pair_role` (kdl_bam_fill_mates)."""
+    `name_hash`, `mate_start` and `pair_role` (kdl_bam_fill_mates).  qual=True (extension): also `qual8`, the
+    qualities beside the bases (kdl_bam_fill_qual); a kept read without qualities is a ValueError."""
     import ctypes as C
 
     filters = check_filters(min_mapq, exclude_flags, min_base_quality)
@@ -687,6 +693,11 @@ def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0,
                         pair_role=np.zeros(n, dtype=np.uint8))
             ptrs = [mask[f].ctypes.data if n else None for f in _MATE_FIELDS]
             _ffi.check(lib.kdl_bam_fill_mates(h, threads, *ptrs), "kdl_bam_fill_mates")
+        if qual:
+            if int(info[15]):
+                raise ValueError(missing_qualities(path, int(info[15])))
+            mask["qual8"] = np.empty(8 * n_words, dtype=np.uint8)
+            _ffi.check(lib.kdl_bam_fill_qual(h, threads, mask["qual8"].ctypes.data if n else None), "kdl_bam_fill_qual")
     finally:
         lib.kdl_bam_close(h)
     return ReadBatch(
@@ -695,6 +706,23 @@ def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0,
         cigar=cigar, seq4=stream, hard_idx=hard_idx, complex_idx=cx_idx, n_events=int(info[8]),
         reads_sorted=bool(info[12]) or n < 2, aligned_bases=int(info[7]), n_records=n_rec,
         max_simple_len=int(info[11]), reach_right=int(info[9]), reach_left=int(info[10]), **mask)
+
+
+def missing_qualities(path, n: int) -> str:
+    return "%s: %d kept read(s) without base qualities (QUAL `*` or 0xff); --qual needs them" % (os.fspath(path), n)
+
+
+def qual_layout(batch: ReadBatch, qual: np.ndarray) -> np.ndarray:
+    """The qual8 of a batch from its reads' qualities concatenated in read order (seq_len bytes per read): base k of
+    read r at byte 8 * seq_off[r] + k, 0xff elsewhere (include/kindel_b200.h kdl_quality_pileup)."""
+    qual = np.asarray(qual, dtype=np.uint8)
+    lens = np.asarray(batch.seq_len, dtype=np.int64)
+    if qual.shape[0] != int(lens.sum()):
+        raise ValueError("qualities must hold exactly one byte per base")
+    out = np.full(8 * int(batch.seq4.shape[0]), 0xFF, dtype=np.uint8)
+    starts = 8 * np.asarray(batch.seq_off, dtype=np.int64)
+    out[np.repeat(starts - (np.cumsum(lens) - lens), lens) + np.arange(qual.shape[0], dtype=np.int64)] = qual
+    return out
 
 
 # ---------------------------------------------------------------------------------------- SAM
@@ -756,11 +784,11 @@ def _sam_qual(text: str, seq: str) -> bytes:
 
 
 def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0,
-             strand: bool = False, mates: bool = False) -> ReadBatch:
+             strand: bool = False, mates: bool = False, qual: bool = False) -> ReadBatch:
     min_mapq, exclude_flags, min_base_quality = check_filters(min_mapq, exclude_flags, min_base_quality)
     header = []
     groups = {}  # rname -> list of (pos0, cigar words, seq, qualities, reverse, (name hash, PNEXT - 1, role))
-    n_records = 0
+    n_records = n_noqual = 0
     with open(path, "rt") as fh:
         for line in fh:
             if line.startswith("@"):
@@ -785,7 +813,9 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
                     raise ValueError("MAPQ %d out of range" % mapq)
                 if mapq < min_mapq:
                     continue
-            qual = _sam_qual(f[10], seq) if min_base_quality else None
+            qv = _sam_qual(f[10], seq) if (min_base_quality or qual) else None
+            if qual and f[10] == "*":
+                n_noqual += 1
             mate = None
             if mates:
                 try:
@@ -794,7 +824,7 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
                     pnext = -1
                 mate = (name_hash(f[0]), pnext - 1 if 0 <= pnext < (1 << 31) else -1,
                         pair_role(flag, f[6] == "=" or f[6] == rname))
-            g.append((int(f[3]) - 1, parse_cigar_text(f[5]), seq, qual, 1 if flag & 0x10 else 0, mate))
+            g.append((int(f[3]) - 1, parse_cigar_text(f[5]), seq, qv, 1 if flag & 0x10 else 0, mate))
     groups.pop("*", None)  # kindel.py:147-148
     names, lens = _sq_from_text("\n".join(header))
     sq = dict(zip(names, lens))
@@ -820,26 +850,33 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
             mate_rows.append(mate)
         read_off.append(len(ref_start))
     seq4 = np.concatenate(seq_parts) if seq_parts else np.zeros(0, dtype=np.uint32)
-    qual = np.frombuffer(b"".join(quals), dtype=np.uint8) if min_base_quality else None
-    return finalize(contig_names, np.array([sq[nm] for nm in contig_names], dtype=np.int64),
+    if n_noqual:
+        raise ValueError(missing_qualities(path, n_noqual))
+    quals = np.frombuffer(b"".join(quals), dtype=np.uint8) if (min_base_quality or qual) else None
+    batch = finalize(contig_names, np.array([sq[nm] for nm in contig_names], dtype=np.int64),
                     np.array(read_off, dtype=np.int64), np.array(ref_start, dtype=np.int64),
                     np.array(seq_off, dtype=np.int64), np.array(l_seq, dtype=np.int64),
                     np.array(cig_off, dtype=np.int64), np.array(cigar, dtype=np.int64), seq4,
-                    n_records=n_records, qual=qual, min_base_quality=min_base_quality,
-                    reverse=np.array(rev, dtype=np.uint8) if strand else None,
-                    mates=tuple(np.array([m[k] for m in mate_rows], dtype=dt) for k, dt in
-                                enumerate((np.uint64, np.int64, np.uint8))) if mates else None)
+                     n_records=n_records, qual=quals, min_base_quality=min_base_quality,
+                     reverse=np.array(rev, dtype=np.uint8) if strand else None,
+                     mates=tuple(np.array([m[k] for m in mate_rows], dtype=dt) for k, dt in
+                                 enumerate((np.uint64, np.int64, np.uint8))) if mates else None)
+    if qual:
+        batch.qual8 = qual_layout(batch, quals)
+    return batch
 
 
 def read_alignment(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0,
-                   strand: bool = False, mates: bool = False) -> ReadBatch:
-    """.bam or .sam (by content, not by suffix) -> ReadBatch.  The filters, strand and mates (extensions): see the
-    module docstring."""
+                   strand: bool = False, mates: bool = False, qual: bool = False) -> ReadBatch:
+    """.bam or .sam (by content, not by suffix) -> ReadBatch.  The filters, strand, mates and qualities (extensions):
+    see the module docstring."""
     path = os.fspath(path)
     filters = dict(zip(("min_mapq", "exclude_flags", "min_base_quality"),
                        check_filters(min_mapq, exclude_flags, min_base_quality)), strand=bool(strand))
     if mates:  # (the keyword only when asked: a reader without it stays as it was)
         filters["mates"] = True
+    if qual:
+        filters["qual"] = True
     with open(path, "rb") as fh:
         magic = fh.read(4)
     if magic[:2] == b"\x1f\x8b" or magic == b"BAM\x01":

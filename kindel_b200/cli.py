@@ -6,7 +6,7 @@ extension one FASTQ record per contig instead),
 `weights` / `features` write TSV to stdout (cli.py:44,50), `version` prints `kindel <version>`;
 `variants` (in the reference's README only) is an extension, see kindel.variants; its `--vcf` writes a sites-only VCF
 (kindel.variants_vcf), against a FASTA with `--reference`, with per-strand counts and a strand odds ratio with
-`--strand` / `--max-sor`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
+`--strand` / `--max-sor`, with a base-quality QUAL with `--qual` / `--min-qual`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
 bases of every read before the pileup (kindel_b200/primers.py); `--mask-overlaps` counts each read pair once where
 its mates overlap (include/kindel_b200.h K10).
 argh derived the flags from the function signatures (first letter as short option unless two
@@ -54,7 +54,7 @@ def features(bam_path, gpus=None, **filters):
 
 
 def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False, absolute=False, gpus=None, vcf=False,
-             reference=None, strand=False, max_sor=None, **filters):
+             reference=None, strand=False, max_sor=None, qual=False, min_qual=None, **filters):
     """Output variants exceeding specified absolute and relative frequency thresholds"""
     from . import kindel
 
@@ -62,6 +62,8 @@ def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False,
         extra = {} if reference is None else dict(reference=reference)
         if strand or max_sor is not None:  # extension: ADF / ADR / SOR (and FILTER sor)
             extra.update(strand=True, max_sor=max_sor)
+        if qual or min_qual is not None:  # extension: QUAL, BQ / AQ (and FILTER lowqual)
+            extra.update(qual=True, min_qual=min_qual)
         sys.stdout.write(kindel.variants_vcf(bam_path, abs_threshold, rel_threshold, devices=gpus, **filters, **extra))
         return
     kindel.variants(bam_path, abs_threshold, rel_threshold, only_variants, absolute, devices=gpus, **filters).to_csv(
@@ -117,6 +119,12 @@ def _max_sor(text: str) -> float:
     from .kindel import check_max_sor
 
     return check_max_sor(float(text))  # ValueError (NaN) -> argparse error
+
+
+def _min_qual(text: str) -> float:
+    from .kindel import check_min_qual
+
+    return check_min_qual(float(text))  # ValueError (NaN) -> argparse error
 
 
 def _filters(a) -> dict:
@@ -200,9 +208,14 @@ def build_parser() -> argparse.ArgumentParser:
                    help="with --vcf: add ADF / ADR (per-strand allele counts) and SOR (strand odds ratio) to INFO")
     p.add_argument("--max-sor", type=_max_sor, default=None, metavar="X",
                    help="with --vcf: FILTER `sor` where an ALT's strand odds ratio is above X (implies --strand)")
+    # extension: a QUAL from the reads' base qualities, the per-allele qualities in INFO, and a filter on it
+    p.add_argument("--qual", action="store_true",
+                   help="with --vcf: QUAL from the base qualities (Poisson error model), BQ / AQ in INFO")
+    p.add_argument("--min-qual", type=_min_qual, default=None, metavar="X",
+                   help="with --vcf: FILTER `lowqual` where QUAL is below X (implies --qual)")
     p.set_defaults(func=lambda a: variants(a.bam_path[0] if len(a.bam_path) == 1 else a.bam_path, a.abs_threshold,
                                            a.rel_threshold, a.only_variants, a.absolute, a.gpus, a.vcf, a.reference,
-                                           a.strand, a.max_sor, **_filters(a)))
+                                           a.strand, a.max_sor, a.qual, a.min_qual, **_filters(a)))
 
     p = sub.add_parser("plot", help=plot.__doc__, description=plot.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")
@@ -221,6 +234,8 @@ def _check_variants_args(parser, args):
             parser.error("variants: several alignment files need --vcf (the table has no sample columns)")
         if args.strand or args.max_sor is not None:
             parser.error("variants: --strand and --max-sor take one alignment file")
+        if args.qual or args.min_qual is not None:
+            parser.error("variants: --qual and --min-qual take one alignment file")
     if getattr(args, "vcf", False):
         for flag, on in (("--absolute", args.absolute), ("--only-variants", args.only_variants)):
             if on:
@@ -229,6 +244,8 @@ def _check_variants_args(parser, args):
         parser.error("variants: --reference needs --vcf (the table has no reference mode)")
     elif getattr(args, "strand", False) or getattr(args, "max_sor", None) is not None:
         parser.error("variants: --strand and --max-sor need --vcf (the table has no strand columns)")
+    elif getattr(args, "qual", False) or getattr(args, "min_qual", None) is not None:
+        parser.error("variants: --qual and --min-qual need --vcf (the table has no QUAL)")
 
 
 def main(argv=None):

@@ -16,6 +16,7 @@
 #include "select.cu"
 #include "primers.cu"
 #include "mates.cu"
+#include "quality.cu"
 
 namespace {
 
@@ -776,6 +777,42 @@ int kdl_overlap_untake(const int32_t* drops, int64_t n_drops, int32_t* counts, i
     if (n_drops == 0) return KDL_OK;
     KDL_LAUNCH(kdl::overlap_untake_kernel, (unsigned)((n_drops + kdl::M_THREADS - 1) / kdl::M_THREADS),
                kdl::M_THREADS, 0, (cudaStream_t)stream, drops, n_drops, counts, n_slots);
+    return check_launch();
+}
+
+int kdl_quality_pileup(const kdl_batch* batch, const uint8_t* qual8, uint32_t* qsum, uint64_t* emass, int64_t n_slots,
+                       void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (!qsum || !emass || n_slots <= 0 || (n_slots & 3) || (batch->n_reads > 0 && !qual8) ||
+        (reinterpret_cast<uintptr_t>(qual8) & 7) || (reinterpret_cast<uintptr_t>(qsum) & 15) ||
+        (reinterpret_cast<uintptr_t>(emass) & 15))
+        return KDL_ERR_INVALID_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned long long* em = reinterpret_cast<unsigned long long*>(emass);
+    const int cap = sm_count() * 8;
+    // the tile-owner path under the conditions of kdl_pileup_range's
+    const bool tiled = batch->n_reads > batch->n_hard && (n_slots % KDL_TILE) == 0 && batch->reads_sorted &&
+                       batch->tile_index && batch->reach_right > 0 &&
+                       batch->reach_right <= KDL_FAST_MAXLEN + KDL_TILE_MAXREACH;
+    if (tiled) {
+        const long long n_tiles = n_slots / KDL_TILE;
+        KDL_LAUNCH(kdl::tile_index_kernel, (unsigned)((n_tiles * 32 + 255) / 256), 256, 0, st, *batch, 0ll, n_tiles,
+                   batch->tile_index);  // K0, into the caller's scratch: no ordering dependency on kdl_pileup
+        if ((rc = check_launch()) != KDL_OK) return rc;
+        KDL_LAUNCH(kdl::quality_tile_kernel, (unsigned)n_tiles, kdl::kQtThreads, 0, st, *batch, qual8, qsum, em, n_slots,
+                   batch->tile_index);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+        if (batch->n_hard == 0) return KDL_OK;
+        KDL_LAUNCH(kdl::quality_general_kernel, grid_for(batch->n_hard, 8, cap), 256, 0, st, *batch, qual8,
+                   batch->hard_idx, batch->n_hard, qsum, em, n_slots);
+        return check_launch();
+    }
+    KDL_LAUNCH(kdl::quality_zero_kernel, sm_count() * 4, 256, 0, st, qsum, em, n_slots);
+    if ((rc = check_launch()) != KDL_OK) return rc;
+    if (batch->n_reads == 0) return KDL_OK;
+    KDL_LAUNCH(kdl::quality_general_kernel, grid_for(batch->n_reads, 8, cap), 256, 0, st, *batch, qual8, nullptr,
+               batch->n_reads, qsum, em, n_slots);
     return check_launch();
 }
 

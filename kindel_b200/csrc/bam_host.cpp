@@ -589,6 +589,7 @@ struct kdl_bam {
     std::vector<uint32_t> n_masked;     // per record, only when filter.min_bq > 0
     std::vector<int64_t> cur_mread, cur_mbase;  // [task][n_ref] start cursors of the mask list
     int64_t masked_bases = 0, masked_reads = 0;
+    int64_t no_qual = 0;                // kept reads without qualities (BAM 0xff, SAM `*`)
     int64_t n_records = 0, n_kept = 0, n_complex = 0, n_hard = 0, aligned = 0, n_events = 0;
     int64_t reach_right = 0, reach_left = 0, max_simple = 0;
     int32_t reads_sorted = 1;
@@ -773,7 +774,8 @@ int kdl_bam_set_filter(kdl_bam* h, int32_t min_mapq, int32_t exclude_flags, int3
 // ref_len[n_ref]: the contig lengths to classify against (the @SQ text's LN, as the reference uses; NULL = the binary
 // dictionary's).  info[16] out: 0 records, 1 kept reads, 2 contigs seen, 3 CIGAR ops of kept reads, 4 words of the
 // read stream, 5 complex reads, 6 hard reads, 7 aligned bases, 8 insertion events, 9 reach_right, 10 reach_left,
-// 11 longest simple read, 12 reads_sorted (valid after kdl_bam_fill), 13 masked bases, 14 reads with masked bases.
+// 11 longest simple read, 12 reads_sorted (valid after kdl_bam_fill), 13 masked bases, 14 reads with masked bases,
+// 15 kept reads without qualities.
 int kdl_bam_prepare(kdl_bam* h, const int32_t* ref_len, int threads, int64_t* info) {
     if (!h || !info) return KDL_ERR_INVALID_ARG;
     const uint8_t* d = h->dptr;
@@ -797,7 +799,7 @@ int kdl_bam_prepare(kdl_bam* h, const int32_t* ref_len, int threads, int64_t* in
     struct Acc { int64_t kept = 0, ops = 0, words = 0, first = -1, mreads = 0, mbases = 0; };  // first: record index inside the task
     const size_t row = (size_t)std::max(1, n_ref);
     std::vector<Acc> acc((size_t)n_tasks * row);
-    struct Tot { int64_t cx = 0, hard = 0, aligned = 0, rr = 0, rl = 0, ms = 0; };
+    struct Tot { int64_t cx = 0, hard = 0, aligned = 0, rr = 0, rl = 0, ms = 0, noq = 0; };
     struct Task { std::vector<int64_t> off; std::vector<Class> cls; std::vector<uint32_t> nm; Tot tot; int64_t start = -1, end = -1; bool bad = false; };
     const Filter flt = h->filter;
     std::vector<Task> task((size_t)n_tasks);
@@ -853,6 +855,7 @@ int kdl_bam_prepare(kdl_bam* h, const int32_t* ref_len, int threads, int64_t* in
                     ac.ops += r.n_cigar;
                     ac.words += ((int64_t)r.l_seq + 7) / 8 + (c.cls == CLS_SIMPLE ? 0 : 2 + (int64_t)r.n_cigar);
                     tk.tot.aligned += al;
+                    if (!r.qual || r.qual[0] == 0xff) tk.tot.noq += 1;  // a kept read without qualities
                     if (c.cls != CLS_SIMPLE) tk.tot.cx += 1;
                     if (c.cls == CLS_HARD) tk.tot.hard += 1;
                     if (c.cls == CLS_SIMPLE && rr > tk.tot.ms) tk.tot.ms = rr;
@@ -907,11 +910,11 @@ int kdl_bam_prepare(kdl_bam* h, const int32_t* ref_len, int threads, int64_t* in
             if (a[c].first >= 0) a[c].first += (int64_t)base;  // -> index over all records
     });
     pt.lap("prepare: verify + gather");
-    h->n_complex = h->n_hard = h->aligned = 0;
+    h->n_complex = h->n_hard = h->aligned = h->no_qual = 0;
     h->reach_right = h->reach_left = h->max_simple = 0;
     for (const Task& tk : task) {
         const Tot& tt = tk.tot;
-        h->n_complex += tt.cx; h->n_hard += tt.hard; h->aligned += tt.aligned;
+        h->n_complex += tt.cx; h->n_hard += tt.hard; h->aligned += tt.aligned; h->no_qual += tt.noq;
         h->reach_right = std::max(h->reach_right, tt.rr); h->reach_left = std::max(h->reach_left, tt.rl);
         h->max_simple = std::max(h->max_simple, tt.ms);
     }
@@ -960,7 +963,7 @@ int kdl_bam_prepare(kdl_bam* h, const int32_t* ref_len, int threads, int64_t* in
     info[0] = n_rec; info[1] = h->n_kept; info[2] = (int64_t)ns; info[3] = h->op_off[ns]; info[4] = h->word_off[ns];
     info[5] = h->n_complex; info[6] = h->n_hard; info[7] = h->aligned; info[8] = 0;
     info[9] = std::max(h->reach_right, h->max_simple); info[10] = h->reach_left; info[11] = h->max_simple; info[12] = 1;
-    info[13] = h->masked_bases; info[14] = h->masked_reads; info[15] = 0;
+    info[13] = h->masked_bases; info[14] = h->masked_reads; info[15] = h->no_qual;
     return KDL_OK;
 }
 
@@ -1141,6 +1144,35 @@ int kdl_bam_fill_mates(kdl_bam* h, int threads, uint64_t* name_hash, int32_t* ma
             const bool ends = ((f & 0x40u) != 0) != ((f & 0x80u) != 0);
             const bool ok = (f & 0x1u) && !(f & (0x8u | 0x100u | 0x800u)) && ends && rd_i32(q + 20) == r.ref_id;
             pair_role[k] = ok ? ((f & 0x40u) ? 1 : 2) : 0;
+        }
+    });
+    return KDL_OK;
+}
+
+// The qualities of the last prepare's kept reads beside their bases (K11, include/kindel_b200.h): base k of kept read r
+// at byte 8 * seq_off[r] + k of qual8 [8 * words], 0xff for the padding, a complex read's trailer words and every base of
+// a read without qualities (prepare's info[15] counts those reads).
+int kdl_bam_fill_qual(kdl_bam* h, int threads, uint8_t* qual8) {
+    if (!h || !h->prepared || (h->n_kept > 0 && !qual8)) return KDL_ERR_INVALID_ARG;
+    const uint8_t* d = h->dptr;
+    const int32_t n_ref = (int32_t)h->ref_name.size();
+    const int64_t n_tasks = (int64_t)h->chunk_lo.size() - 1;
+    h->pool->run(n_tasks, threads, [&](int64_t t, int) {
+        std::vector<int64_t> cw(h->cur_word.begin() + t * n_ref, h->cur_word.begin() + (t + 1) * n_ref);
+        RecView r;
+        for (int64_t i = h->chunk_lo[(size_t)t]; i < h->chunk_lo[(size_t)t + 1]; ++i) {
+            const Class c = h->cls[(size_t)i];
+            if (c.cls == CLS_DROP) continue;
+            const int64_t off_i = h->rec_off[(size_t)i];
+            parse_record(d + off_i, h->rec_off[(size_t)i + 1] - off_i, &r);
+            const size_t ci = (size_t)r.ref_id;
+            const int64_t w = cw[ci], n_words = ((int64_t)r.l_seq + 7) / 8;
+            const int64_t total = n_words + (c.cls == CLS_SIMPLE ? 0 : 2 + (int64_t)r.n_cigar);
+            cw[ci] += total;
+            uint8_t* out = qual8 + 8 * w;
+            const bool has = r.qual && r.qual[0] != 0xff;
+            if (has) std::memcpy(out, r.qual, (size_t)r.l_seq);
+            std::memset(out + (has ? r.l_seq : 0), 0xff, (size_t)(8 * total - (has ? r.l_seq : 0)));
         }
     });
     return KDL_OK;

@@ -18,6 +18,7 @@ implementation behind these functions: without a CUDA device they raise.
     mask_primers(dbatch, arrays)  K9: the batch with its amplicon primer bases masked (extension)
     mask_overlaps(dbatch)      K10p + K10: the batch with its read pairs' second mates masked where the first covers
                                (extension); pileup then runs K10u
+    quality_sums(dbatch, qual8)  K0 + K11 + K11g: the counted bases' qualities summed per slot (extension)
 """
 from __future__ import annotations
 
@@ -711,6 +712,25 @@ def mask_overlaps(dbatch: DeviceBatch, mate: torch.Tensor = None) -> DeviceBatch
                                    drops.data_ptr() if n_drops else None, n_drops, _stream_ptr(dev))
         _ffi.check(rc, "kdl_overlap_apply")
     return dataclasses.replace(dbatch, tensors=tensors, qmask=q, drops=drops, overlap_masked=stats)
+
+
+def quality_sums(dbatch: DeviceBatch, qual8: torch.Tensor):
+    """K0 + K11 (+ K11g): (qsum int32 [4, n_slots] holding uint32 bits, emass int64 [n_slots] holding uint64 bits) on
+    the device -- per slot the summed Phred of the counted A / C / G / T bases and the summed EPS of all of them
+    (include/kindel_b200.h kdl_quality_pileup).  qual8: uint8 [8 * words of seq4] on the batch's device.  Reads the
+    batch's seq4 as it is now, so after K9 / K10 a primer or overlap base counts nowhere; the batch's tile-index
+    scratch is rebuilt."""
+    lib = _ffi.load()
+    dev = dbatch.device
+    n_slots = dbatch.n_slots
+    with torch.cuda.device(dev):
+        qsum = torch.empty((4, n_slots), dtype=torch.int32, device=dev)
+        emass = torch.empty(n_slots, dtype=torch.int64, device=dev)
+        q = qual8 if qual8.numel() else torch.zeros(8, dtype=torch.uint8, device=dev)
+        rc = lib.kdl_quality_pileup(C.byref(dbatch.struct), q.data_ptr(), qsum.data_ptr(), emass.data_ptr(), n_slots,
+                                    _stream_ptr(dev))
+        _ffi.check(rc, "kdl_quality_pileup")
+    return qsum, emass
 
 
 def dropped_event_rows(dbatch: DeviceBatch) -> np.ndarray:

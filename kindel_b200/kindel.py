@@ -56,6 +56,7 @@ class PileupRun:
 
     _device = None   # (count table, DeviceBatch) of host tables, uploaded on demand (device_tables)
     _reverse = None  # (count table, DeviceBatch) of the reverse-strand reads (reverse_table)
+    _quality = None  # (qsum, emass) of the counted bases' qualities (quality_table)
     primers = None   # the PrimerSet whose primer bases the pileup masked (extension), None when off
     mask_overlaps = False  # the pileup counted each read pair once where its mates overlap (extension, K10)
     _dropped_events = None  # K10's dropped insertion-event rows of host tables
@@ -122,6 +123,20 @@ class PileupRun:
             sub = engine.select_reads(dbatch, keep)
             self._reverse = (engine.pileup(sub)[0], sub)
         return self._reverse
+
+    def quality_table(self):
+        """(qsum int32 [4, n_slots], emass int64 [n_slots]) on a device, built once (extension: `variants --vcf
+        --qual`): K11 over the run's masked device batch (device_tables(), so a multi-GPU result too) and its qual8,
+        uploaded here and only here.  The bits are uint32 / uint64 (engine.quality_sums).  Needs a batch decoded with
+        qual=True."""
+        if self._quality is None:
+            import torch
+
+            if self.batch.qual8 is None:
+                raise ValueError("qual needs the reads' qualities: decode the batch with qual=True")
+            _, dbatch = self.device_tables()
+            self._quality = engine.quality_sums(dbatch, torch.from_numpy(self.batch.qual8).to(dbatch.device))
+        return self._quality
 
     def vote(self, min_depth=1, iupac_threshold=None) -> np.ndarray:
         """K2 over the whole table -> call bytes on the host (the device copy is kept for K5).  iupac_threshold:
@@ -254,7 +269,7 @@ def _default_devices(devices):
 
 
 def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq=0, exclude_flags=0,
-               iupac_threshold=None, strand=False, primers=None, mask_overlaps=False):
+               iupac_threshold=None, strand=False, primers=None, mask_overlaps=False, qual=False):
     """(PileupRun, calls) of an alignment file on `devices` GPUs.  devices > 1: one process per GPU, reads (or whole
     contigs) sharded, counts exchanged over NVLink in front of the vote (distributed.run_sharded); the result is
     bit-identical to one GPU.  min_base_quality / min_mapq / exclude_flags (extension, all off by default): a record
@@ -268,12 +283,16 @@ def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq
     is counted once where its mates overlap -- the second mate's bases, deletions and insertions there are masked or
     dropped where the first mate has information (K10p / K10 / K10u, include/kindel_b200.h has the rule); the batch is
     then decoded with its mates.  With several GPUs the pairing and the masking run once on this process's GPU, and
-    every rank takes back its own second mates' drops; the result is the same."""
+    every rank takes back its own second mates' drops; the result is the same.  qual (extension, default False =
+    off): the batch keeps its reads' base qualities (PileupRun.quality_table); a kept read without them is a
+    ValueError."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
     primers = as_primer_set(primers)
     decode = dict(min_mapq=min_mapq, exclude_flags=exclude_flags, min_base_quality=min_base_quality, strand=strand)
     if mask_overlaps:  # (the keyword only when on: the decode stays as it was otherwise)
         decode["mates"] = True
+    if qual:
+        decode["qual"] = True
     batch = bamio.read_alignment(bam_path, **decode)
     arrays = primer_arrays(primers, batch.contig_names, batch.contig_len) if primers is not None else None
     devices = _default_devices(devices)
@@ -1046,7 +1065,7 @@ _VCF_ALT = ((0, "A"), (1, "C"), (2, "G"), (3, "T"), (5, "*"))  # N (4) is not an
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
                  exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None, mask_overlaps=False,
-                 samples=None) -> str:
+                 samples=None, qual=False, min_qual=None) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -1078,12 +1097,23 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     pooled over the samples, and without a reference REF is the pooled most frequent allele.  The options apply to
     every sample as they would to that sample alone; strand / max_sor are not available with a list (ValueError).
     kindel_b200/cohort.py has the layout and the union rules; a list of one path gives the data lines of that path
-    alone in columns 1-8."""
+    alone in columns 1-8.
+
+    qual (extension: `--qual`): a base-quality QUAL.  Every record with a base ALT (A, C, G or T) gets QUAL, the largest
+    AQ of its base ALTs, and INFO ;BQ= (the mean Phred of the counted bases of REF and of each ALT, `.` where there is
+    none or the allele is no base) and ;AQ= (per ALT, `.` for `*`).  min_qual (`--min-qual`, implies qual): FILTER
+    `lowqual` where QUAL < min_qual.  A record without a base ALT (an indel, a `*`-only site) keeps QUAL `.`.  The
+    qualities are summed on the device (K11, include/kindel_b200.h); allele_quality has the model.  Not available with
+    several samples (ValueError); a kept read without qualities is a ValueError."""
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
+    min_qual = check_min_qual(min_qual)
+    qual = bool(qual) or min_qual is not None
     if isinstance(bam_path, (list, tuple)):
         if strand:
             raise ValueError("strand and max_sor are not available with several samples")
+        if qual:
+            raise ValueError("qual and min_qual are not available with several samples")
         from . import cohort
 
         return cohort.variants_vcf(bam_path, abs_threshold, rel_threshold, devices, min_base_quality, min_mapq,
@@ -1092,9 +1122,10 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     if samples is not None:
         raise ValueError("samples= names the columns of several samples: pass the alignment files as a list")
     filters = (min_base_quality, min_mapq, exclude_flags)
-    run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers, mask_overlaps=mask_overlaps)[0]
+    run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers, mask_overlaps=mask_overlaps,
+                     qual=qual)[0]
     return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference, strand=strand,
-                                 max_sor=max_sor)
+                                 max_sor=max_sor, qual=qual, min_qual=min_qual)
 
 
 def check_max_sor(max_sor):
@@ -1105,6 +1136,71 @@ def check_max_sor(max_sor):
     if math.isnan(x):
         raise ValueError("max_sor must be a number, got %r" % max_sor)
     return x
+
+
+def check_min_qual(min_qual):
+    """None (no filter) or a float; NaN raises ValueError."""
+    if min_qual is None:
+        return None
+    x = float(min_qual)
+    if math.isnan(x):
+        raise ValueError("min_qual must be a number, got %r" % min_qual)
+    return x
+
+
+QUAL_CAP = 3000
+_EMASS_UNIT = 3.0 * 2.0 ** 32  # emass counts expected errors in units of 2^-32; a third of them hit one given base
+
+
+def allele_quality(k: int, emass: int) -> int:
+    """AQ of a base ALT with count k at a slot whose counted bases sum to emass (K11): with the expected number of
+    errors that turn into this base, lambda = emass / (3 * 2^32), p = P(Poisson(lambda) >= k) =
+    scipy.special.gammainc(k, lambda) -- the Poisson approximation to LoFreq's Poisson-binomial error model -- and AQ =
+    -10 log10(p) rounded half up, clamped to [0, 3000], 3000 when p underflows to 0.  k = 0 gives 0."""
+    from scipy.special import gammainc
+
+    if k <= 0:
+        return 0
+    p = float(gammainc(float(k), float(emass) / _EMASS_UNIT))
+    if p <= 0.0:
+        return QUAL_CAP
+    return min(max(int(math.floor(-10.0 * math.log10(p) + 0.5)), 0), QUAL_CAP)
+
+
+def _qual_fields(ref_col, alt_cols, counts, qsum, emass, min_qual):
+    """(QUAL, lowqual, INFO tail) of a record: ref_col / alt_cols the table columns of REF and of each ALT (0-3 a base,
+    4 N, 5 the deletion, None a reference base that is no base), counts / qsum their counts and quality sums at the
+    record's slot (columns 0-3), emass the slot's.  A record without a base ALT: (".", False, "")."""
+    if not any(k is not None and k < 4 for k in alt_cols):
+        return ".", False, ""
+
+    def bq(k):
+        return "." if k is None or k > 3 or counts[k] == 0 else "%.1f" % (qsum[k] / counts[k])
+
+    aq = [allele_quality(int(counts[k]), emass) if k < 4 else None for k in alt_cols]
+    q = max(a for a in aq if a is not None)
+    tail = ";BQ={};AQ={}".format(",".join(bq(k) for k in [ref_col] + list(alt_cols)),
+                                ",".join("." if a is None else str(a) for a in aq))
+    return str(q), min_qual is not None and q < min_qual, tail
+
+
+def _filter(strand_filter, lowqual):
+    """FILTER from the strand filter (`sor` or PASS) and lowqual, in the order sor, lowqual."""
+    failed = [f for f, on in (("sor", strand_filter == "sor"), ("lowqual", lowqual)) if on]
+    return ";".join(failed) if failed else "PASS"
+
+
+def _quality_at(run, slots):
+    """(qsum int64 [4, n], emass list of n ints) of the run's quality table at host slots."""
+    import torch
+
+    qsum, emass = run.quality_table()
+    slots = np.asarray(slots, dtype=np.int64)
+    if slots.size == 0:
+        return np.zeros((4, 0), dtype=np.int64), []
+    idx = torch.from_numpy(slots).to(qsum.device)
+    q = qsum.index_select(1, idx).cpu().numpy().view(np.uint32).astype(np.int64)
+    return q, [int(x) for x in emass.index_select(0, idx).cpu().numpy().view(np.uint64).tolist()]
 
 
 def strand_odds_ratio(f_ref, r_ref, f_alt, r_alt) -> float:
@@ -1134,7 +1230,8 @@ def _rows_at(table, slots):
     return table[0:6].index_select(1, idx).cpu().numpy().astype(np.int64)
 
 
-def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None, strand=False, max_sor=None):
+def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None, strand=False, max_sor=None,
+                qual=False, min_qual=None):
     from . import __version__
 
     mbq, mapq, flags = filters if filters is not None else (0, 0, 0)
@@ -1148,6 +1245,8 @@ def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None,
         lines.append("##kindelMateOverlaps=R2 masked where R1 covers")
     if strand:
         lines.append("##kindelStrand=max_sor={}".format("." if max_sor is None else max_sor))
+    if qual:
+        lines.append("##kindelQual=model=poisson;min_qual={}".format("." if min_qual is None else min_qual))
     if reference_name is not None:
         lines.append("##reference={}".format(reference_name))
     lines += ["##contig=<ID={},length={}>".format(name, int(L))
@@ -1170,12 +1269,19 @@ def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None,
         if max_sor is not None:
             lines.append('##FILTER=<ID=sor,Description="The strand odds ratio of an ALT allele is above {}">'
                          .format(max_sor))
+    if qual:
+        lines += ['##INFO=<ID=BQ,Number=R,Type=Float,Description="Mean base quality of the counted bases of REF and of '
+                  'each ALT allele">',
+                  '##INFO=<ID=AQ,Number=A,Type=Integer,Description="Phred-scaled probability that sequencing errors '
+                  'alone give the ALT base its count (Poisson model)">']
+        if min_qual is not None:
+            lines.append('##FILTER=<ID=lowqual,Description="QUAL is below {}">'.format(min_qual))
     lines.append("#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO")
     return lines
 
 
 def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None, reference=None, strand=False,
-                          max_sor=None) -> str:
+                          max_sor=None, qual=False, min_qual=None) -> str:
     """Host half of variants_vcf (see there): the VCF text of a finished pileup.  filters: (min_base_quality,
     min_mapq, exclude_flags) as the pileup applied them, for the header.  reference, strand, max_sor: see variants_vcf;
     with a reference the records are _reference_records'.  Strand needs a run whose batch has `reverse`
@@ -1186,12 +1292,16 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
     the total's minus those, so ADF + ADR == AD.  With one, an SNV's the same (REF 0 where the reference has no A, C,
     G or T); an indel's ALT entry is its reads on that strand (the reverse sub-batch's deletion events, the insertion
     events of reverse reads) and its REF entry max(DP_s - AO_s, 0), DP_s the record's DP taken from strand s's table,
-    so ADF[1] + ADR[1] == AO."""
+    so ADF[1] + ADR[1] == AO.  qual / min_qual: see variants_vcf; needs a run whose batch has `qual8`."""
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
+    min_qual = check_min_qual(min_qual)
+    qual = bool(qual) or min_qual is not None
     if strand and run.batch.reverse is None:
         raise ValueError("strand needs the reads' strands: decode the batch with strand=True")
-    sargs = dict(strand=strand, max_sor=max_sor)
+    if qual and run.batch.qual8 is None:
+        raise ValueError("qual needs the reads' qualities: decode the batch with qual=True")
+    sargs = dict(strand=strand, max_sor=max_sor, qual=qual, min_qual=min_qual)
     if reference is not None:
         from .reference import Reference, load_reference
 
@@ -1201,6 +1311,7 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
     lines = _vcf_header(run, abs_threshold, rel_threshold, filters, **sargs)
     site_slot, site_counts, site_mask = variant_sites(run, abs_threshold, rel_threshold)
     rev = _rows_at(run.reverse_table()[0], site_slot) if strand else None
+    qs, em = _quality_at(run, site_slot) if qual else (None, None)
     batch = run.batch
     contig_slot = np.asarray(batch.contig_slot, dtype=np.int64)
     t = site_counts.astype(np.int64)
@@ -1218,13 +1329,18 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
         ks = [tp] + [k for k, _ in alts]
         info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(str(int(t[k, i])) for k in ks),
                                           ",".join(repr(float(rounded[k, i])) for k, _ in alts))
-        filt = "PASS"
+        filt, score = "PASS", "."
         if strand:
             adr = [int(rev[k, i]) for k in ks]
             filt, tail = _strand_fields([int(t[k, i]) - x for k, x in zip(ks, adr)], adr, max_sor)
             info += tail
+        if qual:
+            score, low, tail = _qual_fields(tp if tp < 4 and depth[i] > 0 else None, [k for k, _ in alts], t[:, i],
+                                            qs[:, i], em[i], min_qual)
+            filt = _filter(filt, low)
+            info += tail
         lines.append("\t".join((batch.contig_names[c], str(int(site_slot[i] - contig_slot[c]) + 1), ".", ref,
-                                ",".join(letter for _, letter in alts), ".", filt, info)))
+                                ",".join(letter for _, letter in alts), score, filt, info)))
     return "\n".join(lines) + "\n"
 
 
@@ -1236,7 +1352,8 @@ def _af(count, depth) -> str:
     return repr(float(np.round(np.float64(count / depth if depth > 0 else 0.0), 4)))
 
 
-def _reference_records(run, ref_codes, abs_threshold, rel_threshold, strand=False, max_sor=None):
+def _reference_records(run, ref_codes, abs_threshold, rel_threshold, strand=False, max_sor=None, qual=False,
+                       min_qual=None):
     """The VCF data lines against reference codes ref_codes (uint8 per slot, reference.py): SNVs from K6r's sites,
     deletions from K7's grouped events, insertions from K6r's candidate slots and their strings (InsertionTable).
 
@@ -1248,7 +1365,7 @@ def _reference_records(run, ref_codes, abs_threshold, rel_threshold, strand=Fals
     p = 0 POS 1, REF ref[0], ALT s + ref[0].  Indels carry INFO INDEL;DP;AO (= c);AF.  An allele passes when its count
     exceeds abs_threshold and its share exceeds rel_threshold.  Order: contigs as in the batch, then POS, then SNV <
     deletion < insertion, then deletion length, then insertion slot and first-seen order.  strand / max_sor: the
-    strand fields of variants_vcf_from_run."""
+    strand fields of variants_vcf_from_run.  qual / min_qual: the quality fields of the SNV records (variants_vcf)."""
     batch = run.batch
     # host tables (the multi-GPU result): the reduced table and the batch go to this process's GPU
     counts, dbatch = run.device_tables()
@@ -1268,6 +1385,9 @@ def _reference_records(run, ref_codes, abs_threshold, rel_threshold, strand=Fals
         rev_site = _rows_at(rev_table, slot)
         # the reverse depth each insertion is measured against: DPa's slot
         rev_dpa = _rows_at(rev_table, np.where(slot - contig_slot[contig] >= 1, slot - 1, slot)).sum(axis=0)
+    snv = np.flatnonzero(mask & 15)
+    qs, em = _quality_at(run, slot[snv]) if qual else (None, None)
+    q_of = {int(i): j for j, i in enumerate(snv.tolist())}
     for i in range(slot.shape[0]):
         c, s, m = int(contig[i]), int(slot[i]), int(mask[i])
         s0, L, name = int(contig_slot[c]), int(contig_len[c]), batch.contig_names[c]
@@ -1278,13 +1398,18 @@ def _reference_records(run, ref_codes, abs_threshold, rel_threshold, strand=Fals
             ad = [int(t[g, i]) if g < 4 else 0] + [int(t[k, i]) for k in alts]
             info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(map(str, ad)),
                                               ",".join(_af(int(t[k, i]), int(depth[i])) for k in alts))
-            filt = "PASS"
+            filt, score = "PASS", "."
             if strand:
                 adr = [int(rev_site[g, i]) if g < 4 else 0] + [int(rev_site[k, i]) for k in alts]
                 filt, tail = _strand_fields([a - b for a, b in zip(ad, adr)], adr, max_sor)
                 info += tail
+            if qual:
+                j = q_of[i]
+                score, low, tail = _qual_fields(g if g < 4 else None, alts, t[:, i], qs[:, j], em[j], min_qual)
+                filt = _filter(filt, low)
+                info += tail
             recs.append((c, p + 1, 0, 0, 0, 0, "\t".join((name, str(p + 1), ".", letters[s],
-                                                            ",".join("ACGT"[k] for k in alts), ".", filt, info))))
+                                                            ",".join("ACGT"[k] for k in alts), score, filt, info))))
         if m & 64 and L > 0:
             da = int(dpa[i])
             strings = ins_table.dict_at(s)

@@ -288,11 +288,12 @@ def to_records(batch: bamio.ReadBatch):
 
 
 def write_simple_bam(path, batch: bamio.ReadBatch, level: int = 1, threads: int = 8, names=None, flag=None,
-                     next_pos=None):
+                     next_pos=None, qual=None):
     """Vectorised BAM writer for an all-simple, uniform-read-length batch (the config 2/4/5 shapes):
     lets tests and tools push 10^5..10^7 synthetic reads through the real decode path quickly.  names (uint8 [n, k]
     fixed-width QNAMEs), flag (per read) and next_pos (PNEXT - 1 per read, RNEXT then the read's own contig): paired
-    reads (write_paired_bam); by default every read is "r", FLAG 0 or 16 by strand, RNEXT / PNEXT -1."""
+    reads (write_paired_bam); by default every read is "r", FLAG 0 or 16 by strand, RNEXT / PNEXT -1.  qual: the
+    reads' Phred qualities concatenated in read order (qualities()); by default none (0xff)."""
     import struct
     from concurrent.futures import ThreadPoolExecutor
 
@@ -334,7 +335,10 @@ def write_simple_bam(path, batch: bamio.ReadBatch, level: int = 1, threads: int 
     put(36 + len(name), np.full(n, L << 4), "<u4")
     seq_be = batch.seq4.reshape(n, words).astype(">u4").view(np.uint8).reshape(n, words * 4)[:, :n_seq]
     rec[:, 40 + len(name):40 + len(name) + n_seq] = seq_be
-    rec[:, 40 + len(name) + n_seq:] = 0xFF
+    if qual is None:
+        rec[:, 40 + len(name) + n_seq:] = 0xFF
+    else:
+        rec[:, 40 + len(name) + n_seq:] = np.asarray(qual, dtype=np.uint8).reshape(n, L)
     header_text = ("@HD\tVN:1.6\tSO:coordinate\n" + "".join(
         "@SQ\tSN:%s\tLN:%d\n" % (nm, ln) for nm, ln in zip(batch.contig_names, batch.contig_len))).encode()
     head = bytearray(b"BAM\x01" + struct.pack("<i", len(header_text)) + header_text + struct.pack("<i", batch.n_contigs))

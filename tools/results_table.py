@@ -58,6 +58,9 @@ def row(path: str, d: dict) -> str:
         work += ", + mate-overlap masking (K10p, K10, K10u)"
     if d.get("cohort_ms"):
         work += ", multi-sample VCF (%d samples, K6m)" % cfg.get("samples", 0)
+    if d.get("floor"):
+        work += ", K11 quality sums alone: %.3f ms, %.2f of its HBM floor" % (km.get("k0_k11_k11g_median", 0),
+                                                                           d["floor"].get("share_of_floor", 0))
     if d.get("map_ab"):
         work += ", zeroing A/B (dirty-sector map)"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
