@@ -464,6 +464,25 @@ int kdl_overlap_untake(const int32_t* drops, int64_t n_drops, int32_t* counts, i
 int kdl_quality_pileup(const kdl_batch* batch, const uint8_t* qual8, uint32_t* qsum, uint64_t* emass, int64_t n_slots,
                        void* stream);
 
+/* K11w (extension: `consensus --quality-vote`): the counted bases of kdl_quality_pileup, each weighted by its quality.
+ *   wsum[4][n_slots]  uint64, 16-byte aligned: for k = A, C, G, T the summed W[min(q, 93)] of the slot's counted bases
+ *                     of allele k, W[q] the integer nearest to 2^16 * 10 log10(3 (1 - e_q) / e_q) with
+ *                     e_q = min(10^(-q / 10), 3/4): the log-likelihood ratio, in 1/65536 Phred, of "the true base is the
+ *                     one read" against "it is one particular other base" (W[0] = W[1] = 0, W[20] = 1620546,
+ *                     W[93] = 6407534; kindel_b200/quality.py holds the table)
+ * The same branches as kdl_quality_pileup (K0 + K11w + K11g-w, or a zeroing pass + K11g-w); the table is written whole
+ * and, as integer sums, does not depend on order.  With constant qualities q, wsum[k][s] == W[q] * counts[k][s].
+ * n_slots % 4 == 0.  Device pointers. */
+int kdl_quality_weights(const kdl_batch* batch, const uint8_t* qual8, uint64_t* wsum, int64_t n_slots, void* stream);
+
+/* K2w (extension: `consensus --quality-vote`): the vote of kdl_vote with the base chosen by base-quality weights.  The
+ * D, N and I decisions, their order and so the change bits of every call byte are kdl_vote's; where a base is emitted it
+ * is b* = the base with the largest wsum[b][s] (kdl_quality_weights), and N (code 4) when that sum is 0 or two bases
+ * share it.  The N column does not vote.  Bit 7 is never set.  qual (may be NULL): qual[s] = min(60, (wsum[b*][s] -
+ * max over b != b* of wsum[b][s]) >> 16), and 0 for every call that emits N or nothing.  n_slots % 4 == 0. */
+int kdl_vote_quality(const int32_t* counts, const uint64_t* wsum, int64_t n_slots, int64_t min_depth_ceil,
+                     uint8_t* calls, uint8_t* qual, void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced

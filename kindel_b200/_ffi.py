@@ -166,6 +166,8 @@ _PROTOTYPES = {
                                     C.POINTER(KdlQmask), C.c_void_p, C.c_int64, C.c_void_p]),
     "kdl_overlap_untake": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "kdl_quality_pileup": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "kdl_quality_weights": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "kdl_vote_quality": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers":(C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,

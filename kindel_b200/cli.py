@@ -22,13 +22,14 @@ from . import __version__
 
 
 def consensus(bam_path, realign=False, min_depth=1, min_overlap=7, clip_decay_threshold=0.1, mask_ends=50,
-              trim_ends=False, uppercase=False, gpus=None, iupac_threshold=None, fastq=False, **filters):
+              trim_ends=False, uppercase=False, gpus=None, iupac_threshold=None, fastq=False, quality_vote=False,
+              **filters):
     """Infer consensus sequence(s) from alignment in SAM/BAM format"""
     from . import kindel
 
     res = kindel.bam_to_consensus(bam_path, realign, min_depth, min_overlap, clip_decay_threshold, mask_ends,
                                   trim_ends, uppercase, devices=gpus, iupac_threshold=iupac_threshold,
-                                  qualities=fastq, **filters)
+                                  qualities=fastq, quality_vote=quality_vote, **filters)
     print("\n".join(res.refs_reports.values()), file=sys.stderr)
     for record in res.consensuses:
         if fastq:  # extension: @name, sequence, +, Phred+33 qualities
@@ -163,9 +164,13 @@ def build_parser() -> argparse.ArgumentParser:
     # extension (not in the reference's CLI): per-base qualities, off by default
     p.add_argument("--fastq", action="store_true",
                    help="write FASTQ with a Phred quality per consensus base instead of FASTA")
+    # extension (not in the reference's CLI): the base by the reads' base qualities, off by default
+    p.add_argument("--quality-vote", action="store_true",
+                   help="emit the base whose reads' base qualities give it the largest summed log-likelihood weight "
+                        "instead of the majority base (not with --iupac-threshold)")
     p.set_defaults(func=lambda a: consensus(a.bam_path, a.realign, a.min_depth, a.min_overlap,
                                             a.clip_decay_threshold, a.mask_ends, a.trim_ends, a.uppercase, a.gpus,
-                                            a.iupac_threshold, a.fastq, **_filters(a)))
+                                            a.iupac_threshold, a.fastq, a.quality_vote, **_filters(a)))
 
     p = sub.add_parser("weights", help=weights.__doc__, description=weights.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")
@@ -226,6 +231,11 @@ def build_parser() -> argparse.ArgumentParser:
     return parser
 
 
+def _check_consensus_args(parser, args):
+    if getattr(args, "command", None) == "consensus" and args.quality_vote and args.iupac_threshold is not None:
+        parser.error("consensus: --quality-vote cannot be combined with --iupac-threshold")
+
+
 def _check_variants_args(parser, args):
     # --absolute and --only-variants shape the table; the VCF always holds the variant sites alone
     paths = getattr(args, "bam_path", None)
@@ -251,6 +261,7 @@ def _check_variants_args(parser, args):
 def main(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
+    _check_consensus_args(parser, args)
     _check_variants_args(parser, args)
     if not getattr(args, "func", None):
         parser.print_usage()

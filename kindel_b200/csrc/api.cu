@@ -780,16 +780,10 @@ int kdl_overlap_untake(const int32_t* drops, int64_t n_drops, int32_t* counts, i
     return check_launch();
 }
 
-int kdl_quality_pileup(const kdl_batch* batch, const uint8_t* qual8, uint32_t* qsum, uint64_t* emass, int64_t n_slots,
-                       void* stream) {
-    int rc = validate_batch(batch);
-    if (rc != KDL_OK) return rc;
-    if (!qsum || !emass || n_slots <= 0 || (n_slots & 3) || (batch->n_reads > 0 && !qual8) ||
-        (reinterpret_cast<uintptr_t>(qual8) & 7) || (reinterpret_cast<uintptr_t>(qsum) & 15) ||
-        (reinterpret_cast<uintptr_t>(emass) & 15))
-        return KDL_ERR_INVALID_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned long long* em = reinterpret_cast<unsigned long long*>(emass);
+// K0 + K11 + K11g of one sum policy (kdl::PhredSums or kdl::WeightSums, quality.cu), arguments checked
+extern "C++" template <class Sums>
+int quality_launch(const kdl_batch* batch, const uint8_t* qual8, Sums sums, int64_t n_slots, cudaStream_t st) {
+    int rc;
     const int cap = sm_count() * 8;
     // the tile-owner path under the conditions of kdl_pileup_range's
     const bool tiled = batch->n_reads > batch->n_hard && (n_slots % KDL_TILE) == 0 && batch->reads_sorted &&
@@ -800,19 +794,54 @@ int kdl_quality_pileup(const kdl_batch* batch, const uint8_t* qual8, uint32_t* q
         KDL_LAUNCH(kdl::tile_index_kernel, (unsigned)((n_tiles * 32 + 255) / 256), 256, 0, st, *batch, 0ll, n_tiles,
                    batch->tile_index);  // K0, into the caller's scratch: no ordering dependency on kdl_pileup
         if ((rc = check_launch()) != KDL_OK) return rc;
-        KDL_LAUNCH(kdl::quality_tile_kernel, (unsigned)n_tiles, kdl::kQtThreads, 0, st, *batch, qual8, qsum, em, n_slots,
-                   batch->tile_index);
+        KDL_LAUNCH(kdl::quality_tile_kernel<Sums>, (unsigned)n_tiles, kdl::kQtThreads, 0, st, *batch, qual8, sums,
+                   n_slots, batch->tile_index);
         if ((rc = check_launch()) != KDL_OK) return rc;
         if (batch->n_hard == 0) return KDL_OK;
-        KDL_LAUNCH(kdl::quality_general_kernel, grid_for(batch->n_hard, 8, cap), 256, 0, st, *batch, qual8,
-                   batch->hard_idx, batch->n_hard, qsum, em, n_slots);
+        KDL_LAUNCH(kdl::quality_general_kernel<Sums>, grid_for(batch->n_hard, 8, cap), 256, 0, st, *batch, qual8,
+                   batch->hard_idx, batch->n_hard, sums, n_slots);
         return check_launch();
     }
-    KDL_LAUNCH(kdl::quality_zero_kernel, sm_count() * 4, 256, 0, st, qsum, em, n_slots);
+    KDL_LAUNCH(kdl::quality_zero_kernel<Sums>, sm_count() * 4, 256, 0, st, sums, n_slots);
     if ((rc = check_launch()) != KDL_OK) return rc;
     if (batch->n_reads == 0) return KDL_OK;
-    KDL_LAUNCH(kdl::quality_general_kernel, grid_for(batch->n_reads, 8, cap), 256, 0, st, *batch, qual8, nullptr,
-               batch->n_reads, qsum, em, n_slots);
+    KDL_LAUNCH(kdl::quality_general_kernel<Sums>, grid_for(batch->n_reads, 8, cap), 256, 0, st, *batch, qual8, nullptr,
+               batch->n_reads, sums, n_slots);
+    return check_launch();
+}
+
+int kdl_quality_pileup(const kdl_batch* batch, const uint8_t* qual8, uint32_t* qsum, uint64_t* emass, int64_t n_slots,
+                       void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (!qsum || !emass || n_slots <= 0 || (n_slots & 3) || (batch->n_reads > 0 && !qual8) ||
+        (reinterpret_cast<uintptr_t>(qual8) & 7) || (reinterpret_cast<uintptr_t>(qsum) & 15) ||
+        (reinterpret_cast<uintptr_t>(emass) & 15))
+        return KDL_ERR_INVALID_ARG;
+    unsigned long long* em = reinterpret_cast<unsigned long long*>(emass);
+    return quality_launch(batch, qual8, kdl::PhredSums{qsum, em}, n_slots, (cudaStream_t)stream);
+}
+
+int kdl_quality_weights(const kdl_batch* batch, const uint8_t* qual8, uint64_t* wsum, int64_t n_slots, void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (!wsum || n_slots <= 0 || (n_slots & 3) || (batch->n_reads > 0 && !qual8) ||
+        (reinterpret_cast<uintptr_t>(qual8) & 7) || (reinterpret_cast<uintptr_t>(wsum) & 15))
+        return KDL_ERR_INVALID_ARG;
+    return quality_launch(batch, qual8, kdl::WeightSums{reinterpret_cast<unsigned long long*>(wsum)}, n_slots,
+                          (cudaStream_t)stream);
+}
+
+int kdl_vote_quality(const int32_t* counts, const uint64_t* wsum, int64_t n_slots, int64_t min_depth_ceil,
+                     uint8_t* calls, uint8_t* qual, void* stream) {
+    if (!counts || !wsum || !calls || n_slots <= 0 || (n_slots & 3)) return KDL_ERR_INVALID_ARG;
+    kdl::Peers none;
+    none.n = 0;
+    const long long quads = n_slots / 4;
+    const long long grid = (quads + 255) / 256;
+    KDL_LAUNCH((kdl::vote_kernel<false, kdl::QualityVote>), (unsigned)grid, 256, 0, (cudaStream_t)stream,
+               counts, none, n_slots, 0, n_slots, min_depth_ceil, calls, nullptr,
+               kdl::QualityVote{reinterpret_cast<const unsigned long long*>(wsum), n_slots, qual});
     return check_launch();
 }
 

@@ -113,20 +113,29 @@ __device__ __forceinline__ int base_vote(int a, int c, int g, int t, int n, int*
     return (best != 0 && ties > 1) ? 4 : code;
 }
 
-// One slot of consensus_sequence (kindel/kindel.py:402-424) in integer arithmetic:
+// The D / N / I decisions of one slot of consensus_sequence (kindel/kindel.py:402-424) in integer arithmetic:
 //   del > 0.5*depth            <=> 2*del > depth
 //   depth < min_depth          <=> depth < ceil(min_depth)
 //   ins > min(0.5*d, 0.5*dn)   <=> 2*ins > min(d, dn)
+// Every vote makes them in this order.  Returns true with the whole call byte in *call for a 'D' or an 'N' slot; false
+// with the change code (0 or 3 for 'I') in bits 4-5 of *call and the base left to the vote.
+__device__ __forceinline__ bool vote_decided(int a, int c, int g, int t, int del, int ins, long long depth_next,
+                                             long long min_depth_ceil, unsigned* call) {
+    const long long depth = (long long)a + c + g + t;  // N excluded (kindel.py:404)
+    if (2ll * del > depth) { *call = (1u << 4) | 4u; return true; }
+    if (depth < min_depth_ceil) { *call = (2u << 4) | 4u; return true; }
+    const long long thr = depth < depth_next ? depth : depth_next;
+    *call = (2ll * ins > thr) ? (3u << 4) : 0u;
+    return false;
+}
+
+// One slot of consensus_sequence with consensus()'s base
 __device__ __forceinline__ unsigned vote_slot(int a, int c, int g, int t, int n, int del, int ins,
                                               long long depth_next, long long min_depth_ceil) {
-    const long long depth = (long long)a + c + g + t;  // N excluded (kindel.py:404)
-    if (2ll * del > depth) return (1u << 4) | 4u;
-    if (depth < min_depth_ceil) return (2u << 4) | 4u;
-    const long long thr = depth < depth_next ? depth : depth_next;
-    const unsigned change = (2ll * ins > thr) ? 3u : 0u;
+    unsigned call;
+    if (vote_decided(a, c, g, t, del, ins, depth_next, min_depth_ceil, &call)) return call;
     int freq, raw;
-    const int code = base_vote(a, c, g, t, n, &freq, &raw);
-    return (change << 4) | (unsigned)code;
+    return call | (unsigned)base_vote(a, c, g, t, n, &freq, &raw);
 }
 
 // descending compare-exchange: x keeps the larger value
@@ -164,26 +173,56 @@ __device__ __forceinline__ unsigned iupac_base(int a, int c, int g, int t, doubl
 // vote_slot with the IUPAC base: the D / N / I decisions and their order are vote_slot's; only the base differs
 __device__ __forceinline__ unsigned vote_slot_iupac(int a, int c, int g, int t, int del, int ins, long long depth_next,
                                                     long long min_depth_ceil, double threshold) {
-    const long long depth = (long long)a + c + g + t;
-    if (2ll * del > depth) return (1u << 4) | 4u;
-    if (depth < min_depth_ceil) return (2u << 4) | 4u;
-    const long long thr = depth < depth_next ? depth : depth_next;
-    const unsigned change = (2ll * ins > thr) ? 3u : 0u;
-    return (change << 4) | iupac_base(a, c, g, t, threshold);
+    unsigned call;
+    if (vote_decided(a, c, g, t, del, ins, depth_next, min_depth_ceil, &call)) return call;
+    return call | iupac_base(a, c, g, t, threshold);
 }
 
-// Vote policies of K2 / K2x (template arguments of vote_kernel and vote_exchange_kernel)
+// The emitted base of the quality vote (extension: `quality_vote`): b* = the base with the largest summed weight
+// (wsum, WeightSums in quality.cu); N when that sum is 0 or two bases share it.  *q = min(60, (wsum[b*] - the
+// runner-up's) >> 16), the Phred-scaled likelihood ratio of the call over the runner-up; 0 for N.  Integer only.
+__device__ __forceinline__ unsigned weight_base(unsigned long long wa, unsigned long long wc, unsigned long long wg,
+                                                unsigned long long wt, unsigned* q) {
+    unsigned long long best = wa, second = 0ull;
+    unsigned code = 0u;
+    const unsigned long long w[3] = {wc, wg, wt};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        if (w[k] > best) { second = best; best = w[k]; code = (unsigned)k + 1u; }
+        else if (w[k] > second) second = w[k];
+    }
+    if (best == 0ull || best == second) { *q = 0u; return 4u; }
+    const unsigned long long d = (best - second) >> 16;
+    *q = d < 60ull ? (unsigned)d : 60u;
+    return code;
+}
+
+// Vote policies of K2 / K2x (template arguments of vote_kernel and vote_exchange_kernel); `s` is the slot
 struct MajorityVote {  // the reference's vote
-    __device__ __forceinline__ unsigned operator()(int a, int c, int g, int t, int n, int del, int ins,
+    __device__ __forceinline__ unsigned operator()(long long, int a, int c, int g, int t, int n, int del, int ins,
                                                    long long depth_next, long long min_depth_ceil) const {
         return vote_slot(a, c, g, t, n, del, ins, depth_next, min_depth_ceil);
     }
 };
 struct IupacVote {  // ambiguity codes below a frequency threshold
     double threshold;
-    __device__ __forceinline__ unsigned operator()(int a, int c, int g, int t, int, int del, int ins,
+    __device__ __forceinline__ unsigned operator()(long long, int a, int c, int g, int t, int, int del, int ins,
                                                    long long depth_next, long long min_depth_ceil) const {
         return vote_slot_iupac(a, c, g, t, del, ins, depth_next, min_depth_ceil, threshold);
+    }
+};
+struct QualityVote {  // the base by summed base-quality weights; qual (may be NULL): the Q of each slot, 0 unless a base
+    const unsigned long long* __restrict__ wsum;  // [4][n_slots]
+    long long n_slots;
+    uint8_t* __restrict__ qual;
+    __device__ __forceinline__ unsigned operator()(long long s, int a, int c, int g, int t, int, int del, int ins,
+                                                   long long depth_next, long long min_depth_ceil) const {
+        unsigned call, q = 0u;
+        if (!vote_decided(a, c, g, t, del, ins, depth_next, min_depth_ceil, &call))
+            call |= weight_base(__ldg(wsum + s), __ldg(wsum + n_slots + s), __ldg(wsum + 2 * n_slots + s),
+                                __ldg(wsum + 3 * n_slots + s), &q);
+        if (qual) qual[s] = (uint8_t)q;
+        return call;
     }
 };
 

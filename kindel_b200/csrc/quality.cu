@@ -22,6 +22,10 @@
 // wrap and right-clip stall included), or every read of a batch K11 cannot take (unsorted, or no tile_index) after a
 // zeroing pass -- one warp per read, global atomics (a native 64-bit RED for emass; in shared memory the 64-bit add is a
 // CAS loop, which only K11's complex reads take).
+//
+// K11w / K11g-w (extension: `consensus --quality-vote`) are the same kernels with the WeightSums policy: per slot
+//   wsum[k * n_slots + s]  uint64  the summed W[min(q, 93)] of the counted bases of allele k (the table below)
+// A lane sums a chunk in uint32 registers, and the four quarters fold them into uint64 at the chunk's end.
 #include "tile_common.cuh"
 
 namespace kdl {
@@ -50,21 +54,170 @@ __constant__ unsigned long long kQualEps[kEpsMax + 1] = {
     4ull, 3ull, 3ull, 2ull,
 };
 
-__device__ __forceinline__ void load_eps(unsigned long long* eps) {
-    for (int i = threadIdx.x; i <= kEpsMax; i += blockDim.x) eps[i] = kQualEps[i];
-}
+// W[q] = the integer nearest to 2^16 * 10 log10(3 (1 - e) / e), e = min(10^(-q / 10), 3/4), q = 0..93: the log-likelihood
+// ratio, in 1/65536 Phred, of "the true base is the one read" against "it is one particular other base", the error
+// spread evenly over the other three (tests/test_quality_vote.py pins it against an exact computation)
+__constant__ uint32_t kQualWeight[kEpsMax + 1] = {
+    0u, 0u, 160037u, 311335u, 430336u, 532174u, 623571u, 708096u,
+    787861u, 864214u, 938059u, 1010026u, 1080568u, 1150020u, 1218628u, 1286580u,
+    1354022u, 1421062u, 1487787u, 1554264u, 1620546u, 1686672u, 1752677u, 1818584u,
+    1884415u, 1950185u, 2015906u, 2081590u, 2147243u, 2212872u, 2278481u, 2344076u,
+    2409659u, 2475232u, 2540797u, 2606356u, 2671911u, 2737461u, 2803009u, 2868554u,
+    2934098u, 2999640u, 3065180u, 3130720u, 3196259u, 3261797u, 3327335u, 3392873u,
+    3458410u, 3523947u, 3589483u, 3655020u, 3720556u, 3786093u, 3851629u, 3917165u,
+    3982701u, 4048238u, 4113774u, 4179310u, 4244846u, 4310382u, 4375918u, 4441454u,
+    4506990u, 4572526u, 4638062u, 4703598u, 4769134u, 4834670u, 4900206u, 4965742u,
+    5031278u, 5096814u, 5162350u, 5227886u, 5293422u, 5358958u, 5424494u, 5490030u,
+    5555566u, 5621102u, 5686638u, 5752174u, 5817710u, 5883246u, 5948782u, 6014318u,
+    6079854u, 6145390u, 6210926u, 6276462u, 6341998u, 6407534u,
+};
 
 // column 0..3 of a one-hot nibble (A=1 C=2 G=4 T=8), -1 for anything else (N, padding, exotic bases)
 __device__ __forceinline__ int acgt_col(uint32_t nib) {
     return (nib == 1u) ? 0 : (nib == 2u) ? 1 : (nib == 4u) ? 2 : (nib == 8u) ? 3 : -1;
 }
 
-__global__ void __launch_bounds__(kQtThreads)
-quality_tile_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, uint32_t* __restrict__ qsum,
-                    unsigned long long* __restrict__ emass, long long n_slots, const uint32_t* __restrict__ index) {
-    __shared__ uint32_t s_q[4][KDL_TILE];            // the complex reads' sums
-    __shared__ unsigned long long s_e[KDL_TILE];
-    __shared__ unsigned long long s_eps[kEpsMax + 1];
+__device__ __forceinline__ uint32_t clamp_q(uint32_t q) { return q < kEpsMax ? q : kEpsMax; }
+
+template <class Sums>
+__device__ __forceinline__ void load_table(typename Sums::Entry* tab) {
+    for (int i = threadIdx.x; i <= kEpsMax; i += blockDim.x) tab[i] = Sums::entry(i);
+}
+
+// Sum policies of K11 / K11g (template arguments): what a counted base of quality q adds to its slot and where the sums
+// live.  In K11 a lane keeps the sums of its 8 slots in registers (Regs), the tile's complex reads add into shared
+// memory (Smem), and store() writes the tile; K11g adds to the tables with global atomics.
+struct PhredSums {  // `variants --vcf --qual`: qsum[4][n_slots] uint32 and emass[n_slots] uint64
+    uint32_t* qsum;
+    unsigned long long* emass;
+    using Entry = unsigned long long;
+    static constexpr int kMinBlocks = 0;  // (0: no minimum, the launch bounds K11 always had)
+    __device__ static Entry entry(int q) { return kQualEps[q]; }
+    struct Smem {
+        uint32_t q[4][KDL_TILE];
+        unsigned long long e[KDL_TILE];
+    };
+    struct Regs {
+        uint32_t s[4][8];
+        unsigned long long e[8];
+    };
+    __device__ static void zero(Smem& sm, int i) {
+        sm.q[0][i] = 0u; sm.q[1][i] = 0u; sm.q[2][i] = 0u; sm.q[3][i] = 0u;
+        sm.e[i] = 0ull;
+    }
+    __device__ static void zero(Regs& r) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { r.s[0][j] = r.s[1][j] = r.s[2][j] = r.s[3][j] = 0u; r.e[j] = 0ull; }
+    }
+    __device__ static void add(Regs& r, int j, uint32_t nib, uint32_t q, const Entry* tab) {
+        r.s[0][j] += nib == 1u ? q : 0u;
+        r.s[1][j] += nib == 2u ? q : 0u;
+        r.s[2][j] += nib == 4u ? q : 0u;
+        r.s[3][j] += nib == 8u ? q : 0u;
+        r.e[j] += (nib && !(nib & (nib - 1u))) ? tab[clamp_q(q)] : 0ull;
+    }
+    __device__ static void end_chunk(Regs&, int) {}
+    __device__ static void add(Smem& sm, int col, int slot, uint32_t q, const Entry* tab) {
+        atomicAdd(&sm.q[col][slot], q);
+        atomicAdd(&sm.e[slot], tab[clamp_q(q)]);
+    }
+    __device__ void add(long long slot, long long n_slots, int col, uint32_t q, const Entry* tab) const {
+        atomicAdd(qsum + (long long)col * n_slots + slot, q);
+        atomicAdd(emass + slot, tab[clamp_q(q)]);
+    }
+    // the four quarters hold partial sums of the same 8 slots: add them, then quarter q writes column q, quarter 0 emass
+    __device__ void store(Regs& r, const Smem& sm, int quarter, int a0, long long t0, long long n_slots) const {
+        uint32_t out[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            uint32_t x = r.s[0][j], y = r.s[1][j], z = r.s[2][j], w = r.s[3][j];
+            unsigned long long m = r.e[j];
+            x += __shfl_xor_sync(0xffffffffu, x, 8);  x += __shfl_xor_sync(0xffffffffu, x, 16);
+            y += __shfl_xor_sync(0xffffffffu, y, 8);  y += __shfl_xor_sync(0xffffffffu, y, 16);
+            z += __shfl_xor_sync(0xffffffffu, z, 8);  z += __shfl_xor_sync(0xffffffffu, z, 16);
+            w += __shfl_xor_sync(0xffffffffu, w, 8);  w += __shfl_xor_sync(0xffffffffu, w, 16);
+            m += __shfl_xor_sync(0xffffffffu, m, 8);  m += __shfl_xor_sync(0xffffffffu, m, 16);
+            out[j] = (quarter == 0 ? x : quarter == 1 ? y : quarter == 2 ? z : w) + sm.q[quarter][a0 + j];
+            r.e[j] = m + sm.e[a0 + j];
+        }
+        uint4* dq = reinterpret_cast<uint4*>(qsum + (long long)quarter * n_slots + t0 + a0);
+        dq[0] = make_uint4(out[0], out[1], out[2], out[3]);
+        dq[1] = make_uint4(out[4], out[5], out[6], out[7]);
+        if (quarter == 0) {
+            ulonglong2* de = reinterpret_cast<ulonglong2*>(emass + t0 + a0);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) de[j] = make_ulonglong2(r.e[2 * j], r.e[2 * j + 1]);
+        }
+    }
+    __device__ void zero_tables(long long gtid, long long stride, long long n_slots) const {
+        for (long long s = gtid; s < 4 * n_slots; s += stride) qsum[s] = 0u;
+        for (long long s = gtid; s < n_slots; s += stride) emass[s] = 0ull;
+    }
+};
+
+struct WeightSums {  // `consensus --quality-vote`: wsum[4][n_slots] uint64, the summed W[min(q, 93)] per base
+    unsigned long long* wsum;
+    using Entry = uint32_t;
+    static constexpr int kMinBlocks = 1;  // (without it ptxas caps K11w at 64 registers and spills)
+    __device__ static Entry entry(int q) { return kQualWeight[q]; }
+    struct Smem {
+        unsigned long long w[4][KDL_TILE];
+    };
+    // s: the chunk's partial sums -- a quarter-warp adds at most kQtChunk / 4 = 256 reads to a slot per chunk, and
+    // 256 * W[93] < 2^32, so uint32 is exact; w: the folded sums of column `quarter` of the lane's 8 slots
+    struct Regs {
+        uint32_t s[4][8];
+        unsigned long long w[8];
+    };
+    __device__ static void zero(Smem& sm, int i) { sm.w[0][i] = 0ull; sm.w[1][i] = 0ull; sm.w[2][i] = 0ull; sm.w[3][i] = 0ull; }
+    __device__ static void zero(Regs& r) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { r.s[0][j] = r.s[1][j] = r.s[2][j] = r.s[3][j] = 0u; r.w[j] = 0ull; }
+    }
+    __device__ static void add(Regs& r, int j, uint32_t nib, uint32_t q, const Entry* tab) {
+        const uint32_t w = tab[clamp_q(q)];
+        r.s[0][j] += nib == 1u ? w : 0u;
+        r.s[1][j] += nib == 2u ? w : 0u;
+        r.s[2][j] += nib == 4u ? w : 0u;
+        r.s[3][j] += nib == 8u ? w : 0u;
+    }
+    // the chunk's partials of the four quarters, added in 64 bits; quarter q keeps column q (whole warp, converged)
+    __device__ static void end_chunk(Regs& r, int quarter) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                unsigned long long x = r.s[k][j];
+                x += __shfl_xor_sync(0xffffffffu, x, 8);
+                x += __shfl_xor_sync(0xffffffffu, x, 16);
+                r.w[j] += quarter == k ? x : 0ull;
+                r.s[k][j] = 0u;
+            }
+        }
+    }
+    __device__ static void add(Smem& sm, int col, int slot, uint32_t q, const Entry* tab) {
+        atomicAdd(&sm.w[col][slot], (unsigned long long)tab[clamp_q(q)]);
+    }
+    __device__ void add(long long slot, long long n_slots, int col, uint32_t q, const Entry* tab) const {
+        atomicAdd(wsum + (long long)col * n_slots + slot, (unsigned long long)tab[clamp_q(q)]);
+    }
+    __device__ void store(Regs& r, const Smem& sm, int quarter, int a0, long long t0, long long n_slots) const {
+        ulonglong2* dw = reinterpret_cast<ulonglong2*>(wsum + (long long)quarter * n_slots + t0 + a0);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            dw[j] = make_ulonglong2(r.w[2 * j] + sm.w[quarter][a0 + 2 * j], r.w[2 * j + 1] + sm.w[quarter][a0 + 2 * j + 1]);
+    }
+    __device__ void zero_tables(long long gtid, long long stride, long long n_slots) const {
+        for (long long s = gtid; s < 4 * n_slots; s += stride) wsum[s] = 0ull;
+    }
+};
+
+template <class Sums>
+__global__ void __launch_bounds__(kQtThreads, Sums::kMinBlocks)
+quality_tile_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, Sums sums, long long n_slots,
+                    const uint32_t* __restrict__ index) {
+    __shared__ typename Sums::Smem s_sum;            // the complex reads' sums
+    __shared__ typename Sums::Entry s_tab[kEpsMax + 1];
     __shared__ int s_start[kQtChunk];                // read start slot relative to the tile (clamped)
     __shared__ uint32_t s_off[kQtChunk];
     __shared__ uint32_t s_lw[kQtChunk];
@@ -75,19 +228,14 @@ quality_tile_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, uint32_t* __
     const long long t0 = (long long)blockIdx.x * KDL_TILE;
     const uint32_t* e = index + F_IDX * blockIdx.x;
     const long long lo = e[0], hi = e[1];
-    for (int i = threadIdx.x; i < KDL_TILE; i += blockDim.x) {
-        s_q[0][i] = 0u; s_q[1][i] = 0u; s_q[2][i] = 0u; s_q[3][i] = 0u;
-        s_e[i] = 0ull;
-    }
-    load_eps(s_eps);
+    for (int i = threadIdx.x; i < KDL_TILE; i += blockDim.x) Sums::zero(s_sum, i);
+    load_table<Sums>(s_tab);
     const uint64_t* __restrict__ qw = reinterpret_cast<const uint64_t*>(qual8);  // 8 qualities per seq4 word
 
     const int quarter = lane >> 3;
     const int a0 = warp * 64 + 8 * (lane & 7);  // the lane's first slot, relative to the tile
-    uint32_t sa[8], sc[8], sg[8], st[8];
-    unsigned long long em[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { sa[j] = sc[j] = sg[j] = st[j] = 0u; em[j] = 0ull; }
+    typename Sums::Regs acc;
+    Sums::zero(acc);
 
     for (long long base = lo; base < hi; base += kQtChunk) {
         const int n = (int)(hi - base < kQtChunk ? hi - base : kQtChunk);
@@ -126,13 +274,10 @@ quality_tile_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, uint32_t* __
             for (int j = 0; j < 8; ++j) {
                 const uint32_t nib = (word >> (28 - 4 * j)) & 0xFu;
                 const uint32_t q = (uint32_t)(qv >> (8 * j)) & 0xFFu;
-                sa[j] += nib == 1u ? q : 0u;
-                sc[j] += nib == 2u ? q : 0u;
-                sg[j] += nib == 4u ? q : 0u;
-                st[j] += nib == 8u ? q : 0u;
-                em[j] += (nib && !(nib & (nib - 1u))) ? s_eps[q < kEpsMax ? q : kEpsMax] : 0ull;
+                Sums::add(acc, j, nib, q, s_tab);
             }
         }
+        Sums::end_chunk(acc, quarter);
         // the complex reads: one warp per read walks its CIGAR (warp-uniform), the lanes stride over an op's bases that
         // land in this tile, shared-memory atomics
         for (int j = warp; j < s_ncx; j += kQtThreads / 32) {
@@ -151,9 +296,7 @@ quality_tile_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, uint32_t* __
                     for (int d = d0 + lane; d < d1; d += 32) {
                         const int col = acgt_col((uint32_t)nibble_at(seq, q_pos + d));
                         if (col < 0) continue;
-                        const uint32_t q = qr[q_pos + d];
-                        atomicAdd(&s_q[col][r_pos + d], q);
-                        atomicAdd(&s_e[r_pos + d], s_eps[q < kEpsMax ? q : kEpsMax]);
+                        Sums::add(s_sum, col, r_pos + d, (uint32_t)qr[q_pos + d], s_tab);
                     }
                     r_pos += len;
                     q_pos += len;
@@ -169,37 +312,17 @@ quality_tile_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, uint32_t* __
         }
     }
     __syncthreads();  // the complex reads' shared sums are complete (also when the tile has no read)
-    // the four quarters hold partial sums of the same 8 slots: add them, then quarter q writes column q, quarter 0 emass
-    uint32_t out[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        uint32_t x = sa[j], y = sc[j], z = sg[j], w = st[j];
-        unsigned long long m = em[j];
-        x += __shfl_xor_sync(0xffffffffu, x, 8);  x += __shfl_xor_sync(0xffffffffu, x, 16);
-        y += __shfl_xor_sync(0xffffffffu, y, 8);  y += __shfl_xor_sync(0xffffffffu, y, 16);
-        z += __shfl_xor_sync(0xffffffffu, z, 8);  z += __shfl_xor_sync(0xffffffffu, z, 16);
-        w += __shfl_xor_sync(0xffffffffu, w, 8);  w += __shfl_xor_sync(0xffffffffu, w, 16);
-        m += __shfl_xor_sync(0xffffffffu, m, 8);  m += __shfl_xor_sync(0xffffffffu, m, 16);
-        out[j] = (quarter == 0 ? x : quarter == 1 ? y : quarter == 2 ? z : w) + s_q[quarter][a0 + j];
-        em[j] = m + s_e[a0 + j];
-    }
-    uint4* dq = reinterpret_cast<uint4*>(qsum + (long long)quarter * n_slots + t0 + a0);
-    dq[0] = make_uint4(out[0], out[1], out[2], out[3]);
-    dq[1] = make_uint4(out[4], out[5], out[6], out[7]);
-    if (quarter == 0) {
-        ulonglong2* de = reinterpret_cast<ulonglong2*>(emass + t0 + a0);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) de[j] = make_ulonglong2(em[2 * j], em[2 * j + 1]);
-    }
+    sums.store(acc, s_sum, quarter, a0, t0, n_slots);
 }
 
 // K11g: one warp per read of `list` (NULL: every read), K1g's walk (kindel.py:40-81 with the Python index wrap and the
 // right-clip stall); a simple read is one M op.  Bases that would raise in K1g are skipped (the pileup raises then).
+template <class Sums>
 __global__ void __launch_bounds__(256)
 quality_general_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, const uint32_t* __restrict__ list, long long n_list,
-                       uint32_t* __restrict__ qsum, unsigned long long* __restrict__ emass, long long n_slots) {
-    __shared__ unsigned long long s_eps[kEpsMax + 1];
-    load_eps(s_eps);
+                       Sums sums, long long n_slots) {
+    __shared__ typename Sums::Entry s_tab[kEpsMax + 1];
+    load_table<Sums>(s_tab);
     __syncthreads();
     const int lane = threadIdx.x & 31;
     const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -226,9 +349,7 @@ quality_general_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, const uin
                     if (q >= lseq || idx < 0) continue;
                     const int col = acgt_col((uint32_t)nibble_at(seq, q));
                     if (col < 0) continue;
-                    const uint32_t qq = qr[q];
-                    atomicAdd(qsum + (long long)col * n_slots + slot0 + idx, qq);
-                    atomicAdd(emass + slot0 + idx, s_eps[qq < kEpsMax ? qq : kEpsMax]);
+                    sums.add(slot0 + idx, n_slots, col, (uint32_t)qr[q], s_tab);
                 }
                 r_pos += len;
                 q_pos += len;
@@ -250,11 +371,10 @@ quality_general_kernel(kdl_batch b, const uint8_t* __restrict__ qual8, const uin
     }
 }
 
-__global__ void __launch_bounds__(256)
-quality_zero_kernel(uint32_t* __restrict__ qsum, unsigned long long* __restrict__ emass, long long n_slots) {
+template <class Sums>
+__global__ void __launch_bounds__(256) quality_zero_kernel(Sums sums, long long n_slots) {
     const long long gtid = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
-    for (long long s = gtid; s < 4 * n_slots; s += stride) qsum[s] = 0u;
-    for (long long s = gtid; s < n_slots; s += stride) emass[s] = 0ull;
+    sums.zero_tables(gtid, stride, n_slots);
 }
 
 }  // namespace kdl

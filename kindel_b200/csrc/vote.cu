@@ -49,9 +49,9 @@ __device__ __forceinline__ int load1(const int32_t* __restrict__ counts, const P
     }
 }
 
-// n_slots % 4 == 0, slot_lo % 4 == 0.  One thread = 4 slots.  Vote: MajorityVote (the reference's) or IupacVote
-// (kdl_common.cuh); the policy argument comes last and defaults to the majority, so the majority instantiations keep
-// their code and their callers.
+// n_slots % 4 == 0, slot_lo % 4 == 0.  One thread = 4 slots.  Vote: MajorityVote (the reference's), IupacVote or
+// QualityVote (kdl_common.cuh); the policy argument comes last and defaults to the majority, so the majority
+// instantiations keep their code and their callers.
 template <bool kPeers, class Vote = MajorityVote>
 __global__ void __launch_bounds__(256)
 vote_kernel(const int32_t* __restrict__ counts, Peers peers, long long n_slots, long long slot_lo,
@@ -87,10 +87,10 @@ vote_kernel(const int32_t* __restrict__ counts, Peers peers, long long n_slots, 
     const long long d1 = (long long)v[0].y + v[1].y + v[2].y + v[3].y;
     const long long d2 = (long long)v[0].z + v[1].z + v[2].z + v[3].z;
     const long long d3 = (long long)v[0].w + v[1].w + v[2].w + v[3].w;
-    const unsigned c0 = vote(v[0].x, v[1].x, v[2].x, v[3].x, v[4].x, v[5].x, v[6].x, d1, min_depth_ceil);
-    const unsigned c1 = vote(v[0].y, v[1].y, v[2].y, v[3].y, v[4].y, v[5].y, v[6].y, d2, min_depth_ceil);
-    const unsigned c2 = vote(v[0].z, v[1].z, v[2].z, v[3].z, v[4].z, v[5].z, v[6].z, d3, min_depth_ceil);
-    const unsigned c3 = vote(v[0].w, v[1].w, v[2].w, v[3].w, v[4].w, v[5].w, v[6].w, dn, min_depth_ceil);
+    const unsigned c0 = vote(s, v[0].x, v[1].x, v[2].x, v[3].x, v[4].x, v[5].x, v[6].x, d1, min_depth_ceil);
+    const unsigned c1 = vote(s + 1, v[0].y, v[1].y, v[2].y, v[3].y, v[4].y, v[5].y, v[6].y, d2, min_depth_ceil);
+    const unsigned c2 = vote(s + 2, v[0].z, v[1].z, v[2].z, v[3].z, v[4].z, v[5].z, v[6].z, d3, min_depth_ceil);
+    const unsigned c3 = vote(s + 3, v[0].w, v[1].w, v[2].w, v[3].w, v[4].w, v[5].w, v[6].w, dn, min_depth_ceil);
     *reinterpret_cast<uint32_t*>(calls + s) = c0 | (c1 << 8) | (c2 << 16) | (c3 << 24);
 }
 
@@ -225,10 +225,10 @@ vote_exchange_kernel(Exchange x, long long n_slots, long long min_depth_ceil, in
             const long long d1 = (long long)v[0].y + v[1].y + v[2].y + v[3].y;
             const long long d2 = (long long)v[0].z + v[1].z + v[2].z + v[3].z;
             const long long d3 = (long long)v[0].w + v[1].w + v[2].w + v[3].w;
-            const unsigned c0 = vote(v[0].x, v[1].x, v[2].x, v[3].x, v[4].x, v[5].x, v[6].x, d1, min_depth_ceil);
-            const unsigned c1 = vote(v[0].y, v[1].y, v[2].y, v[3].y, v[4].y, v[5].y, v[6].y, d2, min_depth_ceil);
-            const unsigned c2 = vote(v[0].z, v[1].z, v[2].z, v[3].z, v[4].z, v[5].z, v[6].z, d3, min_depth_ceil);
-            const unsigned c3 = vote(v[0].w, v[1].w, v[2].w, v[3].w, v[4].w, v[5].w, v[6].w, dn, min_depth_ceil);
+            const unsigned c0 = vote(s, v[0].x, v[1].x, v[2].x, v[3].x, v[4].x, v[5].x, v[6].x, d1, min_depth_ceil);
+            const unsigned c1 = vote(s + 1, v[0].y, v[1].y, v[2].y, v[3].y, v[4].y, v[5].y, v[6].y, d2, min_depth_ceil);
+            const unsigned c2 = vote(s + 2, v[0].z, v[1].z, v[2].z, v[3].z, v[4].z, v[5].z, v[6].z, d3, min_depth_ceil);
+            const unsigned c3 = vote(s + 3, v[0].w, v[1].w, v[2].w, v[3].w, v[4].w, v[5].w, v[6].w, dn, min_depth_ceil);
             *reinterpret_cast<uint32_t*>(calls + s) = c0 | (c1 << 8) | (c2 << 16) | (c3 << 24);
         }
     }
@@ -276,6 +276,8 @@ template __global__ void vote_kernel<true>(const int32_t*, Peers, long long, lon
                                            long long, uint8_t*, int32_t*, MajorityVote);
 template __global__ void vote_kernel<false, IupacVote>(const int32_t*, Peers, long long, long long, long long,
                                                        long long, uint8_t*, int32_t*, IupacVote);
+template __global__ void vote_kernel<false, QualityVote>(const int32_t*, Peers, long long, long long, long long,
+                                                         long long, uint8_t*, int32_t*, QualityVote);
 template __global__ void vote_exchange_kernel<MajorityVote>(Exchange, long long, long long, int, MajorityVote);
 template __global__ void vote_exchange_kernel<IupacVote>(Exchange, long long, long long, int, IupacVote);
 

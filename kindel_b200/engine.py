@@ -19,6 +19,8 @@ implementation behind these functions: without a CUDA device they raise.
     mask_overlaps(dbatch)      K10p + K10: the batch with its read pairs' second mates masked where the first covers
                                (extension); pileup then runs K10u
     quality_sums(dbatch, qual8)  K0 + K11 + K11g: the counted bases' qualities summed per slot (extension)
+    quality_weights(dbatch, qual8)  K0 + K11w + K11g-w: their quality weights summed per slot and base (extension)
+    vote_quality(counts, wsum)  K2w: the vote with the base by summed quality weights, and its Q (extension)
 """
 from __future__ import annotations
 
@@ -731,6 +733,37 @@ def quality_sums(dbatch: DeviceBatch, qual8: torch.Tensor):
                                     _stream_ptr(dev))
         _ffi.check(rc, "kdl_quality_pileup")
     return qsum, emass
+
+
+def quality_weights(dbatch: DeviceBatch, qual8: torch.Tensor) -> torch.Tensor:
+    """K0 + K11w (+ K11g-w): wsum int64 [4, n_slots] holding uint64 bits on the device -- per slot the summed
+    weight W[min(q, 93)] (kindel_b200/quality.py WEIGHT) of the counted A / C / G / T bases (include/kindel_b200.h
+    kdl_quality_weights).  The counted bases and qual8 are quality_sums'."""
+    lib = _ffi.load()
+    dev = dbatch.device
+    n_slots = dbatch.n_slots
+    with torch.cuda.device(dev):
+        wsum = torch.empty((4, n_slots), dtype=torch.int64, device=dev)
+        q = qual8 if qual8.numel() else torch.zeros(8, dtype=torch.uint8, device=dev)
+        rc = lib.kdl_quality_weights(C.byref(dbatch.struct), q.data_ptr(), wsum.data_ptr(), n_slots, _stream_ptr(dev))
+        _ffi.check(rc, "kdl_quality_weights")
+    return wsum
+
+
+def vote_quality(counts: torch.Tensor, wsum: torch.Tensor, min_depth=1, out: torch.Tensor = None):
+    """K2w (extension: quality_vote): (calls uint8[n_slots], qual uint8[n_slots]) on the device.  The change bits are
+    kdl_vote's; the emitted base is the one with the largest summed weight in wsum (quality_weights), N on a tie or
+    when no base has weight; qual is its Q (include/kindel_b200.h kdl_vote_quality)."""
+    lib = _ffi.load()
+    dev = counts.device
+    n_slots = counts.shape[1]
+    with torch.cuda.device(dev):
+        calls = out if out is not None else torch.empty(n_slots, dtype=torch.uint8, device=dev)
+        qual = torch.empty(n_slots, dtype=torch.uint8, device=dev)
+        rc = lib.kdl_vote_quality(counts.data_ptr(), wsum.data_ptr(), n_slots, int(math.ceil(min_depth)),
+                                  calls.data_ptr(), qual.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_vote_quality")
+    return calls, qual
 
 
 def dropped_event_rows(dbatch: DeviceBatch) -> np.ndarray:

@@ -57,6 +57,8 @@ class PileupRun:
     _device = None   # (count table, DeviceBatch) of host tables, uploaded on demand (device_tables)
     _reverse = None  # (count table, DeviceBatch) of the reverse-strand reads (reverse_table)
     _quality = None  # (qsum, emass) of the counted bases' qualities (quality_table)
+    _weights = None  # wsum of the counted bases' quality weights (quality_weights)
+    vote_qual = None  # K2w's Q per slot on the device after vote(quality=True), else None
     primers = None   # the PrimerSet whose primer bases the pileup masked (extension), None when off
     mask_overlaps = False  # the pileup counted each read pair once where its mates overlap (extension, K10)
     _dropped_events = None  # K10's dropped insertion-event rows of host tables
@@ -138,11 +140,40 @@ class PileupRun:
             self._quality = engine.quality_sums(dbatch, torch.from_numpy(self.batch.qual8).to(dbatch.device))
         return self._quality
 
-    def vote(self, min_depth=1, iupac_threshold=None) -> np.ndarray:
+    def quality_weights(self):
+        """wsum int64 [4, n_slots] (uint64 bits) on a device, built once (extension: quality_vote): K11w over the run's
+        masked device batch (device_tables(), so a multi-GPU result too) and its qual8, uploaded here.  Needs a batch
+        decoded with qual=True."""
+        if self._weights is None:
+            import torch
+
+            if self.batch.qual8 is None:
+                raise ValueError("quality_vote needs the reads' qualities: decode the batch with qual=True")
+            _, dbatch = self.device_tables()
+            self._weights = engine.quality_weights(dbatch, torch.from_numpy(self.batch.qual8).to(dbatch.device))
+        return self._weights
+
+    def vote(self, min_depth=1, iupac_threshold=None, quality=False) -> np.ndarray:
         """K2 over the whole table -> call bytes on the host (the device copy is kept for K5).  iupac_threshold:
-        extension, see bam_to_consensus."""
-        self.calls_device = engine.vote(self.counts, min_depth, iupac_threshold=iupac_threshold)
+        extension, see bam_to_consensus.  quality (extension): K2w over the table of device_tables() and
+        quality_weights() instead, its Q kept in vote_qual."""
+        if quality:
+            counts, _ = self.device_tables()
+            self.calls_device, self.vote_qual = engine.vote_quality(counts, self.quality_weights(), min_depth)
+        else:
+            self.calls_device = engine.vote(self.counts, min_depth, iupac_threshold=iupac_threshold)
         return self.calls_device.cpu().numpy()
+
+    def quality_vote_sites(self, min_depth=1) -> np.ndarray:
+        """The slots (int64, ascending) whose call byte of vote(quality=True) differs from kdl_vote's over the same
+        table: one more K2 and a compare on the device; only those slots come back."""
+        import torch
+
+        if self.vote_qual is None:
+            raise ValueError("quality_vote_sites needs the quality vote: call vote(quality=True) first")
+        counts, _ = self.device_tables()
+        base = engine.vote(counts, min_depth)
+        return torch.nonzero(base != self.calls_device).flatten().cpu().numpy().astype(np.int64)
 
     @property
     def ins_table(self) -> InsertionTable:
@@ -642,14 +673,16 @@ DepthRange = namedtuple("DepthRange", ["dmin", "dmax"])  # min / max ACGT depth 
 
 def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_depth, min_overlap,
                  clip_decay_threshold, trim_ends, uppercase, filters=None, iupac_threshold=None, primers=None,
-                 overlaps=None):
+                 overlaps=None, quality_vote_sites=None):
     """REPORT text block (reference kindel/kindel.py:437-485).  filters (extension): (min_base_quality, min_mapq,
     exclude_flags); when any is set, three option lines follow `- uppercase:`, otherwise the text is the reference's.
     iupac_threshold (extension): when set, `- iupac_threshold:` follows the option lines and `- iupac sites:` (the
     positions of multi-base calls, from the `iupac` list of a changes list this module built) follows
     `- ambiguous sites:`.  primers (extension): the primer BED's file name; when set, `- primers:` follows the filter
     lines.  overlaps (extension: mask_overlaps): K10's (pairs, bases, deletions, insertions); when set,
-    `- mate overlaps:` follows the filter and primer lines."""
+    `- mate overlaps:` follows the filter and primer lines.  quality_vote_sites (extension: quality_vote): the 1-based
+    positions (strings) whose call differs from the reference's vote; when set, `- quality_vote: True` follows the
+    option lines and `- quality-vote sites:` follows `- ambiguous sites:`."""
     if isinstance(weights, DepthRange):  # already reduced on the device: no table copy needed
         dmin, dmax = weights.dmin, weights.dmax
     elif isinstance(weights, BaseCounts):
@@ -686,6 +719,8 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
         lines.append("- mate overlaps: {} pairs, {} bases, {} deletions, {} insertions masked".format(*overlaps))
     if iupac_threshold is not None:
         lines.append("- iupac_threshold: {}".format(iupac_threshold))
+    if quality_vote_sites is not None:
+        lines.append("- quality_vote: True")
     lines += [
         "observations:",
         "- min, max observed depth: {}, {}".format(dmin, dmax),
@@ -693,6 +728,8 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
     ]
     if iupac_threshold is not None:
         lines.append("- iupac sites: {}".format(", ".join(getattr(changes, "iupac", None) or [])))
+    if quality_vote_sites is not None:
+        lines.append("- quality-vote sites: {}".format(", ".join(quality_vote_sites)))
     lines += [
         "- insertion sites: {}".format(", ".join(sites["I"])),
         "- deletion sites: {}".format(", ".join(sites["D"])),
@@ -704,7 +741,8 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
 # --------------------------------------------------------------------------------- public API
 def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_decay_threshold=0.1,
                      mask_ends=50, trim_ends=False, uppercase=False, devices=None, min_base_quality=0, min_mapq=0,
-                     exclude_flags=0, iupac_threshold=None, qualities=False, primers=None, mask_overlaps=False):
+                     exclude_flags=0, iupac_threshold=None, qualities=False, primers=None, mask_overlaps=False,
+                     quality_vote=False):
     """Consensus sequence(s) of an alignment file (reference kindel/kindel.py:488-555).
 
     Device work per file: one pileup (K1) and one vote (K2) over all contigs at once; only the
@@ -719,16 +757,32 @@ def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_d
 
     qualities (extension; default False): every record's `.qualities` is then a Phred+33 string, one character per
     character of `.sequence` (kindel_b200/quality.py has the rule); the sequence, changes and reports are those of
-    qualities=False.  Off, `.qualities` is None and nothing else runs."""
+    qualities=False.  Off, `.qualities` is None and nothing else runs.
+
+    quality_vote (extension; default False = off): where a base is emitted, it is the one whose reads' base qualities
+    give it the largest summed log-likelihood weight (W[q], kindel_b200/quality.py; the haploid maximum-likelihood base
+    under uniform priors), N on a tie or when no base has weight; an N count no longer makes the call N.  The D / N / I
+    changes and the inserted strings are those of the reference's vote.  With qualities, a base's Q is the weight gap
+    to the runner-up in Phred, capped at 60.  The batch is decoded with its qualities, so a kept read without them is a
+    ValueError; not together with iupac_threshold (ValueError)."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
+    quality_vote = check_quality_vote(quality_vote, iupac_threshold)
     filters = (min_base_quality, min_mapq, exclude_flags)
     run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold, primers=primers,
-                            mask_overlaps=mask_overlaps)
-    if calls is None:
-        calls = run.vote(min_depth, iupac_threshold)
+                            mask_overlaps=mask_overlaps, qual=quality_vote)
+    if calls is None or quality_vote:  # (several GPUs: the ranks' majority calls give way to the reduced table's)
+        calls = run.vote(min_depth, iupac_threshold, quality=quality_vote)
     return consensus_from_run(run, calls, bam_path, realign, min_depth, min_overlap,
                               clip_decay_threshold, mask_ends, trim_ends, uppercase, filters=filters,
-                              iupac_threshold=iupac_threshold, qualities=qualities)
+                              iupac_threshold=iupac_threshold, qualities=qualities, quality_vote=quality_vote)
+
+
+def check_quality_vote(quality_vote, iupac_threshold=None) -> bool:
+    """The one check of the quality_vote option: it cannot be combined with an IUPAC threshold (ValueError)."""
+    quality_vote = bool(quality_vote)
+    if quality_vote and iupac_threshold is not None:
+        raise ValueError("quality_vote cannot be combined with iupac_threshold")
+    return quality_vote
 
 
 class _Changes(list):
@@ -791,6 +845,8 @@ def _insertion_qualities(run, slots):
 def _slot_qualities(run, calls_all):
     """K2q over the run's table and calls: the device tensor when the table is on the device, else (host tables, e.g.
     a multi-GPU result) the four base columns and the calls go up to the current device and 1 B per slot comes back."""
+    if run.vote_qual is not None:  # (the quality vote wrote its own Q)
+        return run.vote_qual
     if run.counts is not None and run.calls_device is not None:
         return engine.consensus_qual(run.counts, run.calls_device)
     import torch
@@ -825,10 +881,17 @@ def _device_texts(run, calls_all, qual=None, ins_q=None):
 
 def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min_overlap=9,
                        clip_decay_threshold=0.1, mask_ends=50, trim_ends=False, uppercase=False, filters=None,
-                       iupac_threshold=None, qualities=False):
+                       iupac_threshold=None, qualities=False, quality_vote=False):
     """Host half of bam_to_consensus: per contig, optional CDR patches, string assembly, report.  The call bytes
     already carry the vote; iupac_threshold (extension) only adds its lines to the report.  qualities (extension):
-    see bam_to_consensus -- K2q (and, with the device text, K5q) on the device, the host assembly otherwise."""
+    see bam_to_consensus -- K2q (and, with the device text, K5q) on the device, the host assembly otherwise.
+    quality_vote (extension): the calls are the run's vote(quality=True); the qualities are then K2w's and the report
+    gains its lines."""
+    qv_slots = None
+    if quality_vote:
+        if getattr(run, "vote_qual", None) is None:
+            raise ValueError("quality_vote needs the run's quality vote: call vote(quality=True) first")
+        qv_slots = run.quality_vote_sites(min_depth)
     ins_table = run.ins_table
     consensuses, refs_changes, refs_reports = [], {}, {}
     primers_name = getattr(getattr(run, "primers", None), "name", None)
@@ -881,9 +944,13 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
         else:
             cons, changes = assemble_consensus(calls_all[s:e - 1], lambda p, s=s: ins_table.consensus_at(s + p),
                                                cdr_patches, trim_ends, uppercase)
+        qv_sites = None
+        if qv_slots is not None:
+            lo, hi = np.searchsorted(qv_slots, [s, e - 1])
+            qv_sites = [str(x - s + 1) for x in qv_slots[lo:hi].tolist()]
         report = build_report(ref_id, report_weights, changes, cdr_patches, bam_path, realign, min_depth,
                               min_overlap, clip_decay_threshold, trim_ends, uppercase, filters, iupac_threshold,
-                              primers=primers_name, overlaps=overlaps)
+                              primers=primers_name, overlaps=overlaps, quality_vote_sites=qv_sites)
         consensuses.append(consensus_seqrecord(cons, ref_id, quals))
         refs_reports[ref_id] = report
         refs_changes[ref_id] = changes

@@ -9,10 +9,31 @@ for the few characters it decides itself -- inserted strings -- and restates it 
 (D - k + 1) / (D + 2) is the rule of succession's posterior mean of the disagreement rate, so Q grows with agreement
 and with depth.  The compare is one correctly rounded multiply, as in CUDA, so host and device agree bit for bit.
 Quality characters are Phred+33: chr(33 + Q).
+
+The quality vote (extension: `quality_vote=True`, `kindel consensus --quality-vote`) weights each counted base of
+Phred q by WEIGHT[min(q, 93)], a constant table (its formula: DESIGN.md section 1, thirteenth extension): the
+log-likelihood ratio, in 1/65536 Phred, of "the true base is the one read" against "it is one particular other base".
+K11w sums it per slot and base, and K2w votes with the sums (include/kindel_b200.h kdl_quality_weights /
+kdl_vote_quality); the device holds the same table (kQualWeight, kindel_b200/csrc/quality.cu).
 """
 from __future__ import annotations
 
 QUAL_MAX = 60
+
+WEIGHT = (
+    0, 0, 160037, 311335, 430336, 532174, 623571, 708096,
+    787861, 864214, 938059, 1010026, 1080568, 1150020, 1218628, 1286580,
+    1354022, 1421062, 1487787, 1554264, 1620546, 1686672, 1752677, 1818584,
+    1884415, 1950185, 2015906, 2081590, 2147243, 2212872, 2278481, 2344076,
+    2409659, 2475232, 2540797, 2606356, 2671911, 2737461, 2803009, 2868554,
+    2934098, 2999640, 3065180, 3130720, 3196259, 3261797, 3327335, 3392873,
+    3458410, 3523947, 3589483, 3655020, 3720556, 3786093, 3851629, 3917165,
+    3982701, 4048238, 4113774, 4179310, 4244846, 4310382, 4375918, 4441454,
+    4506990, 4572526, 4638062, 4703598, 4769134, 4834670, 4900206, 4965742,
+    5031278, 5096814, 5162350, 5227886, 5293422, 5358958, 5424494, 5490030,
+    5555566, 5621102, 5686638, 5752174, 5817710, 5883246, 5948782, 6014318,
+    6079854, 6145390, 6210926, 6276462, 6341998, 6407534,
+)
 
 TEN = tuple(float.fromhex(h) for h in (
     "0x1.0000000000000p+0", "0x1.4248ef8fc2604p+0", "0x1.95bb8f6d46052p+0", "0x1.fec982d5bb8afp+0",

@@ -61,6 +61,10 @@ def row(path: str, d: dict) -> str:
     if d.get("floor"):
         work += ", K11 quality sums alone: %.3f ms, %.2f of its HBM floor" % (km.get("k0_k11_k11g_median", 0),
                                                                            d["floor"].get("share_of_floor", 0))
+    if d.get("weights_floor"):
+        qv = d.get("quality_vote_ms", {})
+        work += ", K11w quality weights alone: %.3f ms, %.2f of its HBM floor; K2w %.3f ms" % (
+            qv.get("k0_k11w_median", 0), d["weights_floor"].get("share_of_floor", 0), qv.get("k2w_median", 0))
     if d.get("map_ab"):
         work += ", zeroing A/B (dirty-sector map)"
     out = (f"| `{name}` | {work} | {d.get('n_gpus')} | {fmt(d.get('ms_per_step'), '.4f')} | {fmt(d.get('value'))} | "
