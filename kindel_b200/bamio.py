@@ -709,7 +709,8 @@ def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0,
 
 
 def missing_qualities(path, n: int) -> str:
-    return "%s: %d kept read(s) without base qualities (QUAL `*` or 0xff); --qual needs them" % (os.fspath(path), n)
+    return "%s: %d kept read(s) without base qualities (QUAL `*` or 0xff); --qual and --quality-vote need them" % (
+        os.fspath(path), n)
 
 
 def qual_layout(batch: ReadBatch, qual: np.ndarray) -> np.ndarray:

@@ -2,8 +2,9 @@
 qualities (an extension).
 
     qual(counts, calls) -> uint8[n_slots]                  Q of the base every slot emits (linear search over q)
-    fastq(counts, calls, s0, L, ins, patches, trim_ends, uppercase) -> (text, qualities)
-                                                           one contig walked position by position
+    fastq(counts, calls, s0, L, ins, patches, trim_ends, uppercase, qual=None) -> (text, qualities)
+                                                           one contig walked position by position; qual: the Q of
+                                                           every slot's emitted base (default: qual(counts, calls))
 
 `ins` maps a contig position to its insertion dict (string -> count, first-seen order); `patches` are the merged CDR
 Regions (start, end, seq) as the host code applies them.
@@ -43,7 +44,7 @@ def _load():
         lib.fqoracle_qual.restype = None
         lib.fqoracle_qual.argtypes = [vp, vp, i64, vp]
         lib.fqoracle_fastq.restype = i64
-        lib.fqoracle_fastq.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp]
+        lib.fqoracle_fastq.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp]
         _lib = lib
     return _lib
 
@@ -61,10 +62,13 @@ def qual(counts, calls) -> np.ndarray:
     return out
 
 
-def fastq(counts, calls, s0, L, ins, patches=None, trim_ends=False, uppercase=False):
+def fastq(counts, calls, s0, L, ins, patches=None, trim_ends=False, uppercase=False, qual=None):
     lib = _load()
     counts = np.ascontiguousarray(counts, dtype=np.int32)
     calls = np.ascontiguousarray(calls, dtype=np.uint8)
+    if qual is not None:  # (the quality vote's Q, one byte per slot of the table)
+        qual = np.ascontiguousarray(qual, dtype=np.uint8)
+        assert qual.shape == (counts.shape[1],)
     ins_k = np.zeros(L, dtype=np.int64)
     ins_off = np.zeros(L + 1, dtype=np.int64)
     blob = []
@@ -93,5 +97,5 @@ def fastq(counts, calls, s0, L, ins, patches=None, trim_ends=False, uppercase=Fa
     q = np.zeros(cap, dtype=np.uint8)
     n = lib.fqoracle_fastq(counts.ctypes.data, counts.shape[1], int(s0), int(L), calls.ctypes.data, ins_k.ctypes.data,
                            ins_off.ctypes.data, ib.ctypes.data, skip.ctypes.data, p_off.ctypes.data, pb.ctypes.data,
-                           int(bool(trim_ends)), int(bool(uppercase)), text.ctypes.data, q.ctypes.data)
+                           None if qual is None else qual.ctypes.data, int(bool(trim_ends)), int(bool(uppercase)), text.ctypes.data, q.ctypes.data)
     return text[:n].tobytes().decode("ascii"), q[:n].tobytes().decode("ascii")

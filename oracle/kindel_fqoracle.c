@@ -11,6 +11,7 @@
  * IUPAC set (bit 7, mask in bits 0-3, A=1 C=2 G=4 T=8) except the set of all four (the letter N), else 0.
  * An inserted string: k = its count in the position's insertion dict, D = max(min(depth, depth_next), k) with
  * depth_next the ACGT depth of the next slot (0 behind the last slot); a tie emits "N" at Q0.  A CDR patch: Q0.
+ * fqoracle_fastq takes the Q of every emitted base from slot_qual[s] instead when it is not NULL (the quality vote's Q).
  */
 #include <ctype.h>
 #include <stdint.h>
@@ -71,11 +72,12 @@ void fqoracle_qual(const int32_t* counts, const uint8_t* calls, int64_t n_slots,
  *   ins_k[p]    count of the modal inserted string (-1: a tie), read where the call has change 'I'
  *   ins_off[p .. p+1]  that string (as counted, upper case) in ins_bytes
  *   patch_skip[p]  INT64_MIN: no CDR patch starts here; else the patch (patch_off / patch_bytes) and end - start - 1
+ * slot_qual: NULL (the Q of slot_q), or the Q of every slot's emitted base.
  * Returns the length written to text / qual (both at least the untrimmed length). */
 int64_t fqoracle_fastq(const int32_t* counts, int64_t n_slots, int64_t s0, int64_t L, const uint8_t* calls,
                        const int64_t* ins_k, const int64_t* ins_off, const char* ins_bytes, const int64_t* patch_skip,
-                       const int64_t* patch_off, const char* patch_bytes, int trim_ends, int uppercase, char* text,
-                       char* qual) {
+                       const int64_t* patch_off, const char* patch_bytes, const uint8_t* slot_qual, int trim_ends,
+                       int uppercase, char* text, char* qual) {
     static const char* iupac = "=ACMGRSVTWYHKDBN";
     static const char* acgtn = "ACGTN";
     int64_t n = 0, skip = 0;
@@ -112,7 +114,7 @@ int64_t fqoracle_fastq(const int32_t* counts, int64_t n_slots, int64_t s0, int64
             }
         }
         text[n] = (c & 0x80) ? iupac[c & 15] : acgtn[(c & 7) > 4 ? 4 : (c & 7)];
-        qual[n++] = (char)(33 + slot_q(counts, n_slots, s, c));
+        qual[n++] = (char)(33 + (slot_qual ? slot_qual[s] : slot_q(counts, n_slots, s, c)));
     }
     int64_t a = 0, b = n;
     if (trim_ends) {
