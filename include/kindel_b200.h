@@ -483,6 +483,42 @@ int kdl_quality_weights(const kdl_batch* batch, const uint8_t* qual8, uint64_t* 
 int kdl_vote_quality(const int32_t* counts, const uint64_t* wsum, int64_t n_slots, int64_t min_depth_ceil,
                      uint8_t* calls, uint8_t* qual, void* stream);
 
+/* K12 / K12d (extension: `kindel amplicons --primers scheme.bed`): each read's amplicon, and the depth of each
+ * amplicon's insert.  The amplicons are the scheme's on the batch's contigs, numbered 0 .. n_amplicons - 1; per contig c
+ * and side (LEFT / RIGHT primers) the host gives the sorted breakpoints of that side's primer intervals,
+ * [left_off[c], left_off[c + 1]) of left_at, and per breakpoint k the label of the segment [at[k], at[k + 1]): the
+ * amplicon whose primers (alternates included) alone cover it, -3 where primers of several amplicons cover it, -1 where
+ * none does (the last breakpoint of a contig is -1).  Device pointers, int32 coordinates.
+ *   kdl_amplicons_assign  K12.  label[n_reads] int32: with s and e the walk cursors of the read's first and last M/=/X
+ *                         base as K9 takes them (before the Python index wrap), l = the label of s among its contig's
+ *                         LEFT segments and r = that of e among its RIGHT segments (-1 for a cursor outside [0, L) and
+ *                         for both when the read has no M/=/X base): -1 (unprimed) when both are -1; -3 (ambiguous)
+ *                         when either is -3; -2 (mispaired) when they are two different amplicons; else the amplicon
+ *                         one or both name.  One thread per read.
+ *   kdl_amplicons_depth   K12d.  With D(p) = A + C + G + T of `counts` (columns 0-3) at slot contig_slot[amp_contig[j]]
+ *                         + p: stats[3 j] = the sum of D over amplicon j's insert [insert_start[j], insert_end[j]),
+ *                         stats[3 j + 1] = its minimum and stats[3 j + 2] = the number of its positions with
+ *                         D >= min_depth; all three 0 for an insert that does not lie in 0 <= start < end <= L.  One
+ *                         warp per amplicon. */
+typedef struct kdl_amplicons {
+    int32_t n_contigs;
+    int32_t n_amplicons;
+    const int64_t* left_off;   /* [n_contigs + 1] */
+    const int32_t* left_at;
+    const int32_t* left_label;
+    const int64_t* right_off;  /* [n_contigs + 1] */
+    const int32_t* right_at;
+    const int32_t* right_label;
+    const int32_t* amp_contig;   /* [n_amplicons] */
+    const int32_t* insert_start; /* [n_amplicons] */
+    const int32_t* insert_end;   /* [n_amplicons] */
+} kdl_amplicons;
+
+int kdl_amplicons_assign(const kdl_batch* batch, const kdl_amplicons* amplicons, int32_t* label, void* stream);
+int kdl_amplicons_depth(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                        int32_t n_contigs, const kdl_amplicons* amplicons, int64_t min_depth, int64_t* stats,
+                        void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced

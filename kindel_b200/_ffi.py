@@ -82,6 +82,22 @@ class KdlPrimers(C.Structure):
     ]
 
 
+class KdlAmplicons(C.Structure):
+    _fields_ = [
+        ("n_contigs", C.c_int32),
+        ("n_amplicons", C.c_int32),
+        ("left_off", C.c_void_p),
+        ("left_at", C.c_void_p),
+        ("left_label", C.c_void_p),
+        ("right_off", C.c_void_p),
+        ("right_at", C.c_void_p),
+        ("right_label", C.c_void_p),
+        ("amp_contig", C.c_void_p),
+        ("insert_start", C.c_void_p),
+        ("insert_end", C.c_void_p),
+    ]
+
+
 class KdlExchange(C.Structure):
     _fields_ = [
         ("n_ranks", C.c_int32),
@@ -168,6 +184,9 @@ _PROTOTYPES = {
     "kdl_quality_pileup": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "kdl_quality_weights": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "kdl_vote_quality": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_amplicons_assign": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlAmplicons), C.c_void_p, C.c_void_p]),
+    "kdl_amplicons_depth": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
+                                      C.POINTER(KdlAmplicons), C.c_int64, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers":(C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,

@@ -8,7 +8,8 @@ extension one FASTQ record per contig instead),
 (kindel.variants_vcf), against a FASTA with `--reference`, with per-strand counts and a strand odds ratio with
 `--strand` / `--max-sor`, with a base-quality QUAL with `--qual` / `--min-qual`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
 bases of every read before the pileup (kindel_b200/primers.py); `--mask-overlaps` counts each read pair once where
-its mates overlap (include/kindel_b200.h K10).
+its mates overlap (include/kindel_b200.h K10).  `amplicons --primers scheme.bed` (an extension) writes a TSV row per
+sample and amplicon of a tiled scheme: its reads (K12) and the depth of its insert (K12d).
 argh derived the flags from the function signatures (first letter as short option unless two
 parameters share it); argparse spells the same set out.  Note the CLI default `--min-overlap 7`
 (cli.py:13) differs from the API default 9 (kindel.py:492), as in the reference.
@@ -69,6 +70,25 @@ def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False,
         return
     kindel.variants(bam_path, abs_threshold, rel_threshold, only_variants, absolute, devices=gpus, **filters).to_csv(
         sys.stdout, sep="\t", index=False)
+
+
+def amplicons(bam_paths, primers, min_depth=20, gpus=None, **filters):
+    """Report each amplicon's reads and insert depth per sample (tiled amplicon schemes)"""
+    from . import kindel
+
+    df = kindel.amplicons(bam_paths, primers, min_depth, devices=gpus, **filters)
+    for name, (kept, assigned, unprimed, mispaired, ambiguous) in df.attrs["reads"].items():
+        rows = df[df["sample"] == name]
+        drop = rows.loc[rows["status"] == "dropout", "amplicon"].tolist()
+        print("%s: %d reads kept: %d assigned, %d unprimed, %d mispaired, %d ambiguous; %d amplicons, %d dropouts%s"
+              % (name, kept, assigned, unprimed, mispaired, ambiguous, len(rows), len(drop),
+                 (": " + ", ".join(drop)) if drop else ""), file=sys.stderr)
+    out = ["\t".join(kindel.AMPLICON_COLUMNS)]
+    for r in df.itertuples(index=False):
+        out.append("%s\t%s\t%s\t%s\t%d\t%d\t%d\t%d\t%d\t%.2f\t%d\t%.4f\t%s"
+                   % (r.sample, r.contig, r.amplicon, r.pool, r.start, r.end, r.insert_start, r.insert_end, r.reads,
+                      r.mean_depth, r.lowest_depth, r.covered, r.status))
+    sys.stdout.write("\n".join(out) + "\n")
 
 
 def plot(bam_path):
@@ -134,6 +154,12 @@ def _filters(a) -> dict:
         out["primers"] = a.primers
     if a.mask_overlaps:
         out["mask_overlaps"] = True
+    return out
+
+
+def _amplicon_filters(a) -> dict:
+    out = _filters(a)
+    del out["primers"]  # (the scheme itself)
     return out
 
 
@@ -222,6 +248,16 @@ def build_parser() -> argparse.ArgumentParser:
                                            a.rel_threshold, a.only_variants, a.absolute, a.gpus, a.vcf, a.reference,
                                            a.strand, a.max_sor, a.qual, a.min_qual, **_filters(a)))
 
+    # extension: per-amplicon reads and depth of a tiled primer scheme (the BED's name column says which primers pair)
+    p = sub.add_parser("amplicons", help=amplicons.__doc__, description=amplicons.__doc__, formatter_class=fmt)
+    p.add_argument("bam_path", nargs="+", help="path to SAM/BAM file; several files give one row block per sample")
+    p.add_argument("--min-depth", type=int, default=20,
+                   help="an amplicon whose insert's mean depth is below this is a dropout; `covered` counts its "
+                        "positions at or above it")
+    _add_gpus(p)
+    _add_filters(p)
+    p.set_defaults(func=lambda a: amplicons(a.bam_path, a.primers, a.min_depth, a.gpus, **_amplicon_filters(a)))
+
     p = sub.add_parser("plot", help=plot.__doc__, description=plot.__doc__, formatter_class=fmt)
     p.add_argument("bam_path", help="path to SAM/BAM file")
     p.set_defaults(func=lambda a: plot(a.bam_path))
@@ -258,9 +294,16 @@ def _check_variants_args(parser, args):
         parser.error("variants: --qual and --min-qual need --vcf (the table has no QUAL)")
 
 
+def _check_amplicons_args(parser, args):
+    if getattr(args, "command", None) == "amplicons" and args.primers is None:
+        parser.error("amplicons: --primers is required (a primer BED whose 4th column names each primer "
+                     "<amplicon>_LEFT or <amplicon>_RIGHT)")
+
+
 def main(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
+    _check_amplicons_args(parser, args)
     _check_consensus_args(parser, args)
     _check_variants_args(parser, args)
     if not getattr(args, "func", None):

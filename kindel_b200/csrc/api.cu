@@ -17,6 +17,7 @@
 #include "primers.cu"
 #include "mates.cu"
 #include "quality.cu"
+#include "amplicons.cu"
 
 namespace {
 
@@ -777,6 +778,35 @@ int kdl_overlap_untake(const int32_t* drops, int64_t n_drops, int32_t* counts, i
     if (n_drops == 0) return KDL_OK;
     KDL_LAUNCH(kdl::overlap_untake_kernel, (unsigned)((n_drops + kdl::M_THREADS - 1) / kdl::M_THREADS),
                kdl::M_THREADS, 0, (cudaStream_t)stream, drops, n_drops, counts, n_slots);
+    return check_launch();
+}
+
+static bool amplicons_ok(const kdl_amplicons* a, int32_t n_contigs) {
+    return a && a->n_contigs == n_contigs && a->n_amplicons >= 0 && a->left_off && a->right_off &&
+           (a->n_amplicons == 0 || (a->left_at && a->left_label && a->right_at && a->right_label && a->amp_contig &&
+                                    a->insert_start && a->insert_end));
+}
+
+int kdl_amplicons_assign(const kdl_batch* batch, const kdl_amplicons* amplicons, int32_t* label, void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (!amplicons_ok(amplicons, batch->n_contigs) || (batch->n_reads > 0 && !label)) return KDL_ERR_INVALID_ARG;
+    if (batch->n_reads == 0) return KDL_OK;
+    KDL_LAUNCH(kdl::amplicons_assign_kernel, (unsigned)((batch->n_reads + kdl::AM_THREADS - 1) / kdl::AM_THREADS),
+               kdl::AM_THREADS, 0, (cudaStream_t)stream, *batch, *amplicons, label);
+    return check_launch();
+}
+
+int kdl_amplicons_depth(const int32_t* counts, int64_t n_slots, const int64_t* contig_slot, const int32_t* contig_len,
+                        int32_t n_contigs, const kdl_amplicons* amplicons, int64_t min_depth, int64_t* stats,
+                        void* stream) {
+    if (!counts || n_slots <= 0 || n_contigs < 0 || !amplicons_ok(amplicons, n_contigs)) return KDL_ERR_INVALID_ARG;
+    if (amplicons->n_amplicons == 0) return KDL_OK;
+    if (!stats || !contig_slot || !contig_len) return KDL_ERR_INVALID_ARG;
+    const long long n = amplicons->n_amplicons;
+    KDL_LAUNCH(kdl::amplicons_depth_kernel, (unsigned)((n + kdl::AM_WARPS - 1) / kdl::AM_WARPS), kdl::AM_THREADS, 0,
+               (cudaStream_t)stream, counts, n_slots, contig_slot, contig_len, n_contigs, *amplicons, min_depth,
+               reinterpret_cast<long long*>(stats));
     return check_launch();
 }
 

@@ -56,6 +56,36 @@ __device__ __forceinline__ PrimerWindow primer_window(const kdl_primers& p, int 
     return w;
 }
 
+// The walk cursors *s, *e of the first and the last M/=/X base of a complex read (CIGAR words cig[0, n_ops), walk
+// from `start` on a contig of length L), before the Python index wrap: M/=/X and D advance the cursor, a first S does
+// not, a later S advances it while it is below L.  False when the read has no M/=/X base.  Shared by K9 and K12.
+__device__ __forceinline__ bool complex_ends(const uint32_t* __restrict__ cig, uint32_t n_ops, long long start,
+                                             long long L, long long* s, long long* e) {
+    long long r_pos = start;
+    bool any = false;
+    *s = 0;
+    *e = -1;
+    for (uint32_t i = 0; i < n_ops; ++i) {
+        const uint32_t cg = cig[i];
+        const long long len = cg >> 4;
+        const int op = cg & 0xF;
+        if (op == 0 || op == 7 || op == 8) {
+            if (len > 0) {
+                if (!any) *s = r_pos;
+                any = true;
+                *e = r_pos + len - 1;
+            }
+            r_pos += len;
+        } else if (op == 2) {
+            r_pos += len;
+        } else if (op == 4 && i != 0) {
+            long long n_adv = L - r_pos;
+            r_pos += n_adv < 0 ? 0 : (n_adv > len ? len : n_adv);
+        }
+    }
+    return any;
+}
+
 // Calls emit(q0, q1) for the query ranges [q0, q1) of read r's primer bases, ascending and disjoint (clipped to its
 // SEQ: a hard read whose walk runs past it raises in the pileup).  The walk is K1g's (pileup_general.cu): M/=/X and
 // D advance the cursor, a first S does not, a later S advances both cursors while the cursor is below L.
@@ -93,31 +123,12 @@ __device__ void primer_ranges(const kdl_batch& b, const kdl_primers& p, long lon
     const uint32_t n_ops = blk[0];
     const uint32_t* __restrict__ cig = blk + 2;
     // pass 1: the cursors of the first and the last M/=/X base
-    long long s = 0, e = -1, r_pos = start;
-    bool any = false;
-    for (uint32_t i = 0; i < n_ops; ++i) {
-        const uint32_t cg = cig[i];
-        const long long len = cg >> 4;
-        const int op = cg & 0xF;
-        if (op == 0 || op == 7 || op == 8) {
-            if (len > 0) {
-                if (!any) s = r_pos;
-                any = true;
-                e = r_pos + len - 1;
-            }
-            r_pos += len;
-        } else if (op == 2) {
-            r_pos += len;
-        } else if (op == 4 && i != 0) {
-            long long n_adv = L - r_pos;
-            r_pos += n_adv < 0 ? 0 : (n_adv > len ? len : n_adv);
-        }
-    }
-    if (!any) return;
+    long long s, e;
+    if (!complex_ends(cig, n_ops, start, L, &s, &e)) return;
     const PrimerWindow w = primer_window(p, c, s, e);
     if (w.B <= s && w.A > e) return;
     // pass 2: the ranges, op by op
-    r_pos = start;
+    long long r_pos = start;
     long long q_pos = 0;
     for (uint32_t i = 0; i < n_ops; ++i) {
         const uint32_t cg = cig[i];

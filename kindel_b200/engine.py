@@ -21,6 +21,9 @@ implementation behind these functions: without a CUDA device they raise.
     quality_sums(dbatch, qual8)  K0 + K11 + K11g: the counted bases' qualities summed per slot (extension)
     quality_weights(dbatch, qual8)  K0 + K11w + K11g-w: their quality weights summed per slot and base (extension)
     vote_quality(counts, wsum)  K2w: the vote with the base by summed quality weights, and its Q (extension)
+    assign_amplicons(dbatch, arrays)  K12: each read's amplicon label (extension: `kindel amplicons`)
+    amplicon_depth(counts, arrays, min_depth, ...)  K12d: per amplicon the sum, minimum and covered positions of the
+                               depth of its insert (extension)
 """
 from __future__ import annotations
 
@@ -643,6 +646,63 @@ def mask_primers(dbatch: DeviceBatch, arrays) -> DeviceBatch:
         _ffi.check(rc, "kdl_primers_apply")
     return DeviceBatch(host=dbatch.host, device=dev, tensors=tensors, struct=dbatch.struct, qmask=q,
                        primer_masked=(n_pr, n_pb), drops=dbatch.drops, overlap_masked=dbatch.overlap_masked)
+
+
+_AMPLICON_FIELDS = ("left_off", "left_at", "left_label", "right_off", "right_at", "right_label", "contig",
+                    "insert_start", "insert_end")
+
+
+def amplicons_struct(arrays, ptr: dict) -> _ffi.KdlAmplicons:
+    """kdl_amplicons over the pointers `ptr` of a primers.AmpliconArrays' fields."""
+    a = _ffi.KdlAmplicons()
+    a.n_contigs, a.n_amplicons = arrays.n_contigs, arrays.n_amplicons
+    for f in _AMPLICON_FIELDS:
+        setattr(a, "amp_contig" if f == "contig" else f, ptr[f])
+    return a
+
+
+def _amplicons_on(arrays, dev):
+    """(kdl_amplicons, keepalive tensors) of the arrays uploaded to `dev`."""
+    t = {f: torch.from_numpy(np.ascontiguousarray(getattr(arrays, f))).to(dev) for f in _AMPLICON_FIELDS}
+    return amplicons_struct(arrays, {f: (int(x.data_ptr()) if x.numel() else None) for f, x in t.items()}), t
+
+
+def assign_amplicons(dbatch: DeviceBatch, arrays) -> torch.Tensor:
+    """K12 (extension: `kindel amplicons`): int32 [n_reads] on the device, each read's amplicon -- an index into
+    `arrays` (primers.AmpliconArrays over the batch's contigs) -- or -1 (unprimed), -2 (mispaired), -3 (ambiguous);
+    include/kindel_b200.h has the rule.  Reads the batch's CIGARs and starts only, so a primer-masked batch gives the
+    same labels."""
+    lib = _ffi.load()
+    dev = dbatch.device
+    n = int(dbatch.struct.n_reads)
+    if arrays.n_contigs != int(dbatch.struct.n_contigs):
+        raise ValueError("amplicon arrays for %d contigs, the batch has %d" % (arrays.n_contigs, dbatch.struct.n_contigs))
+    with torch.cuda.device(dev):
+        label = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        a, keep = _amplicons_on(arrays, dev)
+        rc = lib.kdl_amplicons_assign(C.byref(dbatch.struct), C.byref(a), label.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_amplicons_assign")
+        del keep  # (the stream orders the kernel before any reuse of the freed blocks)
+    return label[:n]
+
+
+def amplicon_depth(counts: torch.Tensor, arrays, min_depth, contig_slot, contig_len) -> torch.Tensor:
+    """K12d (extension: `kindel amplicons`): int64 [n_amplicons, 3] on the device -- per amplicon of `arrays` the sum,
+    the minimum and the number of positions >= min_depth of A+C+G+T (columns 0-3 of `counts`) over its insert; the
+    table's layout is contig_slot / contig_len (the batch's)."""
+    lib = _ffi.load()
+    dev = counts.device
+    n = arrays.n_amplicons
+    with torch.cuda.device(dev):
+        stats = torch.zeros((max(n, 1), 3), dtype=torch.int64, device=dev)
+        slot, length, n_contigs = _device_layout(contig_slot, contig_len, dev)
+        a, keep = _amplicons_on(arrays, dev)
+        rc = lib.kdl_amplicons_depth(counts.data_ptr(), int(counts.shape[1]), slot.data_ptr(), length.data_ptr(),
+                                     n_contigs, C.byref(a), int(math.ceil(min_depth)), stats.data_ptr(),
+                                     _stream_ptr(dev))
+        _ffi.check(rc, "kdl_amplicons_depth")
+        del keep
+    return stats[:n]
 
 
 _OVERLAP_TOTALS = 8  # words of K10's totals record (include/kindel_b200.h)

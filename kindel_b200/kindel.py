@@ -1603,3 +1603,87 @@ def plotly_clips(bam_path):
                                                   yaxis=dict(type="linear", autorange=True)))
     out_fn = os.path.splitext(os.path.split(bam_path)[1])[0]
     py.plot(fig, filename=out_fn + ".plot.html")
+
+
+# ------------------------------------------------------------------------------------- amplicons (extension)
+AMPLICON_COLUMNS = ["sample", "contig", "amplicon", "pool", "start", "end", "insert_start", "insert_end", "reads",
+                    "mean_depth", "lowest_depth", "covered", "status"]
+
+
+def amplicon_label_counts(labels, n_amplicons):
+    """int64 [3 + n_amplicons] on the device: the reads labelled -3, -2, -1, then those of each amplicon.  The classes
+    are three reductions and only the assigned reads go through torch.bincount, so no bin takes millions of atomic
+    adds: on cfg 4's 6.7 M reads, 74 % of them unprimed, this takes 0.49 ms where one bincount of all labels takes
+    3.86 ms; on an amplicon batch of that size 0.86 ms against 0.51 ms (one H100 at 700 W,
+    profiles/h100_bench_n1_cfg4_5Mb_200x_amplicons.json)."""
+    import torch
+
+    lab = labels.long()
+    classes = torch.stack([(lab == k).sum() for k in (-3, -2, -1)])
+    return torch.cat([classes, torch.bincount(lab[lab >= 0], minlength=n_amplicons)])
+
+
+def amplicons_from_run(run, scheme, min_depth=20):
+    """The amplicon table of one piled run (extension: `kindel amplicons`): a DataFrame with the columns of
+    AMPLICON_COLUMNS but `sample`, one row per amplicon of `scheme` (primers.AmpliconScheme) on the run's contigs, in
+    contig order, then start, then name.  K12 labels every read of the run's device batch (device_tables(), so a
+    multi-GPU run too) and amplicon_label_counts counts them on the device; K12d reduces A+C+G+T of the count table over each
+    insert.  `reads` = the reads K12 gives to the amplicon, `mean_depth` = the sum over the insert / its length,
+    `lowest_depth` its minimum, `covered` = the share of its positions with A+C+G+T >= min_depth, `status` PASS or
+    `dropout` (mean_depth < min_depth).  attrs["reads"] = (kept, assigned, unprimed, mispaired, ambiguous)."""
+    import pandas as pd
+
+    from .primers import AMBIGUOUS, amplicon_arrays
+
+    batch = run.batch
+    arrays = amplicon_arrays(scheme, batch.contig_names, batch.contig_len)
+    counts, dbatch = run.device_tables()
+    n = arrays.n_amplicons
+    per = amplicon_label_counts(engine.assign_amplicons(dbatch, arrays), n).cpu().numpy()
+    stats = engine.amplicon_depth(counts, arrays, min_depth, batch.contig_slot, batch.contig_len).cpu().numpy()
+    idx = arrays.amplicon
+    length = (arrays.insert_end - arrays.insert_start).astype(np.int64)
+    mean = stats[:, 0] / np.maximum(length, 1) if n else np.zeros(0)
+    df = pd.DataFrame({
+        "contig": [batch.contig_names[c] for c in arrays.contig.tolist()],
+        "amplicon": [scheme.names[j] for j in idx.tolist()],
+        "pool": [scheme.pool[j] for j in idx.tolist()],
+        "start": scheme.start[idx], "end": scheme.end[idx],
+        "insert_start": arrays.insert_start.astype(np.int64), "insert_end": arrays.insert_end.astype(np.int64),
+        "reads": per[-AMBIGUOUS:].astype(np.int64),
+        "mean_depth": mean, "lowest_depth": stats[:, 1], "covered": stats[:, 2] / np.maximum(length, 1),
+        "status": np.where(mean < min_depth, "dropout", "PASS") if n else np.zeros(0, dtype=object),
+    }, columns=AMPLICON_COLUMNS[1:])
+    df.attrs["reads"] = (int(batch.n_reads), int(per[-AMBIGUOUS:].sum()), int(per[2]), int(per[1]), int(per[0]))
+    return df
+
+
+def amplicons(bam_path, primers, min_depth=20, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0,
+              mask_overlaps=False, samples=None):
+    """Per sample and amplicon of a tiled primer scheme, its reads and the depth of its insert (extension: `kindel
+    amplicons`; the reference has no such command).  bam_path: one alignment file or a list of them; primers: a named
+    primer BED (primers.load_scheme) or an AmpliconScheme.  Each file is piled with `primers=` the scheme's rows, under
+    the filters and mask_overlaps as in pileup_run, so the depths are the ones `consensus --primers` sees; files are
+    piled one after the other, and samples are named by cohort.sample_names (`samples=` or the file names).  Returns
+    a DataFrame with the columns AMPLICON_COLUMNS, in argument order of the samples, then amplicons_from_run's order;
+    attrs["reads"] = {sample: (kept, assigned, unprimed, mispaired, ambiguous)}."""
+    import pandas as pd
+
+    from .cohort import sample_names
+    from .primers import as_scheme
+
+    scheme = as_scheme(primers)
+    paths = [bam_path] if isinstance(bam_path, (str, os.PathLike)) else list(bam_path)
+    names = sample_names(paths, samples)
+    frames, reads = [], {}
+    for path, name in zip(paths, names):
+        run, _ = pileup_run(path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=scheme.primers,
+                            mask_overlaps=mask_overlaps)
+        df = amplicons_from_run(run, scheme, min_depth)
+        reads[name] = df.attrs["reads"]
+        df.insert(0, "sample", name)
+        frames.append(df)
+        del run
+    out = pd.concat(frames, ignore_index=True) if frames else pd.DataFrame(columns=AMPLICON_COLUMNS)
+    out.attrs["reads"] = reads
+    return out

@@ -240,6 +240,19 @@ def tiled_scheme(seed: int, contig_names, contig_lens, spacing: int = 200, overl
     return rows
 
 
+def named_scheme_bed(rows) -> str:
+    """tiled_scheme's rows as a named primer BED (`kindel amplicons`): per contig the k-th pair is `amp_<k>_LEFT` and
+    `amp_<k>_RIGHT`, pools 1 and 2 alternating, strands + and -."""
+    out, k_of = [], {}
+    for i in range(0, len(rows), 2):
+        (c, a, b), (_, x, y) = rows[i], rows[i + 1]
+        k = k_of.get(c, 0)
+        k_of[c] = k + 1
+        out.append("%s\t%d\t%d\tamp_%d_LEFT\t%d\t+\n" % (c, a, b, k, 1 + k % 2))
+        out.append("%s\t%d\t%d\tamp_%d_RIGHT\t%d\t-\n" % (c, x, y, k, 1 + k % 2))
+    return "".join(out)
+
+
 def amplicon_reads(seed: int, contig_len: int, depth: float, read_len: int = 150, spacing: int = 200,
                    overlap: int = 50, sub_rate: float = 0.01):
     """Tiled-amplicon sequencing of one random contig: (batch, scheme rows).  Every read starts at the start of an

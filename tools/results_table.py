@@ -54,6 +54,8 @@ def row(path: str, d: dict) -> str:
         work += ", + strand split (K8, reverse pileup)"
     if d.get("primers_ms"):
         work += ", + primer masking (K9, K1q)"
+    if d.get("amplicons_ms"):
+        work += ", + per-amplicon report (K12, label counts, K12d)"
     if d.get("mates_ms"):
         work += ", + mate-overlap masking (K10p, K10, K10u)"
     if d.get("cohort_ms"):
