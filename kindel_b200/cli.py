@@ -137,15 +137,15 @@ def _iupac_threshold(text: str) -> float:
 
 
 def _max_sor(text: str) -> float:
-    from .kindel import check_max_sor
+    from .vcf import check_number
 
-    return check_max_sor(float(text))  # ValueError (NaN) -> argparse error
+    return check_number(float(text), "max_sor")  # ValueError (NaN) -> argparse error
 
 
 def _min_qual(text: str) -> float:
-    from .kindel import check_min_qual
+    from .vcf import check_number
 
-    return check_min_qual(float(text))  # ValueError (NaN) -> argparse error
+    return check_number(float(text), "min_qual")  # ValueError (NaN) -> argparse error
 
 
 def _filters(a) -> dict:

@@ -1,6 +1,7 @@
 """Several samples in one VCF (extension: `kindel variants --vcf a.bam b.bam ...`, kindel.variants_vcf with a list).
 
-The one place that knows the shared layout and the union rules of a multi-sample VCF:
+The one place that knows the shared layout of a multi-sample VCF; it piles the samples and gathers what vcf.records
+writes:
 
   layout    the union of the samples' batch contigs -- the first file's batch order, then each contig a later file
             shows first, in that file's order; a name given two @SQ lengths is an error -- laid out by
@@ -11,27 +12,21 @@ The one place that knows the shared layout and the union rules of a multi-sample
             kindel.pileup_run as it would be alone and freed before the next one, so the device holds T and one
             sample's run: 28 * S * n_slots bytes plus one pileup.
   sites     K6m (engine.variant_sites_multi) over T: the slots where some sample passes, with the OR of the bits.
-  records   the single-sample writer's records, with INFO pooled over the samples and FORMAT DP:AD:AF per sample;
-            deletions are the union of the (slot, length) keys that pass in some sample, insertions the union of the
-            strings at a candidate slot that pass in some sample (variants_vcf has the rules)."""
+  records   vcf.records over every sample's rows at the sites, with FORMAT DP:AD:AF per sample: the deletions are
+            engine.deletion_union's union of the (slot, length) keys that pass in some sample, the insertions the
+            union of the samples' strings at a candidate slot (vcf.records has the rules)."""
 from __future__ import annotations
 
 import os
-import types
 
 import numpy as np
 
-from . import bamio, engine
+from . import bamio, engine, vcf
 from .insertions import decode_events
 from .primers import as_primer_set
 
 _LEN_BITS = engine._LEN_BITS
 _CHUNK = 1 << 24  # int32 entries of T gathered to the host at once (64 MB)
-_FORMAT = ['##FORMAT=<ID=DP,Number=1,Type=Integer,Description="The sample\'s depth: A + C + G + T + N + deletions '
-           '(indels: the depth the allele is measured against)">',
-           '##FORMAT=<ID=AD,Number=R,Type=Integer,Description="The sample\'s count of REF and of each ALT allele">',
-           '##FORMAT=<ID=AF,Number=A,Type=Float,Description="The sample\'s share of DP of each ALT allele, rounded '
-           'to 4 decimals">']
 
 
 def sample_names(paths, samples=None) -> list:
@@ -165,39 +160,6 @@ class Cohort:
             out[:, :, lo:lo + step] = self.table[:, 0:6].index_select(2, idx).cpu().numpy()
         return out
 
-    def deletion_union(self, abs_threshold, rel_threshold):
-        """The deletion keys that pass in some sample (count c > abs_threshold and c / depth(r) > rel_threshold, 0 at
-        depth 0), on the device: (slot int64[n], length int64[n], counts int64[S, n], depths int64[S, n]) on the
-        host, keys ascending; every sample's count (0 without the event) and six-allele depth at r."""
-        import torch
-
-        T = self.table
-        dev = T.device
-        a, r = engine.variant_abs_floor(abs_threshold), float(rel_threshold)
-        zero = torch.zeros((), dtype=torch.float64, device=dev)
-        passing = []
-        for i, (key, cnt) in enumerate(self.deletions):
-            if key.numel() == 0:
-                continue
-            depth = T[i, 0:6].index_select(1, key >> _LEN_BITS).to(torch.int64).sum(dim=0)
-            share = torch.where(depth > 0, cnt.to(torch.float64) / depth.clamp(min=1).to(torch.float64), zero)
-            passing.append(key[(cnt > a) & (share > r)])
-        if not passing:
-            z = np.zeros(0, dtype=np.int64)
-            return z, z.copy(), np.zeros((T.shape[0], 0), dtype=np.int64), np.zeros((T.shape[0], 0), dtype=np.int64)
-        union = torch.unique(torch.cat(passing), sorted=True)
-        slot = union >> _LEN_BITS
-        counts, depths = [], []
-        for i, (key, cnt) in enumerate(self.deletions):
-            if key.numel() == 0:
-                counts.append(torch.zeros_like(union))
-            else:
-                at = torch.searchsorted(key, union).clamp(max=key.numel() - 1)
-                counts.append(torch.where(key[at] == union, cnt[at], torch.zeros_like(cnt[at])))
-            depths.append(T[i, 0:6].index_select(1, slot).to(torch.int64).sum(dim=0))
-        return (slot.cpu().numpy(), (union & ((1 << _LEN_BITS) - 1)).cpu().numpy(),
-                torch.stack(counts).cpu().numpy().astype(np.int64), torch.stack(depths).cpu().numpy())
-
     def strings_at(self, i, slot) -> dict:
         """{string: count} of sample i's insertion events at a shared slot, in first-seen order."""
         slots, strings = self.insertions[i]
@@ -209,22 +171,9 @@ class Cohort:
 
 
 # ---------------------------------------------------------------------------------------------------- text
-def _sample_fields(dp, ad) -> list:
-    """FORMAT values DP:AD:AF of every sample: dp int64 [S], ad int64 [S, 1 + m] (REF, then each ALT); AF = each
-    ALT's share of DP rounded to 4 decimals (0 at DP 0)."""
-    dp = np.asarray(dp, dtype=np.int64)
-    ad = np.asarray(ad, dtype=np.int64)
-    with np.errstate(invalid="ignore", divide="ignore"):
-        af = np.round(np.where(dp[:, None] > 0, ad[:, 1:] / np.maximum(dp, 1)[:, None], 0.0), 4).tolist()
-    return ["%d:%s:%s" % (d, ",".join(map(str, a)), ",".join(map(repr, f)))
-            for d, a, f in zip(dp.tolist(), ad.tolist(), af)]
-
-
 def variants_vcf(paths, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
                  exclude_flags=0, reference=None, primers=None, mask_overlaps=False, samples=None) -> str:
     """The multi-sample VCF of kindel.variants_vcf given a list of paths (see there for the rules)."""
-    from .kindel import _af, _vcf_header, _VCF_ALT, _ACGTN
-
     paths = [os.fspath(p) for p in paths]
     if not paths:
         raise ValueError("variants_vcf needs at least one alignment file")
@@ -237,109 +186,21 @@ def variants_vcf(paths, abs_threshold=1, rel_threshold=0.01, devices=None, min_b
         from .reference import Reference, load_reference
 
         ref = reference if isinstance(reference, Reference) else load_reference(reference, lay)
-    like_run = types.SimpleNamespace(batch=lay, primers=cohort.primers, mask_overlaps=cohort.mask_overlaps)
-    header = _vcf_header(like_run, abs_threshold, rel_threshold, filters,
-                         reference_name=None if ref is None else ref.name)
-    header = header[:-1] + _FORMAT + ["##kindelSamples=%d" % len(paths),
-                                      "\t".join(["#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO\tFORMAT"] + names)]
-    lines = _records(cohort, None if ref is None else ref.codes, abs_threshold, rel_threshold, _af, _VCF_ALT, _ACGTN)
-    return "\n".join(header + lines) + "\n"
+    lines = vcf.header(lay.contig_names, lay.contig_len, abs_threshold, rel_threshold, filters, cohort.primers,
+                       cohort.mask_overlaps, reference_name=None if ref is None else ref.name, samples=names)
+    return "\n".join(lines + records(cohort, None if ref is None else ref.codes, abs_threshold, rel_threshold)) + "\n"
 
 
-def _records(cohort, ref_codes, abs_threshold, rel_threshold, _af, vcf_alt, acgtn) -> list:
+def records(cohort, ref_codes, abs_threshold, rel_threshold) -> list:
+    """The data lines of the cohort (vcf.records with FORMAT): K6m's sites, every sample's rows there (and at DPa's
+    slots), its insertion strings and the deletions that pass in some sample."""
     lay = cohort.layout
-    T = cohort.table
-    S = T.shape[0]
-    contig_slot = np.asarray(lay.contig_slot, dtype=np.int64)
-    contig_len = np.asarray(lay.contig_len, dtype=np.int64)
-    slot_t, mask_t = engine.variant_sites_multi(T, contig_slot, contig_len, ref_codes, abs_threshold, rel_threshold)
-    slot, mask = slot_t.cpu().numpy(), mask_t.cpu().numpy()
-    contig = np.searchsorted(contig_slot, slot, side="right") - 1
-    rows = cohort.rows(slot)                      # [S, 6, n]
-    depth = rows.sum(axis=1)                      # [S, n]
-    pooled = rows.sum(axis=0)                     # [6, n]
-    recs = []  # (contig, POS, kind, deletion length, insertion slot, rank, line)
-
-    if ref_codes is None:
-        total = pooled.sum(axis=0)
-        top = pooled.argmax(axis=0)
-        for i in range(slot.shape[0]):
-            m = int(mask[i])
-            alts = [(k, letter) for k, letter in vcf_alt if m >> k & 1]
-            if not alts:
-                continue  # N alone
-            c, tp, d = int(contig[i]), int(top[i]), int(total[i])
-            ks = [tp] + [k for k, _ in alts]
-            info = "DP={};AD={};AF={}".format(d, ",".join(str(int(pooled[k, i])) for k in ks),
-                                              ",".join(_af(int(pooled[k, i]), d) for k, _ in alts))
-            recs.append((c, int(slot[i] - contig_slot[c]) + 1, 0, 0, 0, 0, "\t".join(
-                [lay.contig_names[c], str(int(slot[i] - contig_slot[c]) + 1), ".", "ACGT"[tp] if tp < 4 and d > 0
-                 else "N", ",".join(letter for _, letter in alts), ".", "PASS", info, "DP:AD:AF"]
-                + _sample_fields(depth[:, i], rows[:, ks, i]))))
-        recs.sort(key=lambda x: x[:6])
-        return [x[6] for x in recs]
-
-    letters = np.frombuffer(b"ACGTN", dtype=np.uint8)[np.minimum(np.asarray(ref_codes), 4)].tobytes().decode("ascii")
-    p_all = slot - contig_slot[contig] if slot.size else slot
-    dpa = cohort.rows(np.where(p_all >= 1, slot - 1, slot)).sum(axis=1) if (mask & 64).any() else None  # [S, n]
-    for i in range(slot.shape[0]):
-        c, s, m = int(contig[i]), int(slot[i]), int(mask[i])
-        s0, L, name = int(contig_slot[c]), int(contig_len[c]), lay.contig_names[c]
-        p = s - s0
-        if m & 15:
-            alts = [k for k in range(4) if m >> k & 1]
-            g = int(ref_codes[s])
-            ad = np.zeros((S, 1 + len(alts)), dtype=np.int64)
-            if g < 4:
-                ad[:, 0] = rows[:, g, i]
-            ad[:, 1:] = rows[:, alts, i].reshape(S, len(alts))
-            tot, d = ad.sum(axis=0).tolist(), int(depth[:, i].sum())
-            info = "DP={};AD={};AF={}".format(d, ",".join(map(str, tot)), ",".join(_af(x, d) for x in tot[1:]))
-            recs.append((c, p + 1, 0, 0, 0, 0, "\t".join(
-                [name, str(p + 1), ".", letters[s], ",".join("ACGT"[k] for k in alts), ".", "PASS", info, "DP:AD:AF"]
-                + _sample_fields(depth[:, i], ad))))
-        if m & 64 and L > 0:
-            da = dpa[:, i]
-            per = [cohort.strings_at(j, s) for j in range(S)]
-            union = {}
-            for d_j in per:  # first sample that has the string, then its first-seen rank there
-                for text in d_j:
-                    union.setdefault(text, len(union))
-            for text, rank in union.items():
-                if not text:
-                    continue
-                ao = np.array([d_j.get(text, 0) for d_j in per], dtype=np.int64)
-                if not any(cnt > abs_threshold and (cnt / int(dj) if dj > 0 else 0.0) > rel_threshold
-                           for cnt, dj in zip(ao.tolist(), da.tolist())):
-                    continue
-                tot_dp, tot_ao = int(da.sum()), int(ao.sum())
-                info = "INDEL;DP={};AO={};AF={}".format(tot_dp, tot_ao, _af(tot_ao, tot_dp))
-                alt_text = text.translate(acgtn)
-                if p >= 1:
-                    pos, rf, alt = p, letters[s - 1], letters[s - 1] + alt_text
-                else:
-                    pos, rf, alt = 1, letters[s0], alt_text + letters[s0]
-                recs.append((c, pos, 2, 0, s, rank, "\t".join(
-                    [name, str(pos), ".", rf, alt, ".", "PASS", info, "DP:AD:AF"]
-                    + _sample_fields(da, np.stack([np.maximum(da - ao, 0), ao], axis=1)))))
-
-    d_slot, d_len, d_cnt, d_depth = cohort.deletion_union(abs_threshold, rel_threshold)
-    d_contig = np.searchsorted(contig_slot, d_slot, side="right") - 1
-    for i in range(d_slot.shape[0]):
-        c, s, n = int(d_contig[i]), int(d_slot[i]), int(d_len[i])
-        s0, L, name = int(contig_slot[c]), int(contig_len[c]), lay.contig_names[c]
-        r = s - s0
-        if r >= 1:
-            pos, rf, alt = r, letters[s - 1:s + n], letters[s - 1]
-        elif n < L:
-            pos, rf, alt = 1, letters[s0:s0 + n + 1], letters[s0 + n]
-        else:
-            continue  # the whole contig deleted: no base is left to anchor the record
-        ao, dp = d_cnt[:, i], d_depth[:, i]
-        tot_ao, tot_dp = int(ao.sum()), int(dp.sum())
-        info = "INDEL;DP={};AO={};AF={}".format(tot_dp, tot_ao, _af(tot_ao, tot_dp))
-        recs.append((c, pos, 1, n, 0, 0, "\t".join([name, str(pos), ".", rf, alt, ".", "PASS", info, "DP:AD:AF"]
-                                                   + _sample_fields(dp, np.stack([np.maximum(dp - ao, 0), ao],
-                                                                                 axis=1)))))
-    recs.sort(key=lambda x: x[:6])
-    return [x[6] for x in recs]
+    slot, mask = (x.cpu().numpy() for x in engine.variant_sites_multi(
+        cohort.table, lay.contig_slot, lay.contig_len, ref_codes, abs_threshold, rel_threshold))
+    dpa = dels = None
+    if ref_codes is not None:
+        if (mask & 64).any():
+            dpa = cohort.rows(vcf.dpa_slots(lay, slot)).sum(axis=1)  # [S, n]
+        dels = engine.deletion_union(cohort.deletions, cohort.table, abs_threshold, rel_threshold)
+    return vcf.records(lay, abs_threshold, rel_threshold, slot, mask, cohort.rows(slot), ref_codes=ref_codes, dpa=dpa,
+                       strings_at=cohort.strings_at, deletions=dels, per_sample=True)

@@ -14,6 +14,7 @@ implementation behind these functions: without a CUDA device they raise.
     variant_sites(counts, ...) K6: the variant sites of `variants --only-variants` and the VCF (extension)
     variant_sites_ref(...)     K6r: the SNV and insertion-candidate sites against a reference (extension)
     deletion_alleles(dbatch, counts, ...)  K7 + grouping: the deletion alleles against a reference (extension)
+    deletion_union(groups, table, ...)  the same rule over S samples' K7 groups: the keys that pass in some sample
     select_reads(dbatch, keep) K8: the sub-batch of the kept reads, built on the device (extension)
     mask_primers(dbatch, arrays)  K9: the batch with its amplicon primer bases masked (extension)
     mask_overlaps(dbatch)      K10p + K10: the batch with its read pairs' second mates masked where the first covers
@@ -894,23 +895,43 @@ def _deletion_groups(dbatch: DeviceBatch):
         return key[live], cnt[live]
 
 
-def deletion_alleles(dbatch: DeviceBatch, counts: torch.Tensor, abs_threshold, rel_threshold):
-    """The deletion alleles of `variants --vcf --reference` (extension): K7's events grouped by (slot, length) on the
-    device, each with its count c and the six-allele depth D of its first slot (columns 0-5 of `counts`, a device
-    table of the same batch); kept when c > abs_threshold and c / D > rel_threshold (0 at D = 0).  Only the kept
-    groups leave the device: (slot, length, count, depth), int64 numpy arrays sorted by slot, then length."""
-    key, cnt = _deletion_groups(dbatch)
+def _group_counts(key, cnt, q):
+    """The count of each queried key q in the groups (key ascending, cnt), 0 where it has none; on the device."""
     if key.numel() == 0:
-        z = np.zeros(0, dtype=np.int64)
-        return z, z.copy(), z.copy(), z.copy()
-    with torch.cuda.device(counts.device):
-        slot = key >> _LEN_BITS
-        length = key & ((1 << _LEN_BITS) - 1)
-        depth = counts[0:6].index_select(1, slot).to(torch.int64).sum(dim=0)
-        share = torch.where(depth > 0, cnt.to(torch.float64) / depth.clamp(min=1).to(torch.float64),
-                            torch.zeros((), dtype=torch.float64, device=counts.device))
-        keep = (cnt > variant_abs_floor(abs_threshold)) & (share > float(rel_threshold))
-        return tuple(x[keep].cpu().numpy().astype(np.int64) for x in (slot, length, cnt, depth))
+        return torch.zeros_like(q)
+    at = torch.searchsorted(key, q).clamp(max=key.numel() - 1)
+    return torch.where(key[at] == q, cnt[at], torch.zeros_like(cnt[at]))
+
+
+def deletion_alleles(dbatch: DeviceBatch, counts: torch.Tensor, abs_threshold, rel_threshold):
+    """deletion_union of one sample: K7's events of `dbatch` grouped on the device against `counts`, a device table
+    of the same batch; (slot, length, count, depth), int64 numpy arrays sorted by slot, then length."""
+    slot, length, cnt, depth = deletion_union([_deletion_groups(dbatch)], counts[None], abs_threshold, rel_threshold)
+    return slot, length, cnt[0], depth[0]
+
+
+def deletion_union(groups, table: torch.Tensor, abs_threshold, rel_threshold):
+    """The deletion alleles of `variants --vcf --reference` (extension) of S samples: groups holds each sample's K7
+    events grouped by (slot, length) (_deletion_groups) in the slots of `table`, the samples' device tables
+    (int32 [S, >= 6, n_slots]).  A group passes in its sample when its count c > abs_threshold and c / D >
+    rel_threshold (0 at D = 0), D the sample's six-allele depth at the deletion's first slot.  Only the union of the
+    keys that pass in some sample leaves the device: (slot int64[n], length int64[n], count int64 [S, n], depth int64
+    [S, n]) as numpy arrays sorted by slot, then length, with every sample's c (0 without the event) and D."""
+    a, r = variant_abs_floor(abs_threshold), float(rel_threshold)
+    with torch.cuda.device(table.device):
+        passing = []
+        for i, (key, cnt) in enumerate(groups):
+            depth = table[i, 0:6].index_select(1, key >> _LEN_BITS).to(torch.int64).sum(dim=0)
+            share = torch.where(depth > 0, cnt.to(torch.float64) / depth.clamp(min=1).to(torch.float64),
+                                torch.zeros((), dtype=torch.float64, device=table.device))
+            passing.append(key[(cnt > a) & (share > r)])
+        union = torch.unique(torch.cat(passing), sorted=True)
+        slot = union >> _LEN_BITS
+        counts = torch.stack([_group_counts(key, cnt, union) for key, cnt in groups])
+        depths = torch.stack([table[i, 0:6].index_select(1, slot).to(torch.int64).sum(dim=0)
+                              for i in range(len(groups))])
+        return (slot.cpu().numpy(), (union & ((1 << _LEN_BITS) - 1)).cpu().numpy(),
+                counts.cpu().numpy().astype(np.int64), depths.cpu().numpy())
 
 
 def deletion_counts(dbatch: DeviceBatch, slot, length) -> np.ndarray:
@@ -920,12 +941,8 @@ def deletion_counts(dbatch: DeviceBatch, slot, length) -> np.ndarray:
     if q.size == 0:
         return np.zeros(0, dtype=np.int64)
     key, cnt = _deletion_groups(dbatch)
-    if key.numel() == 0:
-        return np.zeros(q.shape[0], dtype=np.int64)
     with torch.cuda.device(dbatch.device):
-        tq = torch.from_numpy(q).to(key.device)
-        at = torch.searchsorted(key, tq).clamp(max=key.numel() - 1)
-        return torch.where(key[at] == tq, cnt[at], torch.zeros_like(cnt[at])).cpu().numpy().astype(np.int64)
+        return _group_counts(key, cnt, torch.from_numpy(q).to(key.device)).cpu().numpy().astype(np.int64)
 
 
 class HostContext:

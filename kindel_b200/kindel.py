@@ -14,17 +14,18 @@ There is no CPU implementation of the pileup or the vote in this package.
 """
 from __future__ import annotations
 
+import functools
 import logging
-import math
 import os
 from collections import OrderedDict, namedtuple
 
 import numpy as np
 
-from . import bamio, engine, quality
+from . import bamio, engine, quality, vcf
 from .primers import as_primer_set, primer_arrays
 from .insertions import InsertionTable, decode_events, dict_consensus
 from .views import Alignment, BaseCounts, Insertions
+from .vcf import QUAL_CAP, allele_quality, strand_odds_ratio  # noqa: F401  (kindel's VCF names)
 
 Region = namedtuple("Region", ["start", "end", "seq", "direction"])
 result = namedtuple("result", ["consensuses", "refs_changes", "refs_reports"])
@@ -1127,7 +1128,16 @@ def variants_from_run(run, abs_threshold=1, rel_threshold=0.01, only_variants=Fa
 
 
 # ------------------------------------------------------------------------------------------------ VCF
-_VCF_ALT = ((0, "A"), (1, "C"), (2, "G"), (3, "T"), (5, "*"))  # N (4) is not an allele
+# the VCF helpers under their kindel names (kindel_b200/vcf.py has them)
+_strand_fields = vcf.strand_fields
+check_max_sor = functools.partial(vcf.check_number, name="max_sor")
+check_min_qual = functools.partial(vcf.check_number, name="min_qual")
+
+
+def _vcf_header(run, abs_threshold, rel_threshold, filters, **options):
+    """vcf.header of a run: its contigs, primers and mate masking; options: vcf.header's keywords."""
+    return vcf.header(run.batch.contig_names, run.batch.contig_len, abs_threshold, rel_threshold, filters,
+                      getattr(run, "primers", None), getattr(run, "mask_overlaps", False), **options)
 
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
@@ -1150,7 +1160,7 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
 
     strand (extension: `--strand`): every record also carries ADF / ADR, the forward- and reverse-strand counts of REF
     and of each ALT, and SOR, the strand odds ratio of each ALT; max_sor (`--max-sor`, implies strand): FILTER `sor`
-    where some ALT's SOR exceeds it.  _strand_fields has the rules.
+    where some ALT's SOR exceeds it.  vcf.strand_fields has the rules.
 
     primers (extension: `--primers`): see pileup_run; the records then count no primer base (the strand counts
     neither), and the header gets `##kindelPrimers=<the BED's file name>`.
@@ -1170,8 +1180,8 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     AQ of its base ALTs, and INFO ;BQ= (the mean Phred of the counted bases of REF and of each ALT, `.` where there is
     none or the allele is no base) and ;AQ= (per ALT, `.` for `*`).  min_qual (`--min-qual`, implies qual): FILTER
     `lowqual` where QUAL < min_qual.  A record without a base ALT (an indel, a `*`-only site) keeps QUAL `.`.  The
-    qualities are summed on the device (K11, include/kindel_b200.h); allele_quality has the model.  Not available with
-    several samples (ValueError); a kept read without qualities is a ValueError."""
+    qualities are summed on the device (K11, include/kindel_b200.h); vcf.allele_quality has the model.  Not available
+    with several samples (ValueError); a kept read without qualities is a ValueError."""
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
     min_qual = check_min_qual(min_qual)
@@ -1195,68 +1205,6 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
                                  max_sor=max_sor, qual=qual, min_qual=min_qual)
 
 
-def check_max_sor(max_sor):
-    """None (no filter) or a float; NaN raises ValueError."""
-    if max_sor is None:
-        return None
-    x = float(max_sor)
-    if math.isnan(x):
-        raise ValueError("max_sor must be a number, got %r" % max_sor)
-    return x
-
-
-def check_min_qual(min_qual):
-    """None (no filter) or a float; NaN raises ValueError."""
-    if min_qual is None:
-        return None
-    x = float(min_qual)
-    if math.isnan(x):
-        raise ValueError("min_qual must be a number, got %r" % min_qual)
-    return x
-
-
-QUAL_CAP = 3000
-_EMASS_UNIT = 3.0 * 2.0 ** 32  # emass counts expected errors in units of 2^-32; a third of them hit one given base
-
-
-def allele_quality(k: int, emass: int) -> int:
-    """AQ of a base ALT with count k at a slot whose counted bases sum to emass (K11): with the expected number of
-    errors that turn into this base, lambda = emass / (3 * 2^32), p = P(Poisson(lambda) >= k) =
-    scipy.special.gammainc(k, lambda) -- the Poisson approximation to LoFreq's Poisson-binomial error model -- and AQ =
-    -10 log10(p) rounded half up, clamped to [0, 3000], 3000 when p underflows to 0.  k = 0 gives 0."""
-    from scipy.special import gammainc
-
-    if k <= 0:
-        return 0
-    p = float(gammainc(float(k), float(emass) / _EMASS_UNIT))
-    if p <= 0.0:
-        return QUAL_CAP
-    return min(max(int(math.floor(-10.0 * math.log10(p) + 0.5)), 0), QUAL_CAP)
-
-
-def _qual_fields(ref_col, alt_cols, counts, qsum, emass, min_qual):
-    """(QUAL, lowqual, INFO tail) of a record: ref_col / alt_cols the table columns of REF and of each ALT (0-3 a base,
-    4 N, 5 the deletion, None a reference base that is no base), counts / qsum their counts and quality sums at the
-    record's slot (columns 0-3), emass the slot's.  A record without a base ALT: (".", False, "")."""
-    if not any(k is not None and k < 4 for k in alt_cols):
-        return ".", False, ""
-
-    def bq(k):
-        return "." if k is None or k > 3 or counts[k] == 0 else "%.1f" % (qsum[k] / counts[k])
-
-    aq = [allele_quality(int(counts[k]), emass) if k < 4 else None for k in alt_cols]
-    q = max(a for a in aq if a is not None)
-    tail = ";BQ={};AQ={}".format(",".join(bq(k) for k in [ref_col] + list(alt_cols)),
-                                ",".join("." if a is None else str(a) for a in aq))
-    return str(q), min_qual is not None and q < min_qual, tail
-
-
-def _filter(strand_filter, lowqual):
-    """FILTER from the strand filter (`sor` or PASS) and lowqual, in the order sor, lowqual."""
-    failed = [f for f, on in (("sor", strand_filter == "sor"), ("lowqual", lowqual)) if on]
-    return ";".join(failed) if failed else "PASS"
-
-
 def _quality_at(run, slots):
     """(qsum int64 [4, n], emass list of n ints) of the run's quality table at host slots."""
     import torch
@@ -1270,22 +1218,6 @@ def _quality_at(run, slots):
     return q, [int(x) for x in emass.index_select(0, idx).cpu().numpy().view(np.uint64).tolist()]
 
 
-def strand_odds_ratio(f_ref, r_ref, f_alt, r_alt) -> float:
-    """GATK's StrandOddsRatio of one ALT from the forward / reverse counts of REF and of the ALT, in float64."""
-    t00, t01, t10, t11 = float(f_ref + 1), float(r_ref + 1), float(f_alt + 1), float(r_alt + 1)
-    ratio = (t00 / t01) * (t11 / t10) + (t01 / t00) * (t10 / t11)
-    return math.log(ratio) + math.log(min(t00, t01) / max(t00, t01)) - math.log(min(t10, t11) / max(t10, t11))
-
-
-def _strand_fields(adf, adr, max_sor):
-    """(FILTER, INFO tail) of a record whose REF and ALTs have forward counts adf and reverse counts adr: the tail is
-    ;ADF=..;ADR=..;SOR=.. (SOR per ALT, "%.3f"); FILTER is `sor` when max_sor is set and some ALT's SOR as written
-    exceeds it, else PASS."""
-    sor = ["%.3f" % strand_odds_ratio(adf[0], adr[0], adf[k], adr[k]) for k in range(1, len(adf))]
-    filt = "sor" if max_sor is not None and any(float(x) > max_sor for x in sor) else "PASS"
-    return filt, ";ADF={};ADR={};SOR={}".format(",".join(map(str, adf)), ",".join(map(str, adr)), ",".join(sor))
-
-
 def _rows_at(table, slots):
     """Columns 0-5 of a device table at host slots, int64 [6, n] on the host."""
     import torch
@@ -1297,61 +1229,33 @@ def _rows_at(table, slots):
     return table[0:6].index_select(1, idx).cpu().numpy().astype(np.int64)
 
 
-def _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None, strand=False, max_sor=None,
-                qual=False, min_qual=None):
-    from . import __version__
+def _reverse_strand(run, slot, deletions):
+    """The strand option of vcf.records from the run's reverse-strand reads: their rows at the sites and, with a
+    reference (deletions given), their DPa at the sites, each deletion's reverse count and depth and each insertion
+    string's reverse reads at a slot (the event rows whose read is reverse)."""
+    rev_table, rev_batch = run.reverse_table()
+    rows = _rows_at(rev_table, slot)
+    if deletions is None:
+        return rows, None, None, None, None
+    batch = run.batch
 
-    mbq, mapq, flags = filters if filters is not None else (0, 0, 0)
-    lines = ["##fileformat=VCFv4.2", "##source=kindel {}".format(__version__),
-             "##kindelVariants=abs_threshold={};rel_threshold={};min_base_quality={};min_mapq={};exclude_flags={:#x}"
-             .format(abs_threshold, rel_threshold, mbq, mapq, flags)]
-    primers = getattr(run, "primers", None)
-    if primers is not None:
-        lines.append("##kindelPrimers={}".format(primers.name))
-    if getattr(run, "mask_overlaps", False):
-        lines.append("##kindelMateOverlaps=R2 masked where R1 covers")
-    if strand:
-        lines.append("##kindelStrand=max_sor={}".format("." if max_sor is None else max_sor))
-    if qual:
-        lines.append("##kindelQual=model=poisson;min_qual={}".format("." if min_qual is None else min_qual))
-    if reference_name is not None:
-        lines.append("##reference={}".format(reference_name))
-    lines += ["##contig=<ID={},length={}>".format(name, int(L))
-              for name, L in zip(run.batch.contig_names, run.batch.contig_len)]
-    lines += ['##INFO=<ID=DP,Number=1,Type=Integer,Description="Depth: A + C + G + T + N + deletions">',
-              '##INFO=<ID=AD,Number=R,Type=Integer,Description="Count of REF (the most frequent allele) and of each '
-              'ALT allele">' if reference_name is None else
-              '##INFO=<ID=AD,Number=R,Type=Integer,Description="Count of the REF base and of each ALT base (SNVs)">',
-              '##INFO=<ID=AF,Number=A,Type=Float,Description="Share of the depth of each ALT allele, rounded to 4 '
-              'decimals">']
-    if reference_name is not None:
-        lines += ['##INFO=<ID=INDEL,Number=0,Type=Flag,Description="The record is an insertion or a deletion">',
-                  '##INFO=<ID=AO,Number=A,Type=Integer,Description="Count of the reads carrying the ALT allele">']
-    if strand:
-        lines += ['##INFO=<ID=ADF,Number=R,Type=Integer,Description="Forward-strand count of REF and of each ALT '
-                  'allele">',
-                  '##INFO=<ID=ADR,Number=R,Type=Integer,Description="Reverse-strand count of REF and of each ALT '
-                  'allele">',
-                  '##INFO=<ID=SOR,Number=A,Type=Float,Description="Strand odds ratio of each ALT allele against REF">']
-        if max_sor is not None:
-            lines.append('##FILTER=<ID=sor,Description="The strand odds ratio of an ALT allele is above {}">'
-                         .format(max_sor))
-    if qual:
-        lines += ['##INFO=<ID=BQ,Number=R,Type=Float,Description="Mean base quality of the counted bases of REF and of '
-                  'each ALT allele">',
-                  '##INFO=<ID=AQ,Number=A,Type=Integer,Description="Phred-scaled probability that sequencing errors '
-                  'alone give the ALT base its count (Poisson model)">']
-        if min_qual is not None:
-            lines.append('##FILTER=<ID=lowqual,Description="QUAL is below {}">'.format(min_qual))
-    lines.append("#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO")
-    return lines
+    def strings_at(s):
+        events = run.ins_table.rows_at(s)
+        out = {}
+        for text, r in zip(decode_events(batch, events), batch.reverse[events[:, 1].astype(np.int64)].tolist()):
+            out[text] = out.get(text, 0) + r
+        return out
+
+    return (rows, _rows_at(rev_table, vcf.dpa_slots(batch, slot)).sum(axis=0),
+            engine.deletion_counts(rev_batch, deletions[0], deletions[1]),
+            _rows_at(rev_table, deletions[0]).sum(axis=0), strings_at)
 
 
 def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None, reference=None, strand=False,
                           max_sor=None, qual=False, min_qual=None) -> str:
     """Host half of variants_vcf (see there): the VCF text of a finished pileup.  filters: (min_base_quality,
     min_mapq, exclude_flags) as the pileup applied them, for the header.  reference, strand, max_sor: see variants_vcf;
-    with a reference the records are _reference_records'.  Strand needs a run whose batch has `reverse`
+    vcf.records has the rules of the records.  Strand needs a run whose batch has `reverse`
     (ValueError otherwise).  A run piled with primers (extension) adds its `##kindelPrimers` line, one piled with
     mask_overlaps its `##kindelMateOverlaps` line.
 
@@ -1368,169 +1272,31 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
         raise ValueError("strand needs the reads' strands: decode the batch with strand=True")
     if qual and run.batch.qual8 is None:
         raise ValueError("qual needs the reads' qualities: decode the batch with qual=True")
-    sargs = dict(strand=strand, max_sor=max_sor, qual=qual, min_qual=min_qual)
+    batch = run.batch
+    ref = None
     if reference is not None:
         from .reference import Reference, load_reference
 
-        ref = reference if isinstance(reference, Reference) else load_reference(reference, run.batch)
-        lines = _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=ref.name, **sargs)
-        return "\n".join(lines + _reference_records(run, ref.codes, abs_threshold, rel_threshold, **sargs)) + "\n"
-    lines = _vcf_header(run, abs_threshold, rel_threshold, filters, **sargs)
-    site_slot, site_counts, site_mask = variant_sites(run, abs_threshold, rel_threshold)
-    rev = _rows_at(run.reverse_table()[0], site_slot) if strand else None
-    qs, em = _quality_at(run, site_slot) if qual else (None, None)
-    batch = run.batch
-    contig_slot = np.asarray(batch.contig_slot, dtype=np.int64)
-    t = site_counts.astype(np.int64)
-    depth, top, share, _ = variant_alleles(t, abs_threshold, rel_threshold)
-    rounded = np.round(share, 4)
-    contig = np.searchsorted(contig_slot, site_slot, side="right") - 1
-    for i in range(site_slot.shape[0]):
-        m = int(site_mask[i])
-        alts = [(k, letter) for k, letter in _VCF_ALT if m >> k & 1]
-        if not alts:
-            continue  # N alone
-        c = int(contig[i])
-        tp = int(top[i])
-        ref = "ACGT"[tp] if tp < 4 and depth[i] > 0 else "N"
-        ks = [tp] + [k for k, _ in alts]
-        info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(str(int(t[k, i])) for k in ks),
-                                          ",".join(repr(float(rounded[k, i])) for k, _ in alts))
-        filt, score = "PASS", "."
-        if strand:
-            adr = [int(rev[k, i]) for k in ks]
-            filt, tail = _strand_fields([int(t[k, i]) - x for k, x in zip(ks, adr)], adr, max_sor)
-            info += tail
-        if qual:
-            score, low, tail = _qual_fields(tp if tp < 4 and depth[i] > 0 else None, [k for k, _ in alts], t[:, i],
-                                            qs[:, i], em[i], min_qual)
-            filt = _filter(filt, low)
-            info += tail
-        lines.append("\t".join((batch.contig_names[c], str(int(site_slot[i] - contig_slot[c]) + 1), ".", ref,
-                                ",".join(letter for _, letter in alts), score, filt, info)))
+        ref = reference if isinstance(reference, Reference) else load_reference(reference, batch)
+    lines = _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None if ref is None else ref.name,
+                        strand=strand, max_sor=max_sor, qual=qual, min_qual=min_qual)
+    dpa = dels = None
+    if ref is None:
+        slot, site_counts, mask = variant_sites(run, abs_threshold, rel_threshold)
+    else:
+        # host tables (the multi-GPU result): the reduced table and the batch go to this process's GPU
+        counts, dbatch = run.device_tables()
+        slot, site_counts, dpa, mask = engine.variant_sites_ref(counts, batch.contig_slot, batch.contig_len, ref.codes,
+                                                                abs_threshold, rel_threshold)
+        dpa = dpa[None]
+        d_slot, d_len, d_cnt, d_depth = engine.deletion_alleles(dbatch, counts, abs_threshold, rel_threshold)
+        dels = d_slot, d_len, d_cnt[None], d_depth[None]
+    lines += vcf.records(batch, abs_threshold, rel_threshold, slot, mask, site_counts[None, 0:6].astype(np.int64),
+                         ref_codes=None if ref is None else ref.codes, dpa=dpa,
+                         strings_at=lambda j, s: run.ins_table.dict_at(s), deletions=dels,
+                         strand=_reverse_strand(run, slot, dels) if strand else None, max_sor=max_sor,
+                         qual=_quality_at(run, slot) if qual else None, min_qual=min_qual)
     return "\n".join(lines) + "\n"
-
-
-_ACGTN = str.maketrans({c: "N" for c in "=MRSVWYHKDB"})  # inserted bases: anything but A, C, G, T, N becomes N
-
-
-def _af(count, depth) -> str:
-    """A share rounded to 4 decimals as `variants` prints it (0 at depth 0)."""
-    return repr(float(np.round(np.float64(count / depth if depth > 0 else 0.0), 4)))
-
-
-def _reference_records(run, ref_codes, abs_threshold, rel_threshold, strand=False, max_sor=None, qual=False,
-                       min_qual=None):
-    """The VCF data lines against reference codes ref_codes (uint8 per slot, reference.py): SNVs from K6r's sites,
-    deletions from K7's grouped events, insertions from K6r's candidate slots and their strings (InsertionTable).
-
-    SNV, per position p with a variant base: POS p + 1, REF the reference letter, ALT the variant bases in A, C, G, T
-    order; INFO DP (six-allele depth), AD (the REF base's count -- 0 when the reference has no A, C, G or T there --
-    then each ALT's) and AF.  Deletion (r, n), count c, D = the depth at r: POS r, REF ref[r-1 .. r+n], ALT ref[r-1];
-    at r = 0 POS 1, REF ref[0 .. n], ALT ref[n] (no record for n = L).  Insertion of string s at slot p (first-seen
-    order of the slot's strings, empty ones skipped), count c against DPa: POS p, REF ref[p-1], ALT ref[p-1] + s; at
-    p = 0 POS 1, REF ref[0], ALT s + ref[0].  Indels carry INFO INDEL;DP;AO (= c);AF.  An allele passes when its count
-    exceeds abs_threshold and its share exceeds rel_threshold.  Order: contigs as in the batch, then POS, then SNV <
-    deletion < insertion, then deletion length, then insertion slot and first-seen order.  strand / max_sor: the
-    strand fields of variants_vcf_from_run.  qual / min_qual: the quality fields of the SNV records (variants_vcf)."""
-    batch = run.batch
-    # host tables (the multi-GPU result): the reduced table and the batch go to this process's GPU
-    counts, dbatch = run.device_tables()
-    rev_table, rev_batch = run.reverse_table() if strand else (None, None)
-    contig_slot = np.asarray(batch.contig_slot, dtype=np.int64)
-    contig_len = np.asarray(batch.contig_len, dtype=np.int64)
-    letters = np.frombuffer(b"ACGTN", dtype=np.uint8)[np.minimum(np.asarray(ref_codes), 4)].tobytes().decode("ascii")
-    recs = []  # (contig, POS, kind, deletion length, insertion slot, first-seen rank, line)
-
-    slot, site_counts, dpa, mask = engine.variant_sites_ref(counts, contig_slot, contig_len, ref_codes, abs_threshold,
-                                                            rel_threshold)
-    t = site_counts.astype(np.int64)
-    depth = t[0:6].sum(axis=0)
-    contig = np.searchsorted(contig_slot, slot, side="right") - 1
-    ins_table = run.ins_table if (mask & 64).any() else None
-    if strand:
-        rev_site = _rows_at(rev_table, slot)
-        # the reverse depth each insertion is measured against: DPa's slot
-        rev_dpa = _rows_at(rev_table, np.where(slot - contig_slot[contig] >= 1, slot - 1, slot)).sum(axis=0)
-    snv = np.flatnonzero(mask & 15)
-    qs, em = _quality_at(run, slot[snv]) if qual else (None, None)
-    q_of = {int(i): j for j, i in enumerate(snv.tolist())}
-    for i in range(slot.shape[0]):
-        c, s, m = int(contig[i]), int(slot[i]), int(mask[i])
-        s0, L, name = int(contig_slot[c]), int(contig_len[c]), batch.contig_names[c]
-        p = s - s0
-        if m & 15:
-            alts = [k for k in range(4) if m >> k & 1]
-            g = int(ref_codes[s])
-            ad = [int(t[g, i]) if g < 4 else 0] + [int(t[k, i]) for k in alts]
-            info = "DP={};AD={};AF={}".format(int(depth[i]), ",".join(map(str, ad)),
-                                              ",".join(_af(int(t[k, i]), int(depth[i])) for k in alts))
-            filt, score = "PASS", "."
-            if strand:
-                adr = [int(rev_site[g, i]) if g < 4 else 0] + [int(rev_site[k, i]) for k in alts]
-                filt, tail = _strand_fields([a - b for a, b in zip(ad, adr)], adr, max_sor)
-                info += tail
-            if qual:
-                j = q_of[i]
-                score, low, tail = _qual_fields(g if g < 4 else None, alts, t[:, i], qs[:, j], em[j], min_qual)
-                filt = _filter(filt, low)
-                info += tail
-            recs.append((c, p + 1, 0, 0, 0, 0, "\t".join((name, str(p + 1), ".", letters[s],
-                                                            ",".join("ACGT"[k] for k in alts), score, filt, info))))
-        if m & 64 and L > 0:
-            da = int(dpa[i])
-            strings = ins_table.dict_at(s)
-            if strand:  # each string's reverse-strand reads: the event rows whose read is reverse
-                rows = ins_table.rows_at(s)
-                rev_of = {}
-                for text, r in zip(decode_events(batch, rows), batch.reverse[rows[:, 1].astype(np.int64)].tolist()):
-                    rev_of[text] = rev_of.get(text, 0) + r
-            for rank, (text, cnt) in enumerate(strings.items()):
-                if not text or not (cnt > abs_threshold and (cnt / da if da > 0 else 0.0) > rel_threshold):
-                    continue
-                info = "INDEL;DP={};AO={};AF={}".format(da, cnt, _af(cnt, da))
-                filt = "PASS"
-                if strand:
-                    filt, tail = _indel_strand(da, int(rev_dpa[i]), cnt, rev_of.get(text, 0), max_sor)
-                    info += tail
-                text = text.translate(_ACGTN)
-                if p >= 1:
-                    pos, ref, alt = p, letters[s - 1], letters[s - 1] + text
-                else:
-                    pos, ref, alt = 1, letters[s0], text + letters[s0]
-                recs.append((c, pos, 2, 0, s, rank, "\t".join((name, str(pos), ".", ref, alt, ".", filt, info))))
-
-    d_slot, d_len, d_cnt, d_depth = engine.deletion_alleles(dbatch, counts, abs_threshold, rel_threshold)
-    d_contig = np.searchsorted(contig_slot, d_slot, side="right") - 1
-    if strand:
-        d_rev = engine.deletion_counts(rev_batch, d_slot, d_len)
-        d_rev_depth = _rows_at(rev_table, d_slot).sum(axis=0)
-    for i in range(d_slot.shape[0]):
-        c, s, n = int(d_contig[i]), int(d_slot[i]), int(d_len[i])
-        s0, L, name = int(contig_slot[c]), int(contig_len[c]), batch.contig_names[c]
-        r = s - s0
-        if r >= 1:
-            pos, ref, alt = r, letters[s - 1:s + n], letters[s - 1]
-        elif n < L:
-            pos, ref, alt = 1, letters[s0:s0 + n + 1], letters[s0 + n]
-        else:
-            continue  # the whole contig deleted: no base is left to anchor the record
-        cnt, dp = int(d_cnt[i]), int(d_depth[i])
-        info = "INDEL;DP={};AO={};AF={}".format(dp, cnt, _af(cnt, dp))
-        filt = "PASS"
-        if strand:
-            filt, tail = _indel_strand(dp, int(d_rev_depth[i]), cnt, int(d_rev[i]), max_sor)
-            info += tail
-        recs.append((c, pos, 1, n, 0, 0, "\t".join((name, str(pos), ".", ref, alt, ".", filt, info))))
-    recs.sort(key=lambda x: x[:6])
-    return [x[6] for x in recs]
-
-
-def _indel_strand(dp, dp_rev, ao, ao_rev, max_sor):
-    """_strand_fields of an indel record: DP and AO in total and on the reverse strand; forward = total - reverse;
-    REF's entry on strand s is max(DP_s - AO_s, 0)."""
-    dp_fwd, ao_fwd = dp - dp_rev, ao - ao_rev
-    return _strand_fields([max(dp_fwd - ao_fwd, 0), ao_fwd], [max(dp_rev - ao_rev, 0), ao_rev], max_sor)
 
 
 def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0,

@@ -14,7 +14,7 @@ this file adds what the count table does not keep and the VCF rules:
                     depth(p - 1) for p >= 1 and depth(0) for p = 0; depth(L) counts only the deletions at slot L
   deletion          event (r, n) with count c: c > abs and c / depth(r) > rel
 
-and writes the lines as kindel_b200/kindel.py's docstring of _reference_records states them.  Reference letters are
+and writes the lines as kindel_b200/vcf.py's docstring of records states them.  Reference letters are
 A, C, G, T or N (anything else reads as N).  Nothing here imports kindel_b200."""
 from __future__ import annotations
 

@@ -132,7 +132,7 @@ def run_workload(name, tmp):
     import torch
 
     import cohort_cases as CO
-    from kindel_b200 import __version__, bamio, cohort
+    from kindel_b200 import __version__, bamio, cohort, engine
     from kindel_b200 import kindel as K
 
     S, L, depth = WORKLOADS[name]
@@ -166,13 +166,13 @@ def run_workload(name, tmp):
 
     ref_codes = load_reference(fa, co.layout).codes
     t0 = time.perf_counter()
-    co.deletion_union(1, 0.01)
+    engine.deletion_union(co.deletions, co.table, 1, 0.01)
     union_s = time.perf_counter() - t0
     t0 = time.perf_counter()
-    pooled_lines = cohort._records(co, None, 1, 0.01, K._af, K._VCF_ALT, K._ACGTN)
+    pooled_lines = cohort.records(co, None, 1, 0.01)
     text_s = time.perf_counter() - t0
     t0 = time.perf_counter()
-    cohort._records(co, ref_codes, 1, 0.01, K._af, K._VCF_ALT, K._ACGTN)
+    cohort.records(co, ref_codes, 1, 0.01)
     text_ref_s = time.perf_counter() - t0
     kern = kernel_times(co, ref_codes)
     peak = torch.cuda.max_memory_allocated() / 1e9
@@ -219,8 +219,6 @@ def run_workload(name, tmp):
         want_slot = np.flatnonzero(passes.any(axis=0))
         want_mask = (passes[:, want_slot].astype(np.uint8) << np.arange(6, dtype=np.uint8)[:, None]).sum(
             axis=0, dtype=np.uint8)
-        from kindel_b200 import engine
-
         slot, mask = engine.variant_sites_multi(co.table, co.layout.contig_slot, co.layout.contig_len, None, 1, 0.01)
         parity = bool(np.array_equal(slot.cpu().numpy(), want_slot) and np.array_equal(mask.cpu().numpy(), want_mask))
         parity_detail = {"k6m_sites": int(want_slot.size), "oracle": "numpy restatement of the pooled site rule over "
