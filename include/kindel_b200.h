@@ -519,6 +519,25 @@ int kdl_amplicons_depth(const int32_t* counts, int64_t n_slots, const int64_t* c
                         int32_t n_contigs, const kdl_amplicons* amplicons, int64_t min_depth, int64_t* stats,
                         void* stream);
 
+/* K13 (extension: `--normalise N` with a named `--primers` scheme): the reads of each (amplicon, strand) group that
+ * the cap keeps, in batch order.  Per read r: key = 2 label[r] + (reverse[r] != 0) when 0 <= label[r] < n_amplicons
+ * (label: K12's), else none.  rank(r) = the reads before r in the batch with r's key.  keep[r] = 1 when r has no key
+ * or rank(r) < cap, else 0; total[key] = the reads of each key (K = 2 n_amplicons entries); *dropped = the sum over
+ * the keys of max(total - cap, 0) (int64).  cap >= 1.  Device pointers; `scratch` is int32 [scratch_words] with
+ * scratch_words >= kdl_normalise_scratch_words(n_reads, n_amplicons) on the same device.
+ *   K13c  G CTAs, CTA j over a contiguous run of the batch: its keys counted into row j of H[G][K] (scratch).
+ *   K13s  one thread per key: H[.][key] replaced by its exclusive prefix over j, the total and the dropped reads.
+ *   K13m  CTA j again, tile by tile in batch order: rank = H[j][key] + earlier warps' reads of the key in the tile +
+ *         the read's rank among its warp's peers; keep.
+ * G = min(2 SMs, tiles of 256 reads, KDL_NORMALISE_MAX_WORDS / K), at least 1: H takes at most
+ * KDL_NORMALISE_MAX_WORDS int32 (64 MB) unless K alone exceeds it.  The result does not depend on G. */
+#define KDL_NORMALISE_MAX_WORDS (1ll << 24)
+
+int64_t kdl_normalise_scratch_words(int64_t n_reads, int32_t n_amplicons);
+int kdl_normalise(const int32_t* label, const uint8_t* reverse, int64_t n_reads, int32_t n_amplicons, int64_t cap,
+                  int32_t* scratch, int64_t scratch_words, uint8_t* keep, int32_t* total, int64_t* dropped,
+                  void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced

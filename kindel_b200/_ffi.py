@@ -187,6 +187,9 @@ _PROTOTYPES = {
     "kdl_amplicons_assign": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlAmplicons), C.c_void_p, C.c_void_p]),
     "kdl_amplicons_depth": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
                                       C.POINTER(KdlAmplicons), C.c_int64, C.c_void_p, C.c_void_p]),
+    "kdl_normalise_scratch_words": (C.c_int64, [C.c_int64, C.c_int32]),
+    "kdl_normalise": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers":(C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,

@@ -97,7 +97,7 @@ class ReadBatch:
     mate_start: np.ndarray = field(default=None)    # int32 [n]
     pair_role: np.ndarray = field(default=None)     # uint8 [n]
     # base qualities (extension; `qual=True` at decode, K11): base k of read r at byte 8 * seq_off[r] + k, 0xff for the
-    # padding and a complex read's trailer words.  None = not asked for; select_reads and the shards leave it behind.
+    # padding and a complex read's trailer words.  None = not asked for; select_reads carries it, the shards leave it behind.
     qual8: np.ndarray = field(default=None)         # uint8 [8 * words of seq4]
 
     @property
@@ -442,9 +442,12 @@ def select_reads(batch: ReadBatch, idx) -> ReadBatch:
     seq_off = np.concatenate(([0], np.cumsum(words)))
     seq_src = np.repeat(batch.seq_off.astype(np.int64)[idx], words) + (
         np.arange(int(seq_off[-1])) - np.repeat(seq_off[:-1], words))
-    return finalize(batch.contig_names, batch.contig_len, read_off, batch.ref_start[idx], seq_off[:-1], lseq,
-                          cig_off, batch.cigar[cig_src], batch.seq4[seq_src], n_records=n, mask=_mask_of(batch, idx),
-                          reverse=None if batch.reverse is None else batch.reverse[idx], mates=_mates_at(batch, idx))
+    out = finalize(batch.contig_names, batch.contig_len, read_off, batch.ref_start[idx], seq_off[:-1], lseq,
+                   cig_off, batch.cigar[cig_src], batch.seq4[seq_src], n_records=n, mask=_mask_of(batch, idx),
+                   reverse=None if batch.reverse is None else batch.reverse[idx], mates=_mates_at(batch, idx))
+    if batch.qual8 is not None:  # each kept read's qualities, laid out by its new seq_off
+        out.qual8 = qual_layout(out, _ragged_gather(batch.qual8, 8 * batch.seq_off.astype(np.int64)[idx], lseq))
+    return out
 
 
 

@@ -8,7 +8,8 @@ extension one FASTQ record per contig instead),
 (kindel.variants_vcf), against a FASTA with `--reference`, with per-strand counts and a strand odds ratio with
 `--strand` / `--max-sor`, with a base-quality QUAL with `--qual` / `--min-qual`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
 bases of every read before the pileup (kindel_b200/primers.py); `--mask-overlaps` counts each read pair once where
-its mates overlap (include/kindel_b200.h K10).  `amplicons --primers scheme.bed` (an extension) writes a TSV row per
+its mates overlap (include/kindel_b200.h K10); `--normalise N` with a named scheme keeps at most N reads of each
+amplicon and strand (K12 + K13, include/kindel_b200.h).  `amplicons --primers scheme.bed` (an extension) writes a TSV row per
 sample and amplicon of a tiled scheme: its reads (K12) and the depth of its insert (K12d).
 argh derived the flags from the function signatures (first letter as short option unless two
 parameters share it); argparse spells the same set out.  Note the CLI default `--min-overlap 7`
@@ -77,12 +78,15 @@ def amplicons(bam_paths, primers, min_depth=20, gpus=None, **filters):
     from . import kindel
 
     df = kindel.amplicons(bam_paths, primers, min_depth, devices=gpus, **filters)
+    capped = df.attrs.get("dropped", {})  # (--normalise)
     for name, (kept, assigned, unprimed, mispaired, ambiguous) in df.attrs["reads"].items():
         rows = df[df["sample"] == name]
         drop = rows.loc[rows["status"] == "dropout", "amplicon"].tolist()
-        print("%s: %d reads kept: %d assigned, %d unprimed, %d mispaired, %d ambiguous; %d amplicons, %d dropouts%s"
+        print("%s: %d reads kept: %d assigned, %d unprimed, %d mispaired, %d ambiguous; %d amplicons, %d dropouts%s%s"
               % (name, kept, assigned, unprimed, mispaired, ambiguous, len(rows), len(drop),
-                 (": " + ", ".join(drop)) if drop else ""), file=sys.stderr)
+                 (": " + ", ".join(drop)) if drop else "",
+                 "; %d reads over the normalise cap dropped" % capped[name] if name in capped else ""),
+              file=sys.stderr)
     out = ["\t".join(kindel.AMPLICON_COLUMNS)]
     for r in df.itertuples(index=False):
         out.append("%s\t%s\t%s\t%s\t%d\t%d\t%d\t%d\t%d\t%.2f\t%d\t%.4f\t%s"
@@ -128,6 +132,16 @@ def _add_filters(p):
     p.add_argument("--mask-overlaps", action="store_true",
                    help="count each read pair once where its mates overlap: the second mate's bases, deletions and "
                         "insertions there are not counted where the first mate has information")
+    # extension: depth normalisation of amplicon data, off by default
+    p.add_argument("--normalise", type=_normalise, default=None, metavar="N",
+                   help="keep only the first N reads (file order) of each amplicon and strand of the --primers "
+                        "scheme, whose 4th column names each primer <amplicon>_LEFT or <amplicon>_RIGHT")
+
+
+def _normalise(text: str) -> int:
+    from .kindel import check_normalise
+
+    return check_normalise(int(text))  # ValueError (not an integer, below 1) -> argparse error
 
 
 def _iupac_threshold(text: str) -> float:
@@ -154,6 +168,8 @@ def _filters(a) -> dict:
         out["primers"] = a.primers
     if a.mask_overlaps:
         out["mask_overlaps"] = True
+    if a.normalise is not None:
+        out["normalise"] = a.normalise
     return out
 
 
@@ -294,6 +310,20 @@ def _check_variants_args(parser, args):
         parser.error("variants: --qual and --min-qual need --vcf (the table has no QUAL)")
 
 
+def _check_normalise_args(parser, args):
+    if getattr(args, "normalise", None) is None:
+        return
+    if args.primers is None:
+        parser.error("--normalise needs --primers (a primer BED whose 4th column names each primer <amplicon>_LEFT "
+                     "or <amplicon>_RIGHT)")
+    from .primers import load_scheme
+
+    try:
+        load_scheme(args.primers)
+    except (OSError, ValueError) as e:
+        parser.error("--normalise needs a named primer scheme: %s" % e)
+
+
 def _check_amplicons_args(parser, args):
     if getattr(args, "command", None) == "amplicons" and args.primers is None:
         parser.error("amplicons: --primers is required (a primer BED whose 4th column names each primer "
@@ -304,6 +334,7 @@ def main(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
     _check_amplicons_args(parser, args)
+    _check_normalise_args(parser, args)
     _check_consensus_args(parser, args)
     _check_variants_args(parser, args)
     if not getattr(args, "func", None):

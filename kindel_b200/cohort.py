@@ -23,7 +23,6 @@ import numpy as np
 
 from . import bamio, engine, vcf
 from .insertions import decode_events
-from .primers import as_primer_set
 
 _LEN_BITS = engine._LEN_BITS
 _CHUNK = 1 << 24  # int32 entries of T gathered to the host at once (64 MB)
@@ -87,13 +86,14 @@ class Cohort:
     """The samples piled one by one into the stacked table T over the shared layout, with what the records need of
     each: its deletion groups (device) and its insertion events (host), both in shared slots."""
 
-    def __init__(self, paths, devices=None, filters=(0, 0, 0), primers=None, mask_overlaps=False):
-        from .kindel import pileup_run
+    def __init__(self, paths, devices=None, filters=(0, 0, 0), primers=None, mask_overlaps=False, normalise=None):
+        from .kindel import _normalise_scheme, check_normalise, pileup_run
 
         import torch
 
         self.layout = Layout()
-        self.primers = as_primer_set(primers)
+        self.normalise = check_normalise(normalise)
+        self.primers, self.scheme = _normalise_scheme(primers, self.normalise)  # (the scheme: normalise's, loaded once)
         self.mask_overlaps = bool(mask_overlaps)
         self.table = None
         self.deletions = []   # per sample: (key = shared slot << 28 | length, count), device, keys ascending
@@ -101,8 +101,9 @@ class Cohort:
         S = len(paths)
         mbq, mapq, flags = filters
         for i, path in enumerate(paths):
-            run = pileup_run(path, devices, 1, mbq, mapq, flags, primers=self.primers,
-                             mask_overlaps=self.mask_overlaps)[0]
+            run = pileup_run(path, devices, 1, mbq, mapq, flags,
+                             primers=self.primers if self.scheme is None else self.scheme,
+                             mask_overlaps=self.mask_overlaps, normalise=self.normalise)[0]
             counts, dbatch = run.device_tables()
             batch = run.batch
             shared = self.layout.add(batch, path)
@@ -172,14 +173,15 @@ class Cohort:
 
 # ---------------------------------------------------------------------------------------------------- text
 def variants_vcf(paths, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
-                 exclude_flags=0, reference=None, primers=None, mask_overlaps=False, samples=None) -> str:
+                 exclude_flags=0, reference=None, primers=None, mask_overlaps=False, samples=None,
+                 normalise=None) -> str:
     """The multi-sample VCF of kindel.variants_vcf given a list of paths (see there for the rules)."""
     paths = [os.fspath(p) for p in paths]
     if not paths:
         raise ValueError("variants_vcf needs at least one alignment file")
     names = sample_names(paths, samples)
     filters = (min_base_quality, min_mapq, exclude_flags)
-    cohort = Cohort(paths, devices, filters, primers, mask_overlaps)
+    cohort = Cohort(paths, devices, filters, primers, mask_overlaps, normalise)
     lay = cohort.layout
     ref = None
     if reference is not None:
@@ -187,7 +189,8 @@ def variants_vcf(paths, abs_threshold=1, rel_threshold=0.01, devices=None, min_b
 
         ref = reference if isinstance(reference, Reference) else load_reference(reference, lay)
     lines = vcf.header(lay.contig_names, lay.contig_len, abs_threshold, rel_threshold, filters, cohort.primers,
-                       cohort.mask_overlaps, reference_name=None if ref is None else ref.name, samples=names)
+                       cohort.mask_overlaps, reference_name=None if ref is None else ref.name, samples=names,
+                       normalise=cohort.normalise)
     return "\n".join(lines + records(cohort, None if ref is None else ref.codes, abs_threshold, rel_threshold)) + "\n"
 
 

@@ -18,6 +18,7 @@
 #include "mates.cu"
 #include "quality.cu"
 #include "amplicons.cu"
+#include "normalise.cu"
 
 namespace {
 
@@ -807,6 +808,52 @@ int kdl_amplicons_depth(const int32_t* counts, int64_t n_slots, const int64_t* c
     KDL_LAUNCH(kdl::amplicons_depth_kernel, (unsigned)((n + kdl::AM_WARPS - 1) / kdl::AM_WARPS), kdl::AM_THREADS, 0,
                (cudaStream_t)stream, counts, n_slots, contig_slot, contig_len, n_contigs, *amplicons, min_depth,
                reinterpret_cast<long long*>(stats));
+    return check_launch();
+}
+
+// K13's grid: G CTAs of `per` tiles each over the batch's ceil(n / NM_THREADS) tiles -- two per SM as the persistent
+// grids, no more than there are tiles, and so few that H (G * K int32) stays within KDL_NORMALISE_MAX_WORDS (one CTA
+// when K alone exceeds it)
+static int normalise_grid(long long n_reads, long long n_keys, long long* per) {
+    const long long tiles = n_reads > 0 ? (n_reads + kdl::NM_THREADS - 1) / kdl::NM_THREADS : 1;
+    long long g = (long long)sm_count() * 2;
+    if (g > tiles) g = tiles;
+    if (n_keys > 0 && g > KDL_NORMALISE_MAX_WORDS / n_keys) g = KDL_NORMALISE_MAX_WORDS / n_keys;
+    if (g < 1) g = 1;
+    *per = (tiles + g - 1) / g;
+    return (int)((tiles + *per - 1) / *per);
+}
+
+int64_t kdl_normalise_scratch_words(int64_t n_reads, int32_t n_amplicons) {
+    if (n_reads < 0 || n_amplicons < 0 || n_amplicons > (1 << 30)) return -1;
+    long long per;
+    return (int64_t)normalise_grid(n_reads, 2ll * n_amplicons, &per) * 2ll * n_amplicons;
+}
+
+int kdl_normalise(const int32_t* label, const uint8_t* reverse, int64_t n_reads, int32_t n_amplicons, int64_t cap,
+                  int32_t* scratch, int64_t scratch_words, uint8_t* keep, int32_t* total, int64_t* dropped,
+                  void* stream) {
+    if (n_reads < 0 || n_amplicons < 0 || n_amplicons > (1 << 30) || cap < 1 || !dropped) return KDL_ERR_INVALID_ARG;
+    if (n_reads > 0 && (!label || !reverse || !keep)) return KDL_ERR_INVALID_ARG;
+    const long long K = 2ll * n_amplicons;
+    long long per;
+    const int grid = normalise_grid(n_reads, K, &per);
+    if (K > 0 && (!total || !scratch || scratch_words < (long long)grid * K)) return KDL_ERR_INVALID_ARG;
+    const cudaStream_t st = (cudaStream_t)stream;
+    long long* drop = reinterpret_cast<long long*>(dropped);
+    KDL_LAUNCH(kdl::normalise_count_kernel, (unsigned)grid, kdl::NM_THREADS, 0, st, label, reverse, n_reads,
+               n_amplicons, per, scratch, drop);
+    int rc = check_launch();
+    if (rc != KDL_OK) return rc;
+    if (K > 0) {
+        KDL_LAUNCH(kdl::normalise_scan_kernel, (unsigned)((K + kdl::NM_THREADS - 1) / kdl::NM_THREADS),
+                   kdl::NM_THREADS, 0, st, scratch, grid, n_amplicons, cap, total, drop);
+        rc = check_launch();
+        if (rc != KDL_OK) return rc;
+    }
+    if (n_reads == 0) return KDL_OK;
+    KDL_LAUNCH(kdl::normalise_mark_kernel, (unsigned)grid, kdl::NM_THREADS, 0, st, label, reverse, n_reads, n_amplicons,
+               per, cap, scratch, keep);
     return check_launch();
 }
 

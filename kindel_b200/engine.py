@@ -25,6 +25,8 @@ implementation behind these functions: without a CUDA device they raise.
     assign_amplicons(dbatch, arrays)  K12: each read's amplicon label (extension: `kindel amplicons`)
     amplicon_depth(counts, arrays, min_depth, ...)  K12d: per amplicon the sum, minimum and covered positions of the
                                depth of its insert (extension)
+    normalise(label, reverse, n_amplicons, cap)  K13: the reads each (amplicon, strand) cap keeps, in batch order
+                               (extension: `--normalise N`)
 """
 from __future__ import annotations
 
@@ -704,6 +706,30 @@ def amplicon_depth(counts: torch.Tensor, arrays, min_depth, contig_slot, contig_
         _ffi.check(rc, "kdl_amplicons_depth")
         del keep
     return stats[:n]
+
+
+def normalise(label: torch.Tensor, reverse: torch.Tensor, n_amplicons: int, cap: int):
+    """K13 (extension: `--normalise N`): (keep uint8 [n], total int32 [2 * n_amplicons], dropped int64 [1]) on the
+    device.  keep[r] = 0 for a read with an amplicon label (K12's, `label`) that has `cap` reads of its amplicon and
+    strand (`reverse`, 1 = FLAG & 0x10) before it in the batch, else 1; total = the reads of each (amplicon, strand),
+    2 * amplicon + strand; dropped = the reads with keep 0.  include/kindel_b200.h has the rule."""
+    lib = _ffi.load()
+    dev = label.device
+    n = int(label.numel())
+    if int(reverse.numel()) != n:
+        raise ValueError("normalise: %d labels and %d strand bytes" % (n, int(reverse.numel())))
+    with torch.cuda.device(dev):
+        label = label.to(torch.int32).contiguous()
+        reverse = reverse.to(torch.uint8).contiguous()
+        words = int(lib.kdl_normalise_scratch_words(n, int(n_amplicons)))
+        scratch = torch.empty(max(words, 1), dtype=torch.int32, device=dev)
+        keep = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        total = torch.empty(max(2 * int(n_amplicons), 1), dtype=torch.int32, device=dev)
+        dropped = torch.empty(1, dtype=torch.int64, device=dev)
+        rc = lib.kdl_normalise(label.data_ptr(), reverse.data_ptr(), n, int(n_amplicons), int(cap), scratch.data_ptr(),
+                               words, keep.data_ptr(), total.data_ptr(), dropped.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_normalise")
+    return keep[:n], total[:2 * int(n_amplicons)], dropped
 
 
 _OVERLAP_TOTALS = 8  # words of K10's totals record (include/kindel_b200.h)

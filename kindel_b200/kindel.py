@@ -22,7 +22,7 @@ from collections import OrderedDict, namedtuple
 import numpy as np
 
 from . import bamio, engine, quality, vcf
-from .primers import as_primer_set, primer_arrays
+from .primers import AmpliconScheme, PrimerSet, amplicon_arrays, as_primer_set, as_scheme, primer_arrays
 from .insertions import InsertionTable, decode_events, dict_consensus
 from .views import Alignment, BaseCounts, Insertions
 from .vcf import QUAL_CAP, allele_quality, strand_odds_ratio  # noqa: F401  (kindel's VCF names)
@@ -64,6 +64,7 @@ class PileupRun:
     mask_overlaps = False  # the pileup counted each read pair once where its mates overlap (extension, K10)
     _dropped_events = None  # K10's dropped insertion-event rows of host tables
     _overlap_stats = None   # K10's (pairs, bases, deletions, insertions) of host tables
+    normalised = None  # (N, dropped, kept) of the --normalise cap the batch went through (extension), None when off
 
     def __init__(self, batch: bamio.ReadBatch, device=None, primers=None, mask_overlaps=False):
         self.batch = batch
@@ -300,8 +301,52 @@ def _default_devices(devices):
     return max(1, int(devices))
 
 
+def check_normalise(normalise):
+    """The one check of the normalise option: None (off) or an integer >= 1 (ValueError otherwise)."""
+    if normalise is None:
+        return None
+    if isinstance(normalise, (bool, np.bool_)) or not isinstance(normalise, (int, np.integer)) or normalise < 1:
+        raise ValueError("normalise must be an integer >= 1, got %r" % (normalise,))
+    return int(normalise)
+
+
+def _normalise_scheme(primers, normalise):
+    """(PrimerSet or None, AmpliconScheme or None) of pileup_run's primers: normalise needs a named scheme."""
+    if normalise is None:
+        return as_primer_set(primers.primers if isinstance(primers, AmpliconScheme) else primers), None
+    if primers is None:
+        raise ValueError("normalise needs a named primer scheme: pass primers= (a BED whose 4th column names each "
+                         "primer <amplicon>_LEFT or <amplicon>_RIGHT)")
+    if isinstance(primers, PrimerSet):
+        raise ValueError("normalise needs a named primer scheme: pass the BED's path or an AmpliconScheme "
+                         "(primers.load_scheme), not a PrimerSet")
+    scheme = as_scheme(primers)
+    return scheme.primers, scheme
+
+
+def _normalise(batch, scheme, cap, strand):
+    """(the batch of the reads the cap keeps, (cap, dropped, kept)) (extension: normalise): K12 labels every read of
+    the uploaded batch with its amplicon under `scheme`, K13 keeps the first `cap` reads of each (amplicon, strand)
+    group in batch order, and only when it drops a read do the keep bytes (1 B per read) come back and the host batch
+    is rebuilt from the kept reads (bamio.select_reads).  The strand bytes stay only when `strand` asked for them."""
+    import torch
+
+    arrays = amplicon_arrays(scheme, batch.contig_names, batch.contig_len)
+    dbatch = engine.upload(batch, engine.require_cuda())
+    label = engine.assign_amplicons(dbatch, arrays)
+    reverse = torch.from_numpy(np.ascontiguousarray(batch.reverse, dtype=np.uint8)).to(dbatch.device)
+    keep, _, dropped = engine.normalise(label, reverse, arrays.n_amplicons, cap)
+    n_dropped = int(dropped.item())
+    if n_dropped:
+        batch = bamio.select_reads(batch, np.flatnonzero(keep.cpu().numpy()))
+    del dbatch, label, reverse, keep
+    if not strand:
+        batch.reverse = None
+    return batch, (cap, n_dropped, int(batch.n_reads))
+
+
 def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq=0, exclude_flags=0,
-               iupac_threshold=None, strand=False, primers=None, mask_overlaps=False, qual=False):
+               iupac_threshold=None, strand=False, primers=None, mask_overlaps=False, qual=False, normalise=None):
     """(PileupRun, calls) of an alignment file on `devices` GPUs.  devices > 1: one process per GPU, reads (or whole
     contigs) sharded, counts exchanged over NVLink in front of the vote (distributed.run_sharded); the result is
     bit-identical to one GPU.  min_base_quality / min_mapq / exclude_flags (extension, all off by default): a record
@@ -317,19 +362,31 @@ def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq
     then decoded with its mates.  With several GPUs the pairing and the masking run once on this process's GPU, and
     every rank takes back its own second mates' drops; the result is the same.  qual (extension, default False =
     off): the batch keeps its reads' base qualities (PileupRun.quality_table); a kept read without them is a
-    ValueError."""
+    ValueError.  normalise (extension, default None = off): an integer N >= 1 that needs `primers` to be a named
+    scheme (primers.load_scheme: a BED path or an AmpliconScheme; ValueError otherwise).  After the filters, each read
+    gets its amplicon (K12's label) and strand (FLAG & 0x10); of the reads with an amplicon, only the first N of each
+    (amplicon, strand) in batch order are kept (K13), and the others are removed from the batch as if they were not
+    in the file: no count, clip, event or mate of theirs.  Reads without an amplicon are never capped.  Everything
+    else -- primer masking, mate pairing, the pileup, several GPUs -- then runs on the kept reads; the run's
+    `normalised` holds (N, dropped, kept)."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
-    primers = as_primer_set(primers)
-    decode = dict(min_mapq=min_mapq, exclude_flags=exclude_flags, min_base_quality=min_base_quality, strand=strand)
+    normalise = check_normalise(normalise)
+    primers, scheme = _normalise_scheme(primers, normalise)
+    decode = dict(min_mapq=min_mapq, exclude_flags=exclude_flags, min_base_quality=min_base_quality,
+                  strand=strand or normalise is not None)
     if mask_overlaps:  # (the keyword only when on: the decode stays as it was otherwise)
         decode["mates"] = True
     if qual:
         decode["qual"] = True
     batch = bamio.read_alignment(bam_path, **decode)
+    normalised = None
+    if normalise is not None:
+        batch, normalised = _normalise(batch, scheme, normalise, strand)
     arrays = primer_arrays(primers, batch.contig_names, batch.contig_len) if primers is not None else None
     devices = _default_devices(devices)
     if devices <= 1:
         run = PileupRun(batch, primers=primers, mask_overlaps=mask_overlaps)
+        run.normalised = normalised
         return run, None
     from . import distributed
 
@@ -340,17 +397,19 @@ def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq
     calls, counts, derived, events = distributed.run_sharded(shards, devices, min_depth, iupac_threshold=iupac_threshold,
                                                              primers=arrays, drops=drops)
     dropped = None if drops is None else np.sort(drops[drops[:, 3] >= 0, 3].astype(np.int64))
-    return PileupRun.from_host_tables(batch, counts, derived, events, primers=primers, mask_overlaps=mask_overlaps,
-                                      dropped_events=dropped, overlap_stats=stats), calls
+    run = PileupRun.from_host_tables(batch, counts, derived, events, primers=primers, mask_overlaps=mask_overlaps,
+                                     dropped_events=dropped, overlap_stats=stats)
+    run.normalised = normalised
+    return run, calls
 
 
 def parse_bam(bam_path, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None,
-              mask_overlaps=False):
+              mask_overlaps=False, normalise=None):
     """Alignment information for each reference sequence, first-seen order
-    (reference kindel/kindel.py:131-153).  devices, the filters, primers and mask_overlaps: extensions, see
-    pileup_run."""
+    (reference kindel/kindel.py:131-153).  devices, the filters, primers, mask_overlaps and normalise: extensions,
+    see pileup_run."""
     return pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags,
-                      primers=primers, mask_overlaps=mask_overlaps)[0].alignments()
+                      primers=primers, mask_overlaps=mask_overlaps, normalise=normalise)[0].alignments()
 
 
 # --------------------------------------------------------------------------------- consensus
@@ -674,7 +733,7 @@ DepthRange = namedtuple("DepthRange", ["dmin", "dmax"])  # min / max ACGT depth 
 
 def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_depth, min_overlap,
                  clip_decay_threshold, trim_ends, uppercase, filters=None, iupac_threshold=None, primers=None,
-                 overlaps=None, quality_vote_sites=None):
+                 overlaps=None, quality_vote_sites=None, normalised=None):
     """REPORT text block (reference kindel/kindel.py:437-485).  filters (extension): (min_base_quality, min_mapq,
     exclude_flags); when any is set, three option lines follow `- uppercase:`, otherwise the text is the reference's.
     iupac_threshold (extension): when set, `- iupac_threshold:` follows the option lines and `- iupac sites:` (the
@@ -683,7 +742,8 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
     lines.  overlaps (extension: mask_overlaps): K10's (pairs, bases, deletions, insertions); when set,
     `- mate overlaps:` follows the filter and primer lines.  quality_vote_sites (extension: quality_vote): the 1-based
     positions (strings) whose call differs from the reference's vote; when set, `- quality_vote: True` follows the
-    option lines and `- quality-vote sites:` follows `- ambiguous sites:`."""
+    option lines and `- quality-vote sites:` follows `- ambiguous sites:`.  normalised (extension: normalise): the run's
+    (N, dropped, kept); when set, `- normalise:` follows the primer line."""
     if isinstance(weights, DepthRange):  # already reduced on the device: no table copy needed
         dmin, dmax = weights.dmin, weights.dmax
     elif isinstance(weights, BaseCounts):
@@ -716,6 +776,10 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
                   "- exclude_flags: {:#x}".format(filters[2])]
     if primers is not None:
         lines.append("- primers: {}".format(primers))
+    if normalised is not None:
+        cap, dropped, kept = normalised
+        lines.append("- normalise: {} per amplicon and strand, {} of {} reads dropped".format(cap, dropped,
+                                                                                           dropped + kept))
     if overlaps is not None:
         lines.append("- mate overlaps: {} pairs, {} bases, {} deletions, {} insertions masked".format(*overlaps))
     if iupac_threshold is not None:
@@ -743,13 +807,14 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
 def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_decay_threshold=0.1,
                      mask_ends=50, trim_ends=False, uppercase=False, devices=None, min_base_quality=0, min_mapq=0,
                      exclude_flags=0, iupac_threshold=None, qualities=False, primers=None, mask_overlaps=False,
-                     quality_vote=False):
+                     quality_vote=False, normalise=None):
     """Consensus sequence(s) of an alignment file (reference kindel/kindel.py:488-555).
 
     Device work per file: one pileup (K1) and one vote (K2) over all contigs at once; only the
     call bytes, the insertion events and -- for --realign and the report -- count columns come
     back to the host.  `devices` (extension; default $KINDEL_GPUS or 1) shards the pileup over that many GPUs of
-    the node.  min_base_quality / min_mapq / exclude_flags / primers / mask_overlaps: extension, see pileup_run.
+    the node.  min_base_quality / min_mapq / exclude_flags / primers / mask_overlaps / normalise: extension, see
+    pileup_run; with normalise the REPORT gains `- normalise:` after `- primers:`.
 
     iupac_threshold (extension; default None = off, the reference's vote): t in [0, 1].  Where a base is emitted,
     the call is the smallest set of the most frequent bases (A, C, G, T; N is not an allele) that holds at least
@@ -770,7 +835,7 @@ def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_d
     quality_vote = check_quality_vote(quality_vote, iupac_threshold)
     filters = (min_base_quality, min_mapq, exclude_flags)
     run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold, primers=primers,
-                            mask_overlaps=mask_overlaps, qual=quality_vote)
+                            mask_overlaps=mask_overlaps, qual=quality_vote, normalise=normalise)
     if calls is None or quality_vote:  # (several GPUs: the ranks' majority calls give way to the reduced table's)
         calls = run.vote(min_depth, iupac_threshold, quality=quality_vote)
     return consensus_from_run(run, calls, bam_path, realign, min_depth, min_overlap,
@@ -951,7 +1016,8 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
             qv_sites = [str(x - s + 1) for x in qv_slots[lo:hi].tolist()]
         report = build_report(ref_id, report_weights, changes, cdr_patches, bam_path, realign, min_depth,
                               min_overlap, clip_decay_threshold, trim_ends, uppercase, filters, iupac_threshold,
-                              primers=primers_name, overlaps=overlaps, quality_vote_sites=qv_sites)
+                              primers=primers_name, overlaps=overlaps, quality_vote_sites=qv_sites,
+                              normalised=getattr(run, "normalised", None))
         consensuses.append(consensus_seqrecord(cons, ref_id, quals))
         refs_reports[ref_id] = report
         refs_changes[ref_id] = changes
@@ -960,13 +1026,14 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
 
 def weights(bam_path: "path to SAM/BAM file", relative: "output relative nucleotide frequencies" = False,
             confidence: "calculate confidence interval" = True, confidence_alpha: "confidence interval alpha" = 0.01,
-            devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None, mask_overlaps=False):
+            devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None, mask_overlaps=False,
+            normalise=None):
     """DataFrame of per-site nucleotide frequencies, depth, consensus, clip starts/ends, confidence
     interval and entropy (reference kindel/kindel.py:558-630).  Integer columns come from the GPU
-    table; the float tail is the reference's arithmetic, vectorised.  devices, the filters, primers and
-    mask_overlaps: extensions, see pileup_run."""
+    table; the float tail is the reference's arithmetic, vectorised.  devices, the filters, primers,
+    mask_overlaps and normalise: extensions, see pileup_run."""
     run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers,
-                     mask_overlaps=mask_overlaps)[0]
+                     mask_overlaps=mask_overlaps, normalise=normalise)[0]
     return weights_from_run(run, relative, confidence, confidence_alpha)
 
 
@@ -1022,7 +1089,7 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
              rel_threshold: "relative frequency (0.0-1.0) above which to call variants" = 0.01,
              only_variants: "exclude invariant sites from output" = False,
              absolute: "report absolute variant frequencies" = False, devices=None, min_base_quality=0, min_mapq=0,
-             exclude_flags=0, primers=None, mask_overlaps=False):
+             exclude_flags=0, primers=None, mask_overlaps=False, normalise=None):
     """EXTENSION -- not in the reference snapshot.  The reference's README (README.md:106-107) lists a `variants`
     sub-command ("Output variants exceeding specified absolute and relative frequency thresholds") but its code
     (kindel/kindel.py, kindel/cli.py) has no such function, so there is nothing to be bit-exact with: parity
@@ -1032,9 +1099,9 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
     (variant_alleles).  Columns: chrom, pos, depth, consensus (allele letter, `-` = deletion), then one column per
     allele holding its relative (default) or absolute frequency where it is a variant and 0 elsewhere.  With
     only_variants the sites are selected on the device (K6, variant_sites) and only they are copied back.  primers,
-    mask_overlaps: extensions, see pileup_run."""
+    mask_overlaps, normalise: extensions, see pileup_run."""
     run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers,
-                     mask_overlaps=mask_overlaps)[0]
+                     mask_overlaps=mask_overlaps, normalise=normalise)[0]
     return variants_from_run(run, abs_threshold, rel_threshold, only_variants, absolute)
 
 
@@ -1136,13 +1203,15 @@ check_min_qual = functools.partial(vcf.check_number, name="min_qual")
 
 def _vcf_header(run, abs_threshold, rel_threshold, filters, **options):
     """vcf.header of a run: its contigs, primers and mate masking; options: vcf.header's keywords."""
+    normalised = getattr(run, "normalised", None)
     return vcf.header(run.batch.contig_names, run.batch.contig_len, abs_threshold, rel_threshold, filters,
-                      getattr(run, "primers", None), getattr(run, "mask_overlaps", False), **options)
+                      getattr(run, "primers", None), getattr(run, "mask_overlaps", False),
+                      normalise=None if normalised is None else normalised[0], **options)
 
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
                  exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None, mask_overlaps=False,
-                 samples=None, qual=False, min_qual=None) -> str:
+                 samples=None, qual=False, min_qual=None, normalise=None) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -1181,7 +1250,10 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     none or the allele is no base) and ;AQ= (per ALT, `.` for `*`).  min_qual (`--min-qual`, implies qual): FILTER
     `lowqual` where QUAL < min_qual.  A record without a base ALT (an indel, a `*`-only site) keeps QUAL `.`.  The
     qualities are summed on the device (K11, include/kindel_b200.h); vcf.allele_quality has the model.  Not available
-    with several samples (ValueError); a kept read without qualities is a ValueError."""
+    with several samples (ValueError); a kept read without qualities is a ValueError.
+
+    normalise (extension: `--normalise N`, needs a named `primers` scheme): see pileup_run; every sample's reads are
+    capped as it would be alone, and the header gets `##kindelNormalise=N` after `##kindelPrimers`."""
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
     min_qual = check_min_qual(min_qual)
@@ -1195,12 +1267,12 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
 
         return cohort.variants_vcf(bam_path, abs_threshold, rel_threshold, devices, min_base_quality, min_mapq,
                                    exclude_flags, reference=reference, primers=primers, mask_overlaps=mask_overlaps,
-                                   samples=samples)
+                                   samples=samples, normalise=normalise)
     if samples is not None:
         raise ValueError("samples= names the columns of several samples: pass the alignment files as a list")
     filters = (min_base_quality, min_mapq, exclude_flags)
     run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers, mask_overlaps=mask_overlaps,
-                     qual=qual)[0]
+                     qual=qual, normalise=normalise)[0]
     return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference, strand=strand,
                                  max_sor=max_sor, qual=qual, min_qual=min_qual)
 
@@ -1257,7 +1329,7 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
     min_mapq, exclude_flags) as the pileup applied them, for the header.  reference, strand, max_sor: see variants_vcf;
     vcf.records has the rules of the records.  Strand needs a run whose batch has `reverse`
     (ValueError otherwise).  A run piled with primers (extension) adds its `##kindelPrimers` line, one piled with
-    mask_overlaps its `##kindelMateOverlaps` line.
+    mask_overlaps its `##kindelMateOverlaps` line, one piled with normalise its `##kindelNormalise` line.
 
     Strand counts (ADF, ADR): without a reference they are the reverse table's counts of the record's AD columns and
     the total's minus those, so ADF + ADR == AD.  With one, an SNV's the same (REF 0 where the reference has no A, C,
@@ -1300,13 +1372,13 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
 
 
 def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0,
-             primers=None, mask_overlaps=False):
+             primers=None, mask_overlaps=False, normalise=None):
     """DataFrame of relative per-site nucleotide frequencies, indels and entropy
     (reference kindel/kindel.py:633-664), including its indexing of `i`/`d` by global row number
     into the LAST contig's tables (IndexError on most multi-contig files, SURVEY.md A-14).
-    devices, the filters, primers and mask_overlaps: extensions, see pileup_run."""
+    devices, the filters, primers, mask_overlaps and normalise: extensions, see pileup_run."""
     return features_from_run(pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags,
-                                        primers=primers, mask_overlaps=mask_overlaps)[0])
+                                        primers=primers, mask_overlaps=mask_overlaps, normalise=normalise)[0])
 
 
 def features_from_run(run):
@@ -1425,14 +1497,16 @@ def amplicons_from_run(run, scheme, min_depth=20):
 
 
 def amplicons(bam_path, primers, min_depth=20, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0,
-              mask_overlaps=False, samples=None):
+              mask_overlaps=False, samples=None, normalise=None):
     """Per sample and amplicon of a tiled primer scheme, its reads and the depth of its insert (extension: `kindel
     amplicons`; the reference has no such command).  bam_path: one alignment file or a list of them; primers: a named
     primer BED (primers.load_scheme) or an AmpliconScheme.  Each file is piled with `primers=` the scheme's rows, under
     the filters and mask_overlaps as in pileup_run, so the depths are the ones `consensus --primers` sees; files are
     piled one after the other, and samples are named by cohort.sample_names (`samples=` or the file names).  Returns
     a DataFrame with the columns AMPLICON_COLUMNS, in argument order of the samples, then amplicons_from_run's order;
-    attrs["reads"] = {sample: (kept, assigned, unprimed, mispaired, ambiguous)}."""
+    attrs["reads"] = {sample: (kept, assigned, unprimed, mispaired, ambiguous)}.  normalise (extension: `--normalise
+    N`): each file's reads are capped first (pileup_run), so the reads and depths are those of the kept reads, and
+    attrs["dropped"] = {sample: the reads over the cap}."""
     import pandas as pd
 
     from .cohort import sample_names
@@ -1441,15 +1515,21 @@ def amplicons(bam_path, primers, min_depth=20, devices=None, min_base_quality=0,
     scheme = as_scheme(primers)
     paths = [bam_path] if isinstance(bam_path, (str, os.PathLike)) else list(bam_path)
     names = sample_names(paths, samples)
-    frames, reads = [], {}
+    normalise = check_normalise(normalise)
+    frames, reads, dropped = [], {}, {}
     for path, name in zip(paths, names):
-        run, _ = pileup_run(path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=scheme.primers,
-                            mask_overlaps=mask_overlaps)
+        run, _ = pileup_run(path, devices, 1, min_base_quality, min_mapq, exclude_flags,
+                            primers=scheme.primers if normalise is None else scheme, mask_overlaps=mask_overlaps,
+                            normalise=normalise)
         df = amplicons_from_run(run, scheme, min_depth)
         reads[name] = df.attrs["reads"]
+        if normalise is not None:
+            dropped[name] = run.normalised[1]
         df.insert(0, "sample", name)
         frames.append(df)
         del run
     out = pd.concat(frames, ignore_index=True) if frames else pd.DataFrame(columns=AMPLICON_COLUMNS)
     out.attrs["reads"] = reads
+    if normalise is not None:
+        out.attrs["dropped"] = dropped
     return out
