@@ -34,7 +34,7 @@
  *                            too long for a tile: SURVEY.md A-7..A-10); bit 30 clear = "tile-eligible": every
  *                            slot it touches lies in [1, L - 1] of its contig, its query span fits its SEQ,
  *                            it has at most KDL_TILE_MAXOPS ops and reaches at most KDL_TILE_MAXREACH slots
- *                            to either side of its start, and all its bases are A,C,G,T,N -- K1 and K1e
+ *                            to either side of its start, and all its bases are A,C,G,T,N -- K1, K1w and K1e
  *                            walk it without bounds or error logic.  A tile-eligible read keeps its SEQ
  *                            length (<= KDL_FAST_MAXLEN) in bits 0..15 and its number of M/=/X ops in bits
  *                            16..22, so a tile can be sized before its bases are staged; a hard read keeps
@@ -168,8 +168,9 @@ int64_t kdl_launch_count(void);
  * several read shards -- can accumulate into one table) and writes the insertion event rows.
  * err_flag: device int32[4], caller-zeroed; [0] becomes non-zero if any read raised.
  * Coordinate-sorted batches (reads_sorted, tile_index scratch given) take K0 (tile index) + the tile-owner
- * kernel K1 (simple reads and the M/=/X bases of tile-eligible complex reads: no atomics), K1e (the sparse
- * insertion / deletion / clip updates of those complex reads, once per read) and K1g (KDL_HARD reads, atomics);
+ * kernel K1 (simple reads and the M/=/X bases of tile-eligible complex reads: no atomics), K1w (all of those
+ * complex reads' updates when they are rare, window by window) or K1e (their insertion / deletion / clip updates, once
+ * per read) and K1g (KDL_HARD reads, atomics);
  * anything else the order-independent atomic kernels K1s + K1g. */
 int kdl_pileup(const kdl_batch* batch, int32_t* counts, int64_t n_slots, int32_t* ins_events,
                int32_t* err_flag, void* stream);

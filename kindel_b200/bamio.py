@@ -77,7 +77,7 @@ class ReadBatch:
     cigar: np.ndarray             # uint32 [n_ops] (host only)
     seq4: np.ndarray              # uint32 [words]: per read its bases, complex reads followed by [n_ops][evt_off][ops]
     hard_idx: np.ndarray = field(default=None)      # uint32 [n_hard]: KDL_HARD reads (K1g walks them)
-    complex_idx: np.ndarray = field(default=None)   # uint32 [n_complex]: all complex reads (K1e walks the tile-eligible ones)
+    complex_idx: np.ndarray = field(default=None)   # uint32 [n_complex]: all complex reads (K1w / K1e walk the tile-eligible ones)
     n_events: int = 0
     reads_sorted: bool = False
     aligned_bases: int = 0        # sum of M/=/X lengths = sum of the weights table (the metric's unit)

@@ -95,6 +95,21 @@ inline int launch_tile(const kdl_batch& b, int32_t* counts, long long n_slots, l
     return KDL_OK;
 }
 
+// CTAs per unit of work (a tile of K1, a window of K1w) when there are fewer units than `per_sm` CTAs per SM would
+// fill, with at least ~256 reads per CTA; KDL_SPLIT overrides it
+int depth_split(long long units, int per_sm, long long reads) {
+    int split = 1;
+    const long long slots = (long long)sm_count() * per_sm;
+    if (units < slots) {
+        long long want = (slots + units - 1) / units;
+        const long long deep = reads / (units * 256);
+        if (want > deep) want = deep;
+        split = (int)(want < 1 ? 1 : (want > 32 ? 32 : want));
+    }
+    if (const char* ev = getenv("KDL_SPLIT")) { const int v = atoi(ev); if (v >= 1 && v <= 64) split = v; }
+    return split;
+}
+
 int validate_batch(const kdl_batch* b) {
     if (!b || b->n_reads < 0 || b->n_contigs < 0 || b->n_hard < 0 || b->n_complex < b->n_hard)
         return KDL_ERR_INVALID_ARG;
@@ -154,17 +169,7 @@ int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slot
     const long long tile_lo = slot_lo / KDL_TILE, n_tiles = (slot_hi - slot_lo) / KDL_TILE;
     // Depth split: a small reference piled deep has fewer tiles than the GPU has CTA slots (30 kb = 59 tiles for
     // 296 slots); `split` CTAs then share a tile by read range and flush with REDs into a zeroed table.
-    int split = 1;
-    if (tiled && n_tiles > 0) {
-        const long long slots = (long long)sm_count() * 2;
-        if (n_tiles < slots) {
-            long long want = (slots + n_tiles - 1) / n_tiles;
-            const long long deep = batch->n_reads / (n_tiles * 256);  // at least ~256 reads per unit
-            if (want > deep) want = deep;
-            split = (int)(want < 1 ? 1 : (want > 32 ? 32 : want));
-        }
-        if (const char* ev = getenv("KDL_SPLIT")) { const int v = atoi(ev); if (v >= 1 && v <= 64) split = v; }
-    }
+    const int split = tiled && n_tiles > 0 ? depth_split(n_tiles, 2, batch->n_reads) : 1;
     bool cx_by_atomics = (batch->n_complex - batch->n_hard) * 16 < batch->n_reads;
     if (const char* ev = getenv("KDL_CX")) cx_by_atomics = !strcmp(ev, "atomics") ? true : (!strcmp(ev, "pieces") ? false : cx_by_atomics);
     // zeroing that the chosen kernels will not do themselves: the tile kernel overwrites the weight columns of a
@@ -174,9 +179,9 @@ int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slot
     const int zero_to = ((flags & KDL_PILEUP_ZERO_REST) && !zero_in_k1) ? KDL_NCOL : 5;
     const bool zero_pass = zero_to > zero_from && slot_hi > slot_lo;
     // The dirty-sector map.  Complex reads this dense (>= 1 in 16; a few per cent of sectors stay clean at 1 in 100)
-    // dirty nearly every sector: instead of K1e / K1g marking op by op, the kernel that zeroes -- K1's flush, or the
-    // zeroing pass -- leaves every record of the range set, and the next pileup zeroes all of it.  Where neither runs,
-    // the writers mark.
+    // dirty nearly every sector: instead of K1w / K1e / K1g marking what they write, the kernel that zeroes -- K1's
+    // flush, or the zeroing pass -- leaves every record of the range set, and the next pileup zeroes all of it.  Where
+    // neither runs, the writers mark.
     const bool k1_stores = tiled && split == 1 && fresh && n_tiles > 0;
     const bool saturate = dirty_map && batch->n_complex > 0 && batch->n_complex * 16 >= batch->n_reads &&
                           (k1_stores || zero_pass);
@@ -197,7 +202,7 @@ int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slot
             if ((rc = check_launch()) != KDL_OK) return rc;
             // K1: the tile-owner kernel.  Tile-eligible complex reads go through its piece machinery (kCx) when
             // they are a sizeable share of the batch; when they are rare (< 1/16 of the reads) the lean instantiation
-            // runs and K1e counts their bases too, with REDs
+            // runs and K1w counts their bases too
             const bool cx = batch->n_complex > batch->n_hard && !cx_by_atomics;
             if (split > 1) {
                 rc = cx ? launch_tile<kdl::F_ATOMIC, true>(*batch, counts, n_slots, tile_lo, n_tiles, split, 0, nullptr, 0, st)
@@ -214,13 +219,19 @@ int kdl_pileup_range_map(const kdl_batch* batch, int32_t* counts, int64_t n_slot
             if (rc != KDL_OK) return rc;
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
-        if (batch->n_complex > batch->n_hard) {  // K1e: insertions / deletions / clips of the tile-eligible complex reads
-            if (cx_by_atomics)  // their bases too: 8 lanes per read
-                KDL_LAUNCH(kdl::pileup_events_kernel<8>, (unsigned)((batch->n_complex + 31) / 32), 256, 0, st,
-                           *batch, counts, n_slots, ins_events, 1, mark_map);
-            else                // a few scattered REDs per read: one thread per read
-                KDL_LAUNCH(kdl::pileup_events_kernel<1>, (unsigned)((batch->n_complex + 255) / 256), 256, 0, st,
-                           *batch, counts, n_slots, ins_events, 0, mark_map);
+        if (batch->n_complex > batch->n_hard && cx_by_atomics && n_tiles > 0) {
+            // K1w: everything of the rare tile-eligible complex reads the lean K1 left out, window by window (the
+            // windows' reads come from K0's index)
+            const long long n_win = (slot_hi - slot_lo + kdl::CW_SLOTS - 1) / kdl::CW_SLOTS;
+            const int wsplit = depth_split(n_win, 8, batch->n_complex - batch->n_hard);
+            KDL_LAUNCH(kdl::pileup_window_kernel, (unsigned)(n_win * wsplit), kdl::CW_THREADS,
+                       sizeof(int32_t) * kdl::CW_SMEM_COLS * kdl::CW_SLOTS, st, *batch, counts, n_slots, slot_lo,
+                       slot_hi, wsplit, ins_events, mark_map);
+            if ((rc = check_launch()) != KDL_OK) return rc;
+        } else if (batch->n_complex > batch->n_hard && !cx_by_atomics) {
+            // K1e: insertions / deletions / clips of the tile-eligible complex reads whose bases K1 counted as pieces
+            KDL_LAUNCH(kdl::pileup_events_kernel, (unsigned)((batch->n_complex + 255) / 256), 256, 0, st, *batch, counts,
+                       n_slots, ins_events, mark_map);
             if ((rc = check_launch()) != KDL_OK) return rc;
         }
         if (batch->n_hard > 0) {  // K1g: the reads that may wrap or raise, atomically, after the tile stores

@@ -21,7 +21,7 @@
 // entries and its overlap bases --, R2's N nibbles in place, and one row per dropped D or I op.  R1 is only read and
 // no read is both an R1 and an R2, so nothing races.  One thread per read: R1's coverage comes from walking both
 // CIGARs together (a simple R1 is one M op: a range test and a nibble read).
-// K10u: one thread per drop row, after K1q on the same stream, subtracts what K1e / K1g added for the dropped op
+// K10u: one thread per drop row, after K1q on the same stream, subtracts what K1w / K1e / K1g added for the dropped op
 // (they also marked its sectors in the dirty map already).
 #include "kdl_common.cuh"
 

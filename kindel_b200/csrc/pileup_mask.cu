@@ -1,7 +1,7 @@
 // pileup_mask.cu -- K1q: takes back what masked bases added to the base-count columns (extension).
 //
 // A base below min_base_quality is masked at decode: its nibble is N (15) in seq4, so every pileup kernel (K1's
-// bit-sliced count: A+C+G+T raw = coverage + 3N; K1e, K1g, K1s: nib2col(15) = 4) counts it as an N wherever the
+// bit-sliced count: A+C+G+T raw = coverage + 3N; K1w, K1e, K1g, K1s: nib2col(15) = 4) counts it as an N wherever the
 // reference's walk (kindel/kindel.py:40-81) would count that base, and the insertion strings read it as N.  The
 // masking rule is "read as N, then not counted": K1q runs after the pileup kernels in stream order and subtracts 1
 // at the (column, slot) each listed base went to:

@@ -138,7 +138,7 @@ static_assert(TileCfg<true>::kPcap >= KDL_TILE_MAXOPS && TileCfg<true>::kPcap < 
 // as zeros); F_ADD = add to what is there; F_ATOMIC = `split` CTAs share a tile, the table was zeroed, flush with REDs.
 // zero_rest (F_STORE): columns 5..18 hold an earlier pileup's sparse counts; the final flush of a window zeroes them --
 // all of them, or, given the dirty-sector map (kdl_common.cuh), only the sectors it marks.  map_after (F_STORE, with
-// the map): what the window's record holds after the flush -- 0 when K1e / K1g will mark what they write, all ones when
+// the map): what the window's record holds after the flush -- 0 when K1w / K1e / K1g will mark what they write, all ones when
 // they will not (complex reads so dense that nearly every sector is dirty anyway).  Without them (the defaults) no map is read
 // or written.
 template <int kFlush, bool kCx>
@@ -713,7 +713,7 @@ pileup_tile_kernel(kdl_batch b, int32_t* __restrict__ counts, long long n_slots,
             uint4 rec = make_uint4(~0u, ~0u, ~0u, ~0u);
             if (kFresh && zero_rest) {
                 // columns 5..18 of the window hold an earlier pileup's sparse counts: zero them here, under the
-                // counting, instead of in a pass of their own (K1e / K1g add to them after this kernel).  Lane
+                // counting, instead of in a pass of their own (K1w / K1e / K1g add to them after this kernel).  Lane
                 // lane & 7 owns sector lane & 7 of each column; quarter q takes columns 5 + q + 4 k, which are byte q
                 // of word k of the window's map record.
                 int32_t* z = counts + tile_slot + wlo + 8 * (lane & 7);

@@ -410,7 +410,7 @@ __device__ __forceinline__ void flush_window(Planes& acc, int (&rawacc)[8], cons
 
 // zero columns [col_lo, col_hi) of slots [slot_lo, slot_hi) (multiples of 4), 128-bit stores.  dirty_map (may be NULL):
 // map_fill = 0 (given only when the columns include all of 5..18) clears the records of the 64-slot windows wholly
-// inside the range; all ones sets the records of every window the range meets (K1e / K1g will not mark).
+// inside the range; all ones sets the records of every window the range meets (K1w / K1e / K1g will not mark).
 __global__ void __launch_bounds__(256)
 zero_cols_kernel(int32_t* __restrict__ counts, long long n_slots, int col_lo, int col_hi, long long slot_lo,
                  long long slot_hi, uint32_t* __restrict__ dirty_map = nullptr, uint32_t map_fill = 0u) {

@@ -3,7 +3,7 @@ bench.py builds it), bench.py's single-GPU step, then the qualities of its last 
 
     python tools/bench_fastq.py [--steps K] [--warmup W]      # one JSON line on stdout
 
-The timed step is bench.py's -- a fresh pileup into a reused CountTable (K0 + K1 + K1e) and the majority vote -- over
+The timed step is bench.py's -- a fresh pileup into a reused CountTable (K0 + K1 + K1w) and the majority vote -- over
 exactly K back-to-back steps with CUDA events.  On top of bench.py's fields the line carries:
   `qual_ms`      K2q (kdl_consensus_qual) against K2 (kdl_vote) over the last step's table and calls, alternating
                  for `rounds` rounds of `launches_per_timing` back-to-back launches;

@@ -3,7 +3,7 @@ the step's vote replaced by the IUPAC vote at threshold T (kdl_vote_iupac).
 
     python tools/bench_iupac.py [--threshold T] [--steps K] [--warmup W]      # one JSON line on stdout
 
-The timed step is bench.py's single-GPU step -- a fresh pileup into a reused CountTable (K0 + K1 + K1e) and the vote --
+The timed step is bench.py's single-GPU step -- a fresh pileup into a reused CountTable (K0 + K1 + K1w) and the vote --
 over exactly K back-to-back steps with CUDA events.  On top of bench.py's fields the line carries `iupac_threshold`,
 `mixed_sites` (call bytes with bit 7 set: multi-base IUPAC codes) and `vote_ms`: the majority vote (kdl_vote) and the
 IUPAC vote over the last step's table, `launches_per_timing` back-to-back launches per timing, the two alternating

@@ -4,7 +4,7 @@ min_base_quality = 20.
 
     python tools/bench_quality.py [--steps K] [--warmup W]          # one JSON line on stdout
 
-The timed step is bench.py's single-GPU step -- a fresh pileup into a reused CountTable (K0 + K1 + K1e + K1q) and the
+The timed step is bench.py's single-GPU step -- a fresh pileup into a reused CountTable (K0 + K1 + K1w + K1q) and the
 vote -- over exactly K back-to-back steps with CUDA events.  On top of bench.py's fields the line carries a `quality`
 block: the masked fraction, mask bytes per aligned base, K1q timed on its own (CUDA events, back-to-back launches into
 a scratch copy of the table) and K0+K1 without it.  `parity`: the sha256 of the timed loop's call bytes equals that of

@@ -4,12 +4,12 @@ configs[3] (`cfg4_5Mb_200x`, as bench.py builds it) and its all-simple twin.
     python tools/bench_sparse_zero.py [--out DIR] [--steps K] [--warmup W] [--rounds R]   # one JSON line on stdout
 
 Three measurements, each in a run of its own:
-  profile      per-kernel device time of bench.py's single-GPU step (K0, K1, K1e, K1g, K2) with torch.profiler (CUDA
+  profile      per-kernel device time of bench.py's single-GPU step (K0, K1, K1w, K1g, K2) with torch.profiler (CUDA
                activities), ms per step; the trace goes to DIR/sparse_zero_step.pt.trace.json.
   zero_stores  K0 + K1 of the all-simple batch into a reused table with columns 5..18 zeroed in full
                (kdl_pileup_range, KDL_PILEUP_ZERO_REST, no map) against not zeroed at all: what the stores of a full
-               zeroing cost K1, without K1e.
-  map_ab       the cfg4 pileup (K0 + K1 + K1e) into one reused table, full zeroing (kdl_pileup_range) against the
+               zeroing cost K1, without K1w.
+  map_ab       the cfg4 pileup (K0 + K1 + K1w) into one reused table, full zeroing (kdl_pileup_range) against the
                map's (kdl_pileup_range_map), alternating rounds of K back-to-back pileups, min / median / max ms per
                pileup; `bytes_zeroed_per_step` from the map's popcount (32 bytes per set bit) against the full 56 bytes
                per slot.
@@ -35,8 +35,9 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402  (the workload generator, step timer and clock sampler of the main bench)
 
 WORKLOAD = "cfg4_5Mb_200x"
-KERNELS = (("tile_index_kernel", "K0"), ("pileup_tile_kernel", "K1"), ("pileup_events_kernel", "K1e"),
-           ("pileup_general_kernel", "K1g"), ("zero_cols_kernel", "zero"), ("vote_kernel", "K2"))
+KERNELS = (("tile_index_kernel", "K0"), ("pileup_tile_kernel", "K1"), ("pileup_window_kernel", "K1w"),
+           ("pileup_events_kernel", "K1e"), ("pileup_general_kernel", "K1g"), ("zero_cols_kernel", "zero"),
+           ("vote_kernel", "K2"))
 
 
 def stats(v):
@@ -161,7 +162,7 @@ def main(argv=None) -> int:
     line["parity_after_ab"] = bool(np.array_equal(table.t.cpu().numpy(), want))
     del db, table, want
 
-    # ---- the stores of a full zeroing on the all-simple batch (no K1e)
+    # ---- the stores of a full zeroing on the all-simple batch (no K1w)
     simple, _, _ = bench.make_workload("cfg4_5Mb_200x_simple")
     sdb = engine.upload(simple, dev)
     st = engine.CountTable(simple.n_slots, dev)

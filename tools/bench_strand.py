@@ -6,7 +6,7 @@ single-GPU step, then K8 and the reverse pileup over its batch.
 
 The timed step is bench.py's.  On top of bench.py's fields the line carries:
   `strand_ms`   K8 alone (kdl_select_count + kdl_select_scatter with the outputs allocated once), the reverse pileup
-                alone (K0 + K1 + K1e + K1g of the K8 sub-batch into a reused table) and K2 for scale, over the step's
+                alone (K0 + K1 + K1w + K1g of the K8 sub-batch into a reused table) and K2 for scale, over the step's
                 batch and table, in 7 alternating rounds of 20 launches;
   `e2e_vcf`     variants_vcf(path, strand=True) against variants_vcf(path) on a 10^6-read BAM with seeded strands,
                 best of 3, alternating;

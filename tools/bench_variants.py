@@ -4,7 +4,7 @@ table.
 
     python tools/bench_variants.py [--steps K] [--warmup W]      # one JSON line on stdout
 
-The timed step is bench.py's -- a fresh pileup into a reused CountTable (K0 + K1 + K1e) and the majority vote -- over
+The timed step is bench.py's -- a fresh pileup into a reused CountTable (K0 + K1 + K1w) and the majority vote -- over
 exactly K back-to-back steps with CUDA events.  On top of bench.py's fields the line carries:
   `variant_ms`   K6's three launches (kdl_variant_count + kdl_variant_scatter) against K2 (kdl_vote) over the last
                  step's table, alternating for `rounds` rounds of `launches_per_timing` back-to-back launches, at
