@@ -539,6 +539,63 @@ int kdl_normalise(const int32_t* label, const uint8_t* reverse, int64_t n_reads,
                   int32_t* scratch, int64_t scratch_words, uint8_t* keep, int32_t* total, int64_t* dropped,
                   void* stream);
 
+/* K14 (extension: `--dedup`): duplicate reads and read pairs removed before the pileup, as samtools markdup -r and
+ * Picard MarkDuplicates remove them.  Over the batch's reads (after min_mapq / exclude_flags; a 0x400 in the file is
+ * ignored):
+ *   Left alone: dup_score[r] < 0 (the decode gives -1 where FLAG & 0x900), or no M/D/N/=/X op.  Never removed, never
+ *   anyone's duplicate.
+ *   End: (contig, u, strand), strand = reverse[r] (FLAG & 0x10), u the unclipped 5' position in SAM arithmetic:
+ *   forward u = POS0 - the S and H ops before the first M/D/N/=/X op; reverse u = POS0 + the M/D/N/=/X lengths - 1 +
+ *   the S and H ops after the last one.  Encoded e = 2 u + strand (int64), so (u, strand) order is e order.
+ *   Score: dup_score[r], the sum of the read's Phred qualities >= 15 over all of SEQ (0 without qualities).
+ *   Pair: an R2 (mate[r] >= 0, K10p's) and its R1, neither left alone.  Single: any other read not left alone (a
+ *   pair's mate whose partner is left alone included).
+ *   Pairs: key (contig, E1, E2), E1 <= E2 the mates' ends; of each key the pair with the largest score R1 + R2 (int64)
+ *   stays, ties to the smallest min(R1, R2); the others are removed, both mates.
+ *   Singles: removed when a pair (kept or removed) has a mate end equal to theirs; otherwise of each end the single
+ *   with the largest score stays, ties to the smallest index.
+ * keep[r] = 0 for a removed read, else 1.
+ *   kdl_dedup_entries  K14k (three launches, one thread per read): keep = 1, end[], paired[], then the two entry
+ *                      lists, compacted in any order.  Pair list: pair_contig / pair_e1 (E1) / pair_e2 (E2) /
+ *                      pair_rank / pair_r1 / pair_r2, capacity n_reads / 2.  Single list: single_contig, single_key =
+ *                      2 e + 0 for a pair mate's end (two markers per pair) or 2 e + 1 for a single's, single_rank,
+ *                      single_read (-1 for a marker), capacity n_reads.  rank = (0xffffffff - score) << 32 | index
+ *                      (pair: the summed score, the smaller mate index): the best entry has the smallest rank.  end
+ *                      int64 [n_reads] and paired uint8 [n_reads] are scratch.  mate may be NULL (no pairs).  Zeroes
+ *                      the totals record (KDL_DEDUP_TOTALS int64) and writes [0] pair entries, [1] single-list
+ *                      entries: one read-back sizes the sort.
+ *   kdl_dedup_select   K14s (four launches per list, one thread per sorted entry, no thread walking a run): over the
+ *                      lists sorted by key -- pair_order[n_pairs] by (contig, E1, E2), single_order[n_singles] by
+ *                      (contig, single_key), the entry indices in key order -- each run's best candidate stays and
+ *                      the others get keep 0.  Adds [2] pairs removed, [3] singles removed, [4] of those singles the
+ *                      ones a pair end shadowed.  scratch: int32 [kdl_dedup_scratch_words(max(n_pairs, n_singles))],
+ *                      8-byte aligned.  On the stream after kdl_dedup_entries.
+ * Device pointers. */
+#define KDL_DEDUP_TOTALS 8
+#define KDL_DEDUP_ALONE ((int64_t)(-0x7fffffffffffffffll - 1))  /* end[r] of a read left alone */
+
+typedef struct kdl_dedup_lists {
+    int32_t* pair_contig;
+    int64_t* pair_e1;
+    int64_t* pair_e2;
+    uint64_t* pair_rank;
+    int32_t* pair_r1;
+    int32_t* pair_r2;
+    int32_t* single_contig;
+    int64_t* single_key;
+    uint64_t* single_rank;
+    int32_t* single_read;
+    int64_t* end;     /* [n_reads] scratch */
+    uint8_t* paired;  /* [n_reads] scratch */
+} kdl_dedup_lists;
+
+int kdl_dedup_entries(const kdl_batch* batch, const uint8_t* reverse, const int32_t* dup_score, const int32_t* mate,
+                      const kdl_dedup_lists* lists, uint8_t* keep, int64_t* totals, void* stream);
+int64_t kdl_dedup_scratch_words(int64_t n_entries);
+int kdl_dedup_select(const kdl_dedup_lists* lists, const int64_t* pair_order, int64_t n_pairs,
+                     const int64_t* single_order, int64_t n_singles, int32_t* scratch, int64_t scratch_words,
+                     uint8_t* keep, int64_t* totals, void* stream);
+
 /* Fused cross-GPU count reduction + vote (SURVEY.md 8e): sums the 7 vote columns of `n_peers`
  * tables that live on this and on peer GPUs (peer pointers mapped with CUDA IPC / P2P), votes on
  * slots [slot_lo, slot_hi) and writes calls for that range; optionally stores the reduced
@@ -649,7 +706,10 @@ int kdl_ctx_last_timing(kdl_ctx* ctx, float* h2d_ms, float* kernel_ms, float* d2
  *   kdl_bam_fill_mates  after fill (extension): name_hash / mate_start / pair_role [n_kept] of K10, in read order
  *   kdl_bam_fill_qual   after fill (extension): qual8 [8 * words of seq4], the Phred quality of base k of read r at byte
  *                    8 * seq_off[r] + k, 0xff for a complex read's trailer words and the padding.  prepare's info[15] =
- *                    kept reads without qualities (BAM 0xff, SAM `*`): their bytes are 0xff too */
+ *                    kept reads without qualities (BAM 0xff, SAM `*`): their bytes are 0xff too
+ *   kdl_bam_fill_dup    after fill (extension, K14): dup_score [n_kept] int32 in read order, -1 where FLAG & 0x900, else
+ *                    the sum of the read's Phred qualities >= 15 over all of SEQ (0 without qualities), saturating at
+ *                    2^31 - 1 */
 typedef struct kdl_bam kdl_bam;
 int kdl_bam_open(const char* path, int threads, kdl_bam** out);
 void kdl_bam_close(kdl_bam* h);
@@ -667,6 +727,7 @@ int kdl_bam_fill_mask(kdl_bam* h, int threads, uint32_t* read_idx, uint32_t* off
 int kdl_bam_fill_strand(kdl_bam* h, int threads, uint8_t* reverse);
 int kdl_bam_fill_mates(kdl_bam* h, int threads, uint64_t* name_hash, int32_t* mate_start, uint8_t* pair_role);
 int kdl_bam_fill_qual(kdl_bam* h, int threads, uint8_t* qual8);
+int kdl_bam_fill_dup(kdl_bam* h, int threads, int32_t* dup_score);
 
 #ifdef __cplusplus
 }

@@ -32,6 +32,7 @@ KDL_FAST_MAXLEN = 8192
 KDL_OK = 0
 KDL_ERR_INDEX = 10
 KDL_ERR_KEY = 11
+KDL_DEDUP_TOTALS = 8
 
 
 class KdlBatch(C.Structure):
@@ -96,6 +97,12 @@ class KdlAmplicons(C.Structure):
         ("insert_start", C.c_void_p),
         ("insert_end", C.c_void_p),
     ]
+
+
+class KdlDedupLists(C.Structure):
+    _fields_ = [(f, C.c_void_p) for f in ("pair_contig", "pair_e1", "pair_e2", "pair_rank", "pair_r1", "pair_r2",
+                                          "single_contig", "single_key", "single_rank", "single_read", "end",
+                                          "paired")]
 
 
 class KdlExchange(C.Structure):
@@ -190,6 +197,11 @@ _PROTOTYPES = {
     "kdl_normalise_scratch_words": (C.c_int64, [C.c_int64, C.c_int32]),
     "kdl_normalise": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_dedup_entries": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.POINTER(KdlDedupLists), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kdl_dedup_scratch_words": (C.c_int64, [C.c_int64]),
+    "kdl_dedup_select": (C.c_int, [C.POINTER(KdlDedupLists), C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                   C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers":(C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_vote_peers_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,
@@ -226,6 +238,7 @@ _PROTOTYPES = {
     "kdl_bam_fill_strand": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "kdl_bam_fill_mates": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_bam_fill_qual": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "kdl_bam_fill_dup": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -31,6 +31,9 @@ With `strand=True` the batch also keeps each kept read's strand (`reverse`, FLAG
 reads by (`name_hash`, `mate_start`, `pair_role`: include/kindel_b200.h K10 has the rule); nothing is decoded when off.
 With `qual=True` it keeps every base's quality beside its bases (`qual8`, which K11 sums for `variants --vcf --qual`);
 a kept read without qualities is then a ValueError naming the file: nothing is guessed.
+With `dup=True` it keeps each kept read's duplicate score (`dup_score`, what `--dedup` ranks duplicates by,
+include/kindel_b200.h K14): -1 where FLAG has 0x100 or 0x800, else the sum of its Phred qualities >= 15 over all of SEQ
+(0 without qualities), saturating at 2^31 - 1.  It is summed while QUAL is read, so no quality byte is kept for it.
 
 The result is a `ReadBatch` (numpy arrays in host memory) described in include/kindel_b200.h.
 """
@@ -99,6 +102,9 @@ class ReadBatch:
     # base qualities (extension; `qual=True` at decode, K11): base k of read r at byte 8 * seq_off[r] + k, 0xff for the
     # padding and a complex read's trailer words.  None = not asked for; select_reads carries it, the shards leave it behind.
     qual8: np.ndarray = field(default=None)         # uint8 [8 * words of seq4]
+    # duplicate score (extension; `dup=True` at decode, K14): -1 for FLAG & 0x900, else the summed Phred >= 15.  None =
+    # not asked for.
+    dup_score: np.ndarray = field(default=None)     # int32 [n]
 
     @property
     def mates(self):
@@ -244,7 +250,8 @@ def mask_bases(seq4: np.ndarray, seq_off: np.ndarray, counts: np.ndarray, qpos: 
 
 
 def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_seq, cig_off, cigar, seq4,
-             n_records=0, exotic=None, qual=None, min_base_quality=0, mask=None, reverse=None, mates=None) -> ReadBatch:
+             n_records=0, exotic=None, qual=None, min_base_quality=0, mask=None, reverse=None, mates=None,
+             dup_score=None) -> ReadBatch:
     """Classify reads (simple / tile-eligible complex / hard), lay the complex reads' CIGARs behind their bases,
     detect coordinate order.  All vectorised numpy; shared by the BAM, SAM and synthetic paths.
 
@@ -254,7 +261,7 @@ def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_se
     threshold are masked (N in seq4, listed in the mask) BEFORE classification.  mask = (per-read counts, query
     offsets): a mask already applied to `seq4` (re-finalizing a masked batch), carried into the result.
     reverse: the reads' strand bytes (1 = FLAG & 0x10), carried into the result.  mates: (name_hash, mate_start,
-    pair_role) of the reads, carried into the result."""
+    pair_role) of the reads, carried into the result.  dup_score: the reads' duplicate scores, carried into the result."""
     contig_len = np.ascontiguousarray(contig_len, dtype=np.int32)
     contig_read_off = np.ascontiguousarray(contig_read_off, dtype=np.int64)
     ref_start = np.ascontiguousarray(ref_start, dtype=np.int32)
@@ -367,6 +374,7 @@ def finalize(contig_names, contig_len, contig_read_off, ref_start, seq_off, l_se
         n_records=int(n_records), max_simple_len=int(oplen[simple].max()) if simple.any() else 0,
         reach_right=reach_right, reach_left=reach_left, mask_read=mask_read, mask_off=mask_off, mask_qpos=mask_qpos,
         reverse=None if reverse is None else np.ascontiguousarray(reverse, dtype=np.uint8),
+        dup_score=None if dup_score is None else np.ascontiguousarray(dup_score, dtype=np.int32),
         **_mate_fields(mates),
     )
 
@@ -420,7 +428,7 @@ def with_mask(batch: ReadBatch, counts: np.ndarray, qpos: np.ndarray) -> ReadBat
     seq4 = mask_bases(batch.seq4, batch.seq_off, counts, qpos)
     return finalize(batch.contig_names, batch.contig_len, batch.contig_read_off, batch.ref_start, batch.seq_off,
                     batch.seq_len, batch.cig_off, batch.cigar, seq4, n_records=batch.n_records, mask=(counts, qpos),
-                    reverse=batch.reverse, mates=batch.mates)
+                    reverse=batch.reverse, mates=batch.mates, dup_score=batch.dup_score)
 
 
 def select_reads(batch: ReadBatch, idx) -> ReadBatch:
@@ -444,7 +452,8 @@ def select_reads(batch: ReadBatch, idx) -> ReadBatch:
         np.arange(int(seq_off[-1])) - np.repeat(seq_off[:-1], words))
     out = finalize(batch.contig_names, batch.contig_len, read_off, batch.ref_start[idx], seq_off[:-1], lseq,
                    cig_off, batch.cigar[cig_src], batch.seq4[seq_src], n_records=n, mask=_mask_of(batch, idx),
-                   reverse=None if batch.reverse is None else batch.reverse[idx], mates=_mates_at(batch, idx))
+                   reverse=None if batch.reverse is None else batch.reverse[idx], mates=_mates_at(batch, idx),
+                   dup_score=None if batch.dup_score is None else batch.dup_score[idx])
     if batch.qual8 is not None:  # each kept read's qualities, laid out by its new seq_off
         out.qual8 = qual_layout(out, _ragged_gather(batch.qual8, 8 * batch.seq_off.astype(np.int64)[idx], lseq))
     return out
@@ -493,9 +502,12 @@ def merge_batches(batches) -> ReadBatch:
     mates = None
     if all(b.mates is not None for b in batches):
         mates = tuple(np.concatenate([b.mates[k] for b in batches])[order] for k in range(3))
+    dup_score = None
+    if all(b.dup_score is not None for b in batches):
+        dup_score = np.concatenate([b.dup_score for b in batches])[order]
     return finalize(first.contig_names, first.contig_len, read_off, ref_start[order], base_at[order], lseq[order],
                     cig_off, _ragged_gather(cigar, cig_at[order], nco), bases, n_records=int(order.shape[0]), mask=mask,
-                    reverse=reverse, mates=mates)
+                    reverse=reverse, mates=mates, dup_score=dup_score)
 
 
 _SAVE_FIELDS = ("contig_len", "contig_read_off", "contig_slot", "ref_start", "seq_off", "l_seq", "seq_len", "cig_off",
@@ -505,6 +517,7 @@ _SAVE_SCALARS = ("n_slots", "n_events", "reads_sorted", "aligned_bases", "n_reco
 _MASK_FIELDS = ("mask_read", "mask_off", "mask_qpos")  # saved only when the batch has masked bases
 _STRAND_FIELDS = ("reverse",)  # saved only when the batch has its strands
 _MATE_FIELDS = ("name_hash", "mate_start", "pair_role")  # saved only when the batch has its mates
+_DUP_FIELDS = ("dup_score",)  # saved only when the batch has its duplicate scores
 
 
 def save_batch(directory: str, batch: ReadBatch) -> None:
@@ -512,11 +525,12 @@ def save_batch(directory: str, batch: ReadBatch) -> None:
     import json
 
     os.makedirs(directory, exist_ok=True)
-    for f in _MASK_FIELDS + _STRAND_FIELDS + _MATE_FIELDS:
+    for f in _MASK_FIELDS + _STRAND_FIELDS + _MATE_FIELDS + _DUP_FIELDS:
         if os.path.exists(os.path.join(directory, f + ".npy")):
             os.remove(os.path.join(directory, f + ".npy"))
     for f in (_SAVE_FIELDS + (_MASK_FIELDS if batch.n_masked else ())
-              + (_STRAND_FIELDS if batch.reverse is not None else ()) + (_MATE_FIELDS if batch.mates is not None else ())):
+              + (_STRAND_FIELDS if batch.reverse is not None else ()) + (_MATE_FIELDS if batch.mates is not None else ())
+              + (_DUP_FIELDS if batch.dup_score is not None else ())):
         np.save(os.path.join(directory, f + ".npy"), np.ascontiguousarray(getattr(batch, f)))
     meta = {k: (bool(getattr(batch, k)) if k == "reads_sorted" else int(getattr(batch, k))) for k in _SAVE_SCALARS}
     meta["contig_names"] = list(batch.contig_names)
@@ -530,7 +544,7 @@ def load_batch(directory: str, mmap: bool = True) -> ReadBatch:
     with open(os.path.join(directory, "batch.json")) as fh:
         meta = json.load(fh)
     arrays = {f: np.load(os.path.join(directory, f + ".npy"), mmap_mode="r" if mmap else None) for f in _SAVE_FIELDS}
-    for f in _MASK_FIELDS + _STRAND_FIELDS + _MATE_FIELDS:
+    for f in _MASK_FIELDS + _STRAND_FIELDS + _MATE_FIELDS + _DUP_FIELDS:
         if os.path.exists(os.path.join(directory, f + ".npy")):
             arrays[f] = np.load(os.path.join(directory, f + ".npy"), mmap_mode="r" if mmap else None)
     return ReadBatch(contig_names=meta.pop("contig_names"), **arrays, **meta)
@@ -618,14 +632,16 @@ def decode_threads() -> int:
 
 
 def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0, exclude_flags: int = 0,
-             min_base_quality: int = 0, strand: bool = False, mates: bool = False, qual: bool = False) -> ReadBatch:
+             min_base_quality: int = 0, strand: bool = False, mates: bool = False, qual: bool = False,
+             dup: bool = False) -> ReadBatch:
     """.bam -> ReadBatch through the C++ decoder (bam_host.cpp): BGZF inflate, filter, classification and the
     device layout (inline CIGAR blocks included) in threads, no Python per-record or per-array work.
     pinned=True puts the arrays the device consumes into page-locked memory (needs torch + CUDA).
     min_mapq / exclude_flags / min_base_quality: the filters of this module's docstring (extension).  strand=True
     (extension): also the kept reads' strands, `reverse` (kdl_bam_fill_strand).  mates=True (extension): also
     `name_hash`, `mate_start` and `pair_role` (kdl_bam_fill_mates).  qual=True (extension): also `qual8`, the
-    qualities beside the bases (kdl_bam_fill_qual); a kept read without qualities is a ValueError."""
+    qualities beside the bases (kdl_bam_fill_qual); a kept read without qualities is a ValueError.  dup=True
+    (extension): also `dup_score` (kdl_bam_fill_dup)."""
     import ctypes as C
 
     filters = check_filters(min_mapq, exclude_flags, min_base_quality)
@@ -701,6 +717,10 @@ def read_bam(path, threads: int = None, pinned: bool = False, min_mapq: int = 0,
                 raise ValueError(missing_qualities(path, int(info[15])))
             mask["qual8"] = np.empty(8 * n_words, dtype=np.uint8)
             _ffi.check(lib.kdl_bam_fill_qual(h, threads, mask["qual8"].ctypes.data if n else None), "kdl_bam_fill_qual")
+        if dup:
+            mask["dup_score"] = np.zeros(n, dtype=np.int32)
+            if lib.kdl_bam_fill_dup(h, threads, mask["dup_score"].ctypes.data if n else None) != 0:
+                raise ValueError("%s: QUAL fields the C++ text parser does not take" % path)
     finally:
         lib.kdl_bam_close(h)
     return ReadBatch(
@@ -787,8 +807,22 @@ def _sam_qual(text: str, seq: str) -> bytes:
     return bytes(c - 33 for c in raw)
 
 
+_DUP_CAP = (1 << 31) - 1
+
+
+def dup_score(flag: int, qual_text: str, seq: str) -> int:
+    """The duplicate score of a SAM record (K14): -1 for FLAG & 0x900, else the sum of its Phred qualities >= 15 over
+    all of SEQ (0 for QUAL `*`), saturating at 2^31 - 1; ValueError for a malformed QUAL."""
+    if flag & 0x900:
+        return -1
+    q = np.frombuffer(_sam_qual(qual_text, seq), dtype=np.uint8)
+    if qual_text == "*":
+        return 0
+    return int(min(int(q[q >= 15].sum(dtype=np.int64)), _DUP_CAP))
+
+
 def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0,
-             strand: bool = False, mates: bool = False, qual: bool = False) -> ReadBatch:
+             strand: bool = False, mates: bool = False, qual: bool = False, dup: bool = False) -> ReadBatch:
     min_mapq, exclude_flags, min_base_quality = check_filters(min_mapq, exclude_flags, min_base_quality)
     header = []
     groups = {}  # rname -> list of (pos0, cigar words, seq, qualities, reverse, (name hash, PNEXT - 1, role))
@@ -828,7 +862,8 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
                     pnext = -1
                 mate = (name_hash(f[0]), pnext - 1 if 0 <= pnext < (1 << 31) else -1,
                         pair_role(flag, f[6] == "=" or f[6] == rname))
-            g.append((int(f[3]) - 1, parse_cigar_text(f[5]), seq, qv, 1 if flag & 0x10 else 0, mate))
+            g.append((int(f[3]) - 1, parse_cigar_text(f[5]), seq, qv, 1 if flag & 0x10 else 0, mate,
+                      dup_score(flag, f[10], seq) if dup else None))
     groups.pop("*", None)  # kindel.py:147-148
     names, lens = _sq_from_text("\n".join(header))
     sq = dict(zip(names, lens))
@@ -836,11 +871,12 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
     for nm in contig_names:
         if nm not in sq:
             raise KeyError(nm)  # refs_lens[ref_id], kindel.py:151
-    ref_start, l_seq, cig_off, cigar, seq_off, seq_parts, quals, rev, mate_rows = [], [], [0], [], [], [], [], [], []
+    ref_start, l_seq, cig_off, cigar, seq_off, seq_parts, quals, rev, mate_rows, scores = ([], [], [0], [], [], [], [],
+                                                                                          [], [], [])
     read_off = [0]
     words = 0
     for nm in contig_names:
-        for pos0, cig, seq, qual, is_rev, mate in groups[nm]:
+        for pos0, cig, seq, qual, is_rev, mate, score in groups[nm]:
             ref_start.append(pos0)
             l_seq.append(len(seq))
             cigar.extend(cig)
@@ -852,6 +888,7 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
             quals.append(qual)
             rev.append(is_rev)
             mate_rows.append(mate)
+            scores.append(score)
         read_off.append(len(ref_start))
     seq4 = np.concatenate(seq_parts) if seq_parts else np.zeros(0, dtype=np.uint32)
     if n_noqual:
@@ -864,14 +901,15 @@ def read_sam(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: 
                      n_records=n_records, qual=quals, min_base_quality=min_base_quality,
                      reverse=np.array(rev, dtype=np.uint8) if strand else None,
                      mates=tuple(np.array([m[k] for m in mate_rows], dtype=dt) for k, dt in
-                                 enumerate((np.uint64, np.int64, np.uint8))) if mates else None)
+                                 enumerate((np.uint64, np.int64, np.uint8))) if mates else None,
+                     dup_score=np.array(scores, dtype=np.int32) if dup else None)
     if qual:
         batch.qual8 = qual_layout(batch, quals)
     return batch
 
 
 def read_alignment(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_quality: int = 0,
-                   strand: bool = False, mates: bool = False, qual: bool = False) -> ReadBatch:
+                   strand: bool = False, mates: bool = False, qual: bool = False, dup: bool = False) -> ReadBatch:
     """.bam or .sam (by content, not by suffix) -> ReadBatch.  The filters, strand, mates and qualities (extensions):
     see the module docstring."""
     path = os.fspath(path)
@@ -881,6 +919,8 @@ def read_alignment(path, min_mapq: int = 0, exclude_flags: int = 0, min_base_qua
         filters["mates"] = True
     if qual:
         filters["qual"] = True
+    if dup:
+        filters["dup"] = True
     with open(path, "rb") as fh:
         magic = fh.read(4)
     if magic[:2] == b"\x1f\x8b" or magic == b"BAM\x01":

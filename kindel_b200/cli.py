@@ -9,7 +9,7 @@ extension one FASTQ record per contig instead),
 `--strand` / `--max-sor`, with a base-quality QUAL with `--qual` / `--min-qual`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
 bases of every read before the pileup (kindel_b200/primers.py); `--mask-overlaps` counts each read pair once where
 its mates overlap (include/kindel_b200.h K10); `--normalise N` with a named scheme keeps at most N reads of each
-amplicon and strand (K12 + K13, include/kindel_b200.h).  `amplicons --primers scheme.bed` (an extension) writes a TSV row per
+amplicon and strand (K12 + K13, include/kindel_b200.h); `--dedup` removes duplicate reads and read pairs (K14).  `amplicons --primers scheme.bed` (an extension) writes a TSV row per
 sample and amplicon of a tiled scheme: its reads (K12) and the depth of its insert (K12d).
 argh derived the flags from the function signatures (first letter as short option unless two
 parameters share it); argparse spells the same set out.  Note the CLI default `--min-overlap 7`
@@ -79,13 +79,15 @@ def amplicons(bam_paths, primers, min_depth=20, gpus=None, **filters):
 
     df = kindel.amplicons(bam_paths, primers, min_depth, devices=gpus, **filters)
     capped = df.attrs.get("dropped", {})  # (--normalise)
+    duplicates = df.attrs.get("duplicates", {})  # (--dedup)
     for name, (kept, assigned, unprimed, mispaired, ambiguous) in df.attrs["reads"].items():
         rows = df[df["sample"] == name]
         drop = rows.loc[rows["status"] == "dropout", "amplicon"].tolist()
-        print("%s: %d reads kept: %d assigned, %d unprimed, %d mispaired, %d ambiguous; %d amplicons, %d dropouts%s%s"
+        print("%s: %d reads kept: %d assigned, %d unprimed, %d mispaired, %d ambiguous; %d amplicons, %d dropouts%s%s%s"
               % (name, kept, assigned, unprimed, mispaired, ambiguous, len(rows), len(drop),
                  (": " + ", ".join(drop)) if drop else "",
-                 "; %d reads over the normalise cap dropped" % capped[name] if name in capped else ""),
+                 "; %d reads over the normalise cap dropped" % capped[name] if name in capped else "",
+                 "; %d duplicate reads removed" % duplicates[name] if name in duplicates else ""),
               file=sys.stderr)
     out = ["\t".join(kindel.AMPLICON_COLUMNS)]
     for r in df.itertuples(index=False):
@@ -136,6 +138,10 @@ def _add_filters(p):
     p.add_argument("--normalise", type=_normalise, default=None, metavar="N",
                    help="keep only the first N reads (file order) of each amplicon and strand of the --primers "
                         "scheme, whose 4th column names each primer <amplicon>_LEFT or <amplicon>_RIGHT")
+    # extension: duplicate removal, off by default
+    p.add_argument("--dedup", action="store_true",
+                   help="remove duplicate reads and read pairs (same unclipped 5' ends and strands) before the "
+                        "pileup, keeping the one with the highest sum of base qualities >= 15, as samtools markdup -r")
 
 
 def _normalise(text: str) -> int:
@@ -170,6 +176,8 @@ def _filters(a) -> dict:
         out["mask_overlaps"] = True
     if a.normalise is not None:
         out["normalise"] = a.normalise
+    if a.dedup:
+        out["dedup"] = True
     return out
 
 

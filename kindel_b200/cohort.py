@@ -86,13 +86,15 @@ class Cohort:
     """The samples piled one by one into the stacked table T over the shared layout, with what the records need of
     each: its deletion groups (device) and its insertion events (host), both in shared slots."""
 
-    def __init__(self, paths, devices=None, filters=(0, 0, 0), primers=None, mask_overlaps=False, normalise=None):
-        from .kindel import _normalise_scheme, check_normalise, pileup_run
+    def __init__(self, paths, devices=None, filters=(0, 0, 0), primers=None, mask_overlaps=False, normalise=None,
+                 dedup=False):
+        from .kindel import _normalise_scheme, check_dedup, check_normalise, pileup_run
 
         import torch
 
         self.layout = Layout()
         self.normalise = check_normalise(normalise)
+        self.dedup = check_dedup(dedup)
         self.primers, self.scheme = _normalise_scheme(primers, self.normalise)  # (the scheme: normalise's, loaded once)
         self.mask_overlaps = bool(mask_overlaps)
         self.table = None
@@ -103,7 +105,7 @@ class Cohort:
         for i, path in enumerate(paths):
             run = pileup_run(path, devices, 1, mbq, mapq, flags,
                              primers=self.primers if self.scheme is None else self.scheme,
-                             mask_overlaps=self.mask_overlaps, normalise=self.normalise)[0]
+                             mask_overlaps=self.mask_overlaps, normalise=self.normalise, dedup=self.dedup)[0]
             counts, dbatch = run.device_tables()
             batch = run.batch
             shared = self.layout.add(batch, path)
@@ -174,14 +176,14 @@ class Cohort:
 # ---------------------------------------------------------------------------------------------------- text
 def variants_vcf(paths, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
                  exclude_flags=0, reference=None, primers=None, mask_overlaps=False, samples=None,
-                 normalise=None) -> str:
+                 normalise=None, dedup=False) -> str:
     """The multi-sample VCF of kindel.variants_vcf given a list of paths (see there for the rules)."""
     paths = [os.fspath(p) for p in paths]
     if not paths:
         raise ValueError("variants_vcf needs at least one alignment file")
     names = sample_names(paths, samples)
     filters = (min_base_quality, min_mapq, exclude_flags)
-    cohort = Cohort(paths, devices, filters, primers, mask_overlaps, normalise)
+    cohort = Cohort(paths, devices, filters, primers, mask_overlaps, normalise, dedup)
     lay = cohort.layout
     ref = None
     if reference is not None:
@@ -190,7 +192,7 @@ def variants_vcf(paths, abs_threshold=1, rel_threshold=0.01, devices=None, min_b
         ref = reference if isinstance(reference, Reference) else load_reference(reference, lay)
     lines = vcf.header(lay.contig_names, lay.contig_len, abs_threshold, rel_threshold, filters, cohort.primers,
                        cohort.mask_overlaps, reference_name=None if ref is None else ref.name, samples=names,
-                       normalise=cohort.normalise)
+                       normalise=cohort.normalise, dedup=cohort.dedup)
     return "\n".join(lines + records(cohort, None if ref is None else ref.codes, abs_threshold, rel_threshold)) + "\n"
 
 

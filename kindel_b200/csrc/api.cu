@@ -19,6 +19,7 @@
 #include "quality.cu"
 #include "amplicons.cu"
 #include "normalise.cu"
+#include "dedup.cu"
 
 namespace {
 
@@ -866,6 +867,79 @@ int kdl_normalise(const int32_t* label, const uint8_t* reverse, int64_t n_reads,
     KDL_LAUNCH(kdl::normalise_mark_kernel, (unsigned)grid, kdl::NM_THREADS, 0, st, label, reverse, n_reads, n_amplicons,
                per, cap, scratch, keep);
     return check_launch();
+}
+
+// K14's grids: one thread per read (K14k) or per sorted entry (K14s), at least one CTA
+static long long dedup_ctas(long long items) { return items > 0 ? (items + kdl::DD_THREADS - 1) / kdl::DD_THREADS : 1; }
+
+static bool dedup_lists_ok(const kdl_dedup_lists* l) {
+    return l && l->pair_contig && l->pair_e1 && l->pair_e2 && l->pair_rank && l->pair_r1 && l->pair_r2 &&
+           l->single_contig && l->single_key && l->single_rank && l->single_read && l->end && l->paired;
+}
+
+int kdl_dedup_entries(const kdl_batch* batch, const uint8_t* reverse, const int32_t* dup_score, const int32_t* mate,
+                      const kdl_dedup_lists* lists, uint8_t* keep, int64_t* totals, void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (!totals || (batch->n_reads > 0 && (!reverse || !dup_score || !keep || !dedup_lists_ok(lists))))
+        return KDL_ERR_INVALID_ARG;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const unsigned grid = (unsigned)dedup_ctas(batch->n_reads);
+    unsigned long long* tot = reinterpret_cast<unsigned long long*>(totals);
+    kdl_dedup_lists l = {};
+    if (lists) l = *lists;
+    KDL_LAUNCH(kdl::dedup_ends_kernel, grid, kdl::DD_THREADS, 0, st, *batch, reverse, dup_score, l.end, l.paired, keep,
+               tot);
+    if ((rc = check_launch()) != KDL_OK || batch->n_reads == 0) return rc;
+    if (mate) {
+        KDL_LAUNCH(kdl::dedup_pairs_kernel, grid, kdl::DD_THREADS, 0, st, *batch, dup_score, mate, l, l.end, l.paired,
+                   tot);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+    }
+    KDL_LAUNCH(kdl::dedup_singles_kernel, grid, kdl::DD_THREADS, 0, st, *batch, dup_score, l, l.end, l.paired, tot);
+    return check_launch();
+}
+
+int64_t kdl_dedup_scratch_words(int64_t n_entries) {
+    if (n_entries < 0 || n_entries >= (1ll << 31)) return -1;
+    return 3 * n_entries + 2 * dedup_ctas(n_entries);
+}
+
+int kdl_dedup_select(const kdl_dedup_lists* lists, const int64_t* pair_order, int64_t n_pairs,
+                     const int64_t* single_order, int64_t n_singles, int32_t* scratch, int64_t scratch_words,
+                     uint8_t* keep, int64_t* totals, void* stream) {
+    if (n_pairs < 0 || n_singles < 0 || n_pairs >= (1ll << 31) || n_singles >= (1ll << 31) || !totals)
+        return KDL_ERR_INVALID_ARG;
+    if (n_pairs + n_singles == 0) return KDL_OK;
+    const long long need = kdl_dedup_scratch_words(n_pairs > n_singles ? n_pairs : n_singles);
+    if (!dedup_lists_ok(lists) || !keep || !scratch || scratch_words < need || (n_pairs > 0 && !pair_order) ||
+        (n_singles > 0 && !single_order))
+        return KDL_ERR_INVALID_ARG;
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned long long* tot = reinterpret_cast<unsigned long long*>(totals);
+    const kdl_dedup_lists& l = *lists;
+    const kdl::DedupList pairs = {pair_order, n_pairs, l.pair_contig, l.pair_e1, l.pair_e2,
+                                  reinterpret_cast<const unsigned long long*>(l.pair_rank), l.pair_r1, l.pair_r2};
+    const kdl::DedupList singles = {single_order, n_singles, l.single_contig, l.single_key, nullptr,
+                                    reinterpret_cast<const unsigned long long*>(l.single_rank), l.single_read, nullptr};
+    int rc = KDL_OK;
+    for (const kdl::DedupList& L : {pairs, singles}) {  // (one after the other on the stream: the scratch is reused)
+        if (L.m == 0) continue;
+        const long long ctas = dedup_ctas(L.m);
+        unsigned long long* best = reinterpret_cast<unsigned long long*>(scratch);
+        int32_t* run = scratch + 2 * L.m;
+        int32_t* cta_head = run + L.m;
+        int32_t* carry = cta_head + ctas;
+        KDL_LAUNCH(kdl::dedup_heads_kernel, (unsigned)ctas, kdl::DD_THREADS, 0, st, L, best, cta_head);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+        KDL_LAUNCH(kdl::dedup_carry_kernel, 1, kdl::DD_THREADS, 0, st, cta_head, carry, ctas);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+        KDL_LAUNCH(kdl::dedup_best_kernel, (unsigned)ctas, kdl::DD_THREADS, 0, st, L, carry, run, best);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+        KDL_LAUNCH(kdl::dedup_mark_kernel, (unsigned)ctas, kdl::DD_THREADS, 0, st, L, run, best, keep, tot);
+        if ((rc = check_launch()) != KDL_OK) return rc;
+    }
+    return rc;
 }
 
 // K0 + K11 + K11g of one sum policy (kdl::PhredSums or kdl::WeightSums, quality.cu), arguments checked

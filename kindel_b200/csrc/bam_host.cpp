@@ -1178,4 +1178,34 @@ int kdl_bam_fill_qual(kdl_bam* h, int threads, uint8_t* qual8) {
     return KDL_OK;
 }
 
+// The duplicate score of the last prepare's kept reads, in read order (K14, include/kindel_b200.h): -1 where FLAG has
+// 0x100 or 0x800, else the sum of the Phred qualities >= 15 over all of SEQ (0 for a read without qualities),
+// saturating at 2^31 - 1.  Summed here, while the record is at hand, so that no quality byte travels to the device.
+// Refused for SAM text with a QUAL field the text parser could not carry: the caller's text reader decides.
+int kdl_bam_fill_dup(kdl_bam* h, int threads, int32_t* dup_score) {
+    if (!h || !h->prepared || (h->n_kept > 0 && !dup_score) || (h->sam_odd & 2)) return KDL_ERR_INVALID_ARG;
+    const uint8_t* d = h->dptr;
+    const int32_t n_ref = (int32_t)h->ref_name.size();
+    const int64_t n_tasks = (int64_t)h->chunk_lo.size() - 1;
+    h->pool->run(n_tasks, threads, [&](int64_t t, int) {
+        std::vector<int64_t> cr(h->cur_read.begin() + t * n_ref, h->cur_read.begin() + (t + 1) * n_ref);
+        RecView r;
+        for (int64_t i = h->chunk_lo[(size_t)t]; i < h->chunk_lo[(size_t)t + 1]; ++i) {
+            if (h->cls[(size_t)i].cls == CLS_DROP) continue;
+            const int64_t off_i = h->rec_off[(size_t)i];
+            parse_record(d + off_i, h->rec_off[(size_t)i + 1] - off_i, &r);
+            const int64_t k = cr[(size_t)r.ref_id]++;
+            if (r.flag & 0x900u) {
+                dup_score[k] = -1;
+                continue;
+            }
+            int64_t s = 0;
+            if (r.qual && r.l_seq > 0 && r.qual[0] != 0xff)
+                for (int32_t q = 0; q < r.l_seq; ++q) s += r.qual[q] >= 15 ? r.qual[q] : 0;
+            dup_score[k] = s > 0x7fffffff ? 0x7fffffff : (int32_t)s;
+        }
+    });
+    return KDL_OK;
+}
+
 }  // extern "C"

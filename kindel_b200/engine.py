@@ -27,6 +27,8 @@ implementation behind these functions: without a CUDA device they raise.
                                depth of its insert (extension)
     normalise(label, reverse, n_amplicons, cap)  K13: the reads each (amplicon, strand) cap keeps, in batch order
                                (extension: `--normalise N`)
+    dedup(dbatch, mate)        K10p + K14k + sort + K14s: the reads and read pairs duplicate removal keeps (extension:
+                               `--dedup`)
 """
 from __future__ import annotations
 
@@ -730,6 +732,66 @@ def normalise(label: torch.Tensor, reverse: torch.Tensor, n_amplicons: int, cap:
                                words, keep.data_ptr(), total.data_ptr(), dropped.data_ptr(), _stream_ptr(dev))
         _ffi.check(rc, "kdl_normalise")
     return keep[:n], total[:2 * int(n_amplicons)], dropped
+
+
+def _lexsort(keys):
+    """int64 permutation that orders the rows by `keys` (device tensors, most significant first): one stable
+    torch.sort per key, least significant first."""
+    perm = None
+    for k in reversed(keys):
+        idx = torch.sort(k if perm is None else k.index_select(0, perm), stable=True)[1]
+        perm = idx if perm is None else perm.index_select(0, idx)
+    return perm.contiguous()
+
+
+_DEDUP_LISTS = (("pair_contig", torch.int32, 0), ("pair_e1", torch.int64, 0), ("pair_e2", torch.int64, 0),
+                ("pair_rank", torch.int64, 0), ("pair_r1", torch.int32, 0), ("pair_r2", torch.int32, 0),
+                ("single_contig", torch.int32, 1), ("single_key", torch.int64, 1), ("single_rank", torch.int64, 1),
+                ("single_read", torch.int32, 1), ("end", torch.int64, 1), ("paired", torch.uint8, 1))
+
+
+def dedup(dbatch: DeviceBatch, mate: torch.Tensor = None):
+    """K14 (extension: `--dedup`): (keep uint8 [n] on the device, (pairs removed, singles removed, singles shadowed by
+    a pair end)).  keep[r] = 0 for a read that duplicate removal takes out (include/kindel_b200.h has the rule).  Needs a
+    host batch decoded with strand and dup (its `reverse` and `dup_score`); mate: K10p's result, run here when the
+    batch has its mates and mate is None (no mates: every read is a single).  K14k fills the two entry lists; one
+    read-back of the totals record sizes them; each is sorted by key on the device (stable torch.sort passes); K14s
+    selects, and a second read-back gives the totals."""
+    h = dbatch.host
+    if getattr(h, "dup_score", None) is None or getattr(h, "reverse", None) is None:
+        raise ValueError("dedup needs the reads' strands and duplicate scores: decode with strand=True, dup=True")
+    lib = _ffi.load()
+    dev = dbatch.device
+    n = int(dbatch.struct.n_reads)
+    if mate is None and getattr(h, "mates", None) is not None:
+        mate = pair_mates(dbatch)
+    with torch.cuda.device(dev):
+        reverse = torch.from_numpy(np.ascontiguousarray(h.reverse, dtype=np.uint8)).to(dev)
+        score = torch.from_numpy(np.ascontiguousarray(h.dup_score, dtype=np.int32)).to(dev)
+        if mate is not None:
+            mate = mate.to(dev, torch.int32).contiguous()
+        t = {f: torch.empty(max(n if full else n // 2, 1), dtype=dt, device=dev) for f, dt, full in _DEDUP_LISTS}
+        lists = _ffi.KdlDedupLists(*(int(t[f].data_ptr()) for f, _, _ in _DEDUP_LISTS))
+        keep = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        totals = torch.zeros(_ffi.KDL_DEDUP_TOTALS, dtype=torch.int64, device=dev)
+        rc = lib.kdl_dedup_entries(C.byref(dbatch.struct), reverse.data_ptr(), score.data_ptr(),
+                                   mate.data_ptr() if mate is not None and n else None, C.byref(lists),
+                                   keep.data_ptr(), totals.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_dedup_entries")
+        n_pair, n_single = (int(x) for x in totals[:2].cpu())
+        one = int(dbatch.struct.n_contigs) <= 1  # (one contig: its key needs no pass)
+        pk = [t["pair_e1"][:n_pair], t["pair_e2"][:n_pair]]
+        sk = [t["single_key"][:n_single]]
+        p_order = _lexsort(pk if one else [t["pair_contig"][:n_pair]] + pk) if n_pair else None
+        s_order = _lexsort(sk if one else [t["single_contig"][:n_single]] + sk) if n_single else None
+        words = int(lib.kdl_dedup_scratch_words(max(n_pair, n_single)))
+        scratch = torch.empty(max(words, 2), dtype=torch.int32, device=dev)
+        rc = lib.kdl_dedup_select(C.byref(lists), p_order.data_ptr() if n_pair else None, n_pair,
+                                  s_order.data_ptr() if n_single else None, n_single, scratch.data_ptr(), words,
+                                  keep.data_ptr(), totals.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_dedup_select")
+        stats = tuple(int(x) for x in totals[2:5].cpu())
+    return keep[:n], stats
 
 
 _OVERLAP_TOTALS = 8  # words of K10's totals record (include/kindel_b200.h)

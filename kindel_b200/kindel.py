@@ -65,6 +65,7 @@ class PileupRun:
     _dropped_events = None  # K10's dropped insertion-event rows of host tables
     _overlap_stats = None   # K10's (pairs, bases, deletions, insertions) of host tables
     normalised = None  # (N, dropped, kept) of the --normalise cap the batch went through (extension), None when off
+    deduplicated = None  # (pairs removed, singles removed, kept, before) of --dedup (extension), None when off
 
     def __init__(self, batch: bamio.ReadBatch, device=None, primers=None, mask_overlaps=False):
         self.batch = batch
@@ -345,8 +346,35 @@ def _normalise(batch, scheme, cap, strand):
     return batch, (cap, n_dropped, int(batch.n_reads))
 
 
+def check_dedup(dedup) -> bool:
+    """The one check of the dedup option: True or False (ValueError otherwise)."""
+    if not isinstance(dedup, (bool, np.bool_)):
+        raise ValueError("dedup must be True or False, got %r" % (dedup,))
+    return bool(dedup)
+
+
+def _dedup(batch, strand, mates):
+    """(the batch of the reads duplicate removal keeps, (pairs removed, singles removed, kept, before)) (extension:
+    dedup): K10p pairs the mates of the uploaded batch, K14k / the sort / K14s find the duplicates on the device, and
+    only when a read is removed do the keep bytes (1 B per read) come back and the host batch is rebuilt from the kept
+    reads (bamio.select_reads).  The strand bytes and the mates stay only when `strand` / `mates` asked for them."""
+    dbatch = engine.upload(batch, engine.require_cuda())
+    keep, (pairs, singles, _) = engine.dedup(dbatch)
+    before = int(batch.n_reads)
+    if pairs or singles:
+        batch = bamio.select_reads(batch, np.flatnonzero(keep.cpu().numpy()))
+    del dbatch, keep
+    batch.dup_score = None
+    if not strand:
+        batch.reverse = None
+    if not mates:
+        batch.name_hash = batch.mate_start = batch.pair_role = None
+    return batch, (pairs, singles, int(batch.n_reads), before)
+
+
 def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq=0, exclude_flags=0,
-               iupac_threshold=None, strand=False, primers=None, mask_overlaps=False, qual=False, normalise=None):
+               iupac_threshold=None, strand=False, primers=None, mask_overlaps=False, qual=False, normalise=None,
+               dedup=False):
     """(PileupRun, calls) of an alignment file on `devices` GPUs.  devices > 1: one process per GPU, reads (or whole
     contigs) sharded, counts exchanged over NVLink in front of the vote (distributed.run_sharded); the result is
     bit-identical to one GPU.  min_base_quality / min_mapq / exclude_flags (extension, all off by default): a record
@@ -368,25 +396,35 @@ def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq
     (amplicon, strand) in batch order are kept (K13), and the others are removed from the batch as if they were not
     in the file: no count, clip, event or mate of theirs.  Reads without an amplicon are never capped.  Everything
     else -- primer masking, mate pairing, the pileup, several GPUs -- then runs on the kept reads; the run's
-    `normalised` holds (N, dropped, kept)."""
+    `normalised` holds (N, dropped, kept).  dedup (extension, default False = off): after the filters and before
+    normalise, duplicate reads and read pairs are removed as samtools markdup -r removes them: by fragment ends (each
+    read's unclipped 5' end and strand, both mates' for a pair) and a base-quality score, the best of each duplicate set
+    staying (K14, include/kindel_b200.h has the rule).  The removed reads are taken out as if they were not in the
+    file, on this process's GPU before any sharding; the run's `deduplicated` holds (pairs removed, singles removed,
+    kept, before).  A 0x400 flag in the file is not read: `exclude_flags=0x400` honours it."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
     normalise = check_normalise(normalise)
+    dedup = check_dedup(dedup)
     primers, scheme = _normalise_scheme(primers, normalise)
     decode = dict(min_mapq=min_mapq, exclude_flags=exclude_flags, min_base_quality=min_base_quality,
-                  strand=strand or normalise is not None)
-    if mask_overlaps:  # (the keyword only when on: the decode stays as it was otherwise)
+                  strand=strand or normalise is not None or dedup)
+    if mask_overlaps or dedup:  # (the keyword only when on: the decode stays as it was otherwise)
         decode["mates"] = True
     if qual:
         decode["qual"] = True
+    if dedup:
+        decode["dup"] = True
     batch = bamio.read_alignment(bam_path, **decode)
-    normalised = None
+    deduplicated = normalised = None
+    if dedup:
+        batch, deduplicated = _dedup(batch, strand or normalise is not None, mask_overlaps)
     if normalise is not None:
         batch, normalised = _normalise(batch, scheme, normalise, strand)
     arrays = primer_arrays(primers, batch.contig_names, batch.contig_len) if primers is not None else None
     devices = _default_devices(devices)
     if devices <= 1:
         run = PileupRun(batch, primers=primers, mask_overlaps=mask_overlaps)
-        run.normalised = normalised
+        run.normalised, run.deduplicated = normalised, deduplicated
         return run, None
     from . import distributed
 
@@ -399,17 +437,17 @@ def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq
     dropped = None if drops is None else np.sort(drops[drops[:, 3] >= 0, 3].astype(np.int64))
     run = PileupRun.from_host_tables(batch, counts, derived, events, primers=primers, mask_overlaps=mask_overlaps,
                                      dropped_events=dropped, overlap_stats=stats)
-    run.normalised = normalised
+    run.normalised, run.deduplicated = normalised, deduplicated
     return run, calls
 
 
 def parse_bam(bam_path, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None,
-              mask_overlaps=False, normalise=None):
+              mask_overlaps=False, normalise=None, dedup=False):
     """Alignment information for each reference sequence, first-seen order
-    (reference kindel/kindel.py:131-153).  devices, the filters, primers, mask_overlaps and normalise: extensions,
-    see pileup_run."""
+    (reference kindel/kindel.py:131-153).  devices, the filters, primers, mask_overlaps, normalise and dedup:
+    extensions, see pileup_run."""
     return pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags,
-                      primers=primers, mask_overlaps=mask_overlaps, normalise=normalise)[0].alignments()
+                      primers=primers, mask_overlaps=mask_overlaps, normalise=normalise, dedup=dedup)[0].alignments()
 
 
 # --------------------------------------------------------------------------------- consensus
@@ -733,7 +771,7 @@ DepthRange = namedtuple("DepthRange", ["dmin", "dmax"])  # min / max ACGT depth 
 
 def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_depth, min_overlap,
                  clip_decay_threshold, trim_ends, uppercase, filters=None, iupac_threshold=None, primers=None,
-                 overlaps=None, quality_vote_sites=None, normalised=None):
+                 overlaps=None, quality_vote_sites=None, normalised=None, deduplicated=None):
     """REPORT text block (reference kindel/kindel.py:437-485).  filters (extension): (min_base_quality, min_mapq,
     exclude_flags); when any is set, three option lines follow `- uppercase:`, otherwise the text is the reference's.
     iupac_threshold (extension): when set, `- iupac_threshold:` follows the option lines and `- iupac sites:` (the
@@ -743,7 +781,9 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
     `- mate overlaps:` follows the filter and primer lines.  quality_vote_sites (extension: quality_vote): the 1-based
     positions (strings) whose call differs from the reference's vote; when set, `- quality_vote: True` follows the
     option lines and `- quality-vote sites:` follows `- ambiguous sites:`.  normalised (extension: normalise): the run's
-    (N, dropped, kept); when set, `- normalise:` follows the primer line."""
+    (N, dropped, kept); when set, `- normalise:` follows the primer line.  deduplicated (extension: dedup): the run's
+    (pairs removed, singles removed, kept, before); when set, `- duplicates:` follows the primer line, before
+    `- normalise:`."""
     if isinstance(weights, DepthRange):  # already reduced on the device: no table copy needed
         dmin, dmax = weights.dmin, weights.dmax
     elif isinstance(weights, BaseCounts):
@@ -776,6 +816,8 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
                   "- exclude_flags: {:#x}".format(filters[2])]
     if primers is not None:
         lines.append("- primers: {}".format(primers))
+    if deduplicated is not None:
+        lines.append("- duplicates: {} pairs and {} single reads removed, {} of {} reads kept".format(*deduplicated))
     if normalised is not None:
         cap, dropped, kept = normalised
         lines.append("- normalise: {} per amplicon and strand, {} of {} reads dropped".format(cap, dropped,
@@ -807,14 +849,15 @@ def build_report(ref_id, weights, changes, cdr_patches, bam_path, realign, min_d
 def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_decay_threshold=0.1,
                      mask_ends=50, trim_ends=False, uppercase=False, devices=None, min_base_quality=0, min_mapq=0,
                      exclude_flags=0, iupac_threshold=None, qualities=False, primers=None, mask_overlaps=False,
-                     quality_vote=False, normalise=None):
+                     quality_vote=False, normalise=None, dedup=False):
     """Consensus sequence(s) of an alignment file (reference kindel/kindel.py:488-555).
 
     Device work per file: one pileup (K1) and one vote (K2) over all contigs at once; only the
     call bytes, the insertion events and -- for --realign and the report -- count columns come
     back to the host.  `devices` (extension; default $KINDEL_GPUS or 1) shards the pileup over that many GPUs of
-    the node.  min_base_quality / min_mapq / exclude_flags / primers / mask_overlaps / normalise: extension, see
-    pileup_run; with normalise the REPORT gains `- normalise:` after `- primers:`.
+    the node.  min_base_quality / min_mapq / exclude_flags / primers / mask_overlaps / normalise / dedup: extension,
+    see pileup_run; with normalise the REPORT gains `- normalise:` after `- primers:`, with dedup `- duplicates:`
+    between the two.
 
     iupac_threshold (extension; default None = off, the reference's vote): t in [0, 1].  Where a base is emitted,
     the call is the smallest set of the most frequent bases (A, C, G, T; N is not an allele) that holds at least
@@ -835,7 +878,7 @@ def bam_to_consensus(bam_path, realign=False, min_depth=1, min_overlap=9, clip_d
     quality_vote = check_quality_vote(quality_vote, iupac_threshold)
     filters = (min_base_quality, min_mapq, exclude_flags)
     run, calls = pileup_run(bam_path, devices, min_depth, *filters, iupac_threshold=iupac_threshold, primers=primers,
-                            mask_overlaps=mask_overlaps, qual=quality_vote, normalise=normalise)
+                            mask_overlaps=mask_overlaps, qual=quality_vote, normalise=normalise, dedup=dedup)
     if calls is None or quality_vote:  # (several GPUs: the ranks' majority calls give way to the reduced table's)
         calls = run.vote(min_depth, iupac_threshold, quality=quality_vote)
     return consensus_from_run(run, calls, bam_path, realign, min_depth, min_overlap,
@@ -1017,7 +1060,8 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
         report = build_report(ref_id, report_weights, changes, cdr_patches, bam_path, realign, min_depth,
                               min_overlap, clip_decay_threshold, trim_ends, uppercase, filters, iupac_threshold,
                               primers=primers_name, overlaps=overlaps, quality_vote_sites=qv_sites,
-                              normalised=getattr(run, "normalised", None))
+                              normalised=getattr(run, "normalised", None),
+                              deduplicated=getattr(run, "deduplicated", None))
         consensuses.append(consensus_seqrecord(cons, ref_id, quals))
         refs_reports[ref_id] = report
         refs_changes[ref_id] = changes
@@ -1027,13 +1071,13 @@ def consensus_from_run(run, calls_all, bam_path, realign=False, min_depth=1, min
 def weights(bam_path: "path to SAM/BAM file", relative: "output relative nucleotide frequencies" = False,
             confidence: "calculate confidence interval" = True, confidence_alpha: "confidence interval alpha" = 0.01,
             devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0, primers=None, mask_overlaps=False,
-            normalise=None):
+            normalise=None, dedup=False):
     """DataFrame of per-site nucleotide frequencies, depth, consensus, clip starts/ends, confidence
     interval and entropy (reference kindel/kindel.py:558-630).  Integer columns come from the GPU
     table; the float tail is the reference's arithmetic, vectorised.  devices, the filters, primers,
-    mask_overlaps and normalise: extensions, see pileup_run."""
+    mask_overlaps, normalise and dedup: extensions, see pileup_run."""
     run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers,
-                     mask_overlaps=mask_overlaps, normalise=normalise)[0]
+                     mask_overlaps=mask_overlaps, normalise=normalise, dedup=dedup)[0]
     return weights_from_run(run, relative, confidence, confidence_alpha)
 
 
@@ -1089,7 +1133,7 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
              rel_threshold: "relative frequency (0.0-1.0) above which to call variants" = 0.01,
              only_variants: "exclude invariant sites from output" = False,
              absolute: "report absolute variant frequencies" = False, devices=None, min_base_quality=0, min_mapq=0,
-             exclude_flags=0, primers=None, mask_overlaps=False, normalise=None):
+             exclude_flags=0, primers=None, mask_overlaps=False, normalise=None, dedup=False):
     """EXTENSION -- not in the reference snapshot.  The reference's README (README.md:106-107) lists a `variants`
     sub-command ("Output variants exceeding specified absolute and relative frequency thresholds") but its code
     (kindel/kindel.py, kindel/cli.py) has no such function, so there is nothing to be bit-exact with: parity
@@ -1099,9 +1143,9 @@ def variants(bam_path: "path to SAM/BAM file", abs_threshold: "absolute frequenc
     (variant_alleles).  Columns: chrom, pos, depth, consensus (allele letter, `-` = deletion), then one column per
     allele holding its relative (default) or absolute frequency where it is a variant and 0 elsewhere.  With
     only_variants the sites are selected on the device (K6, variant_sites) and only they are copied back.  primers,
-    mask_overlaps, normalise: extensions, see pileup_run."""
+    mask_overlaps, normalise, dedup: extensions, see pileup_run."""
     run = pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags, primers=primers,
-                     mask_overlaps=mask_overlaps, normalise=normalise)[0]
+                     mask_overlaps=mask_overlaps, normalise=normalise, dedup=dedup)[0]
     return variants_from_run(run, abs_threshold, rel_threshold, only_variants, absolute)
 
 
@@ -1206,12 +1250,13 @@ def _vcf_header(run, abs_threshold, rel_threshold, filters, **options):
     normalised = getattr(run, "normalised", None)
     return vcf.header(run.batch.contig_names, run.batch.contig_len, abs_threshold, rel_threshold, filters,
                       getattr(run, "primers", None), getattr(run, "mask_overlaps", False),
-                      normalise=None if normalised is None else normalised[0], **options)
+                      normalise=None if normalised is None else normalised[0],
+                      dedup=getattr(run, "deduplicated", None) is not None, **options)
 
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
                  exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None, mask_overlaps=False,
-                 samples=None, qual=False, min_qual=None, normalise=None) -> str:
+                 samples=None, qual=False, min_qual=None, normalise=None, dedup=False) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -1253,7 +1298,10 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     with several samples (ValueError); a kept read without qualities is a ValueError.
 
     normalise (extension: `--normalise N`, needs a named `primers` scheme): see pileup_run; every sample's reads are
-    capped as it would be alone, and the header gets `##kindelNormalise=N` after `##kindelPrimers`."""
+    capped as it would be alone, and the header gets `##kindelNormalise=N` after `##kindelPrimers`.
+
+    dedup (extension: `--dedup`): see pileup_run; every sample's duplicates are removed as they would be alone, and the
+    header gets `##kindelDedup=fragment ends, base-quality score` after `##kindelPrimers`, before `##kindelNormalise`."""
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
     min_qual = check_min_qual(min_qual)
@@ -1267,12 +1315,12 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
 
         return cohort.variants_vcf(bam_path, abs_threshold, rel_threshold, devices, min_base_quality, min_mapq,
                                    exclude_flags, reference=reference, primers=primers, mask_overlaps=mask_overlaps,
-                                   samples=samples, normalise=normalise)
+                                   samples=samples, normalise=normalise, dedup=dedup)
     if samples is not None:
         raise ValueError("samples= names the columns of several samples: pass the alignment files as a list")
     filters = (min_base_quality, min_mapq, exclude_flags)
     run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers, mask_overlaps=mask_overlaps,
-                     qual=qual, normalise=normalise)[0]
+                     qual=qual, normalise=normalise, dedup=dedup)[0]
     return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference, strand=strand,
                                  max_sor=max_sor, qual=qual, min_qual=min_qual)
 
@@ -1329,7 +1377,8 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
     min_mapq, exclude_flags) as the pileup applied them, for the header.  reference, strand, max_sor: see variants_vcf;
     vcf.records has the rules of the records.  Strand needs a run whose batch has `reverse`
     (ValueError otherwise).  A run piled with primers (extension) adds its `##kindelPrimers` line, one piled with
-    mask_overlaps its `##kindelMateOverlaps` line, one piled with normalise its `##kindelNormalise` line.
+    mask_overlaps its `##kindelMateOverlaps` line, one piled with normalise its `##kindelNormalise` line, one piled
+    with dedup its `##kindelDedup` line.
 
     Strand counts (ADF, ADR): without a reference they are the reverse table's counts of the record's AD columns and
     the total's minus those, so ADF + ADR == AD.  With one, an SNV's the same (REF 0 where the reference has no A, C,
@@ -1372,13 +1421,14 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
 
 
 def features(bam_path: "path to SAM/BAM file", devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0,
-             primers=None, mask_overlaps=False, normalise=None):
+             primers=None, mask_overlaps=False, normalise=None, dedup=False):
     """DataFrame of relative per-site nucleotide frequencies, indels and entropy
     (reference kindel/kindel.py:633-664), including its indexing of `i`/`d` by global row number
     into the LAST contig's tables (IndexError on most multi-contig files, SURVEY.md A-14).
-    devices, the filters, primers, mask_overlaps and normalise: extensions, see pileup_run."""
+    devices, the filters, primers, mask_overlaps, normalise and dedup: extensions, see pileup_run."""
     return features_from_run(pileup_run(bam_path, devices, 1, min_base_quality, min_mapq, exclude_flags,
-                                        primers=primers, mask_overlaps=mask_overlaps, normalise=normalise)[0])
+                                        primers=primers, mask_overlaps=mask_overlaps, normalise=normalise,
+                                        dedup=dedup)[0])
 
 
 def features_from_run(run):
@@ -1497,7 +1547,7 @@ def amplicons_from_run(run, scheme, min_depth=20):
 
 
 def amplicons(bam_path, primers, min_depth=20, devices=None, min_base_quality=0, min_mapq=0, exclude_flags=0,
-              mask_overlaps=False, samples=None, normalise=None):
+              mask_overlaps=False, samples=None, normalise=None, dedup=False):
     """Per sample and amplicon of a tiled primer scheme, its reads and the depth of its insert (extension: `kindel
     amplicons`; the reference has no such command).  bam_path: one alignment file or a list of them; primers: a named
     primer BED (primers.load_scheme) or an AmpliconScheme.  Each file is piled with `primers=` the scheme's rows, under
@@ -1506,7 +1556,8 @@ def amplicons(bam_path, primers, min_depth=20, devices=None, min_base_quality=0,
     a DataFrame with the columns AMPLICON_COLUMNS, in argument order of the samples, then amplicons_from_run's order;
     attrs["reads"] = {sample: (kept, assigned, unprimed, mispaired, ambiguous)}.  normalise (extension: `--normalise
     N`): each file's reads are capped first (pileup_run), so the reads and depths are those of the kept reads, and
-    attrs["dropped"] = {sample: the reads over the cap}."""
+    attrs["dropped"] = {sample: the reads over the cap}.  dedup (extension: `--dedup`): each file's duplicates are
+    removed first (pileup_run), and attrs["duplicates"] = {sample: the reads removed}."""
     import pandas as pd
 
     from .cohort import sample_names
@@ -1516,15 +1567,19 @@ def amplicons(bam_path, primers, min_depth=20, devices=None, min_base_quality=0,
     paths = [bam_path] if isinstance(bam_path, (str, os.PathLike)) else list(bam_path)
     names = sample_names(paths, samples)
     normalise = check_normalise(normalise)
-    frames, reads, dropped = [], {}, {}
+    dedup = check_dedup(dedup)
+    frames, reads, dropped, duplicates = [], {}, {}, {}
     for path, name in zip(paths, names):
         run, _ = pileup_run(path, devices, 1, min_base_quality, min_mapq, exclude_flags,
                             primers=scheme.primers if normalise is None else scheme, mask_overlaps=mask_overlaps,
-                            normalise=normalise)
+                            normalise=normalise, dedup=dedup)
         df = amplicons_from_run(run, scheme, min_depth)
         reads[name] = df.attrs["reads"]
         if normalise is not None:
             dropped[name] = run.normalised[1]
+        if dedup:
+            pairs, singles, _, _ = run.deduplicated
+            duplicates[name] = 2 * pairs + singles
         df.insert(0, "sample", name)
         frames.append(df)
         del run
@@ -1532,4 +1587,6 @@ def amplicons(bam_path, primers, min_depth=20, devices=None, min_base_quality=0,
     out.attrs["reads"] = reads
     if normalise is not None:
         out.attrs["dropped"] = dropped
+    if dedup:
+        out.attrs["duplicates"] = duplicates
     return out

@@ -649,3 +649,77 @@ def simple_pairs(seed: int, contig_len: int, depth: float, read_len: int = 150, 
                            np.arange(n + 1, dtype=np.int64), np.full(n, read_len << 4, dtype=np.int64), seq4,
                            n_records=n, reverse=((flag & 0x10) != 0).astype(np.uint8), mates=mates)
     return batch, flag, frag
+
+
+def dup_pairs(seed: int, contig_len: int, depth: float, read_len: int = 150, insert_mean: float = 300,
+              insert_sd: float = 40, dup_frac: float = 0.2, clip_frac: float = 0.3, sub_rate: float = 0.01,
+              amplicons=None, want_qual: bool = False):
+    """Shotgun read pairs with planted PCR duplicates (`--dedup`), vectorised: simple_pairs' fragments, of which a
+    seeded share `dup_frac` is copied 1-5 more times, so many that the pairs, copies included, make `depth`.  Each copy is a fragment of its own (QNAME, qualities) over the
+    same two ends: which mate is first (FLAG 0x40) is drawn afresh, and with probability `clip_frac` each mate soft-clips
+    1-20 bases of its 5' end (the left mate's start moves right by the clip, the right mate's M shrinks), which leaves
+    its unclipped end where it was.  amplicons: scheme rows; every fragment is then one whole amplicon (the extreme
+    case: thousands of copies of one key).  The batch has strands, mates and `dup_score` (the sum of its seeded
+    qualities >= 15, synth.qualities).  Returns (batch, flag, frag, qual): qual the concatenated qualities in read order
+    when want_qual, else None."""
+    rng = np.random.default_rng(seed)
+    n0 = int(round(depth * contig_len / (2 * read_len) / (1 + 3 * dup_frac)))  # 3 copies on average: depth overall
+    if amplicons is None:
+        ins0 = np.clip(np.round(rng.normal(insert_mean, insert_sd, n0)), read_len, contig_len - 2).astype(np.int64)
+        lo0 = rng.integers(1, np.maximum(contig_len - ins0, 2))
+    else:
+        a = np.array([x for _, x, _ in amplicons[0::2]], dtype=np.int64)
+        b = np.array([y for _, _, y in amplicons[1::2]], dtype=np.int64)
+        k = rng.integers(0, a.shape[0], size=n0)
+        lo0, ins0 = a[k], np.maximum(b[k] - a[k], read_len)
+    copies = np.where(rng.random(n0) < dup_frac, rng.integers(1, 6, n0), 0)
+    src = np.repeat(np.arange(n0), 1 + copies)
+    n_frag = src.shape[0]
+    lo, ins = lo0[src], ins0[src]
+    is_copy = np.concatenate(([False], src[1:] == src[:-1]))
+    clip = np.where(is_copy[:, None] & (rng.random((n_frag, 2)) < clip_frac), rng.integers(1, 21, (n_frag, 2)), 0)
+    first_left = rng.random(n_frag) < 0.5
+    L = read_len
+    frag = np.repeat(np.arange(n_frag, dtype=np.int64), 2)
+    left = np.tile(np.array([True, False]), n_frag)
+    win = np.where(left, np.repeat(lo, 2), np.repeat(lo + ins - L, 2))  # the mate's SEQ is ref[win : win + L]
+    cl = np.where(left, np.repeat(clip[:, 0], 2), np.repeat(clip[:, 1], 2))  # the mate's 5' soft clip
+    start = win + np.where(left, cl, 0)
+    mate_start = np.where(left, np.repeat(lo + ins - L, 2), np.repeat(lo + clip[:, 0], 2))
+    first = left == np.repeat(first_left, 2)
+    flag = (0x1 | 0x2 | np.where(first, 0x40, 0x80) | np.where(left, 0x20, 0x10)).astype(np.uint16)
+    order = np.argsort(start, kind="stable")
+    start, mate_start, flag, frag, win, cl, left = (x[order] for x in (start, mate_start, flag, frag, win, cl, left))
+    n = start.shape[0]
+    n_ops = np.where(cl > 0, 2, 1)
+    cig_off = np.concatenate(([0], np.cumsum(n_ops)))
+    cigar = np.empty(int(cig_off[-1]), dtype=np.int64)
+    at = cig_off[:-1]
+    m_len = L - cl
+    cigar[at] = np.where((cl > 0) & left, (cl << 4) | 4, m_len << 4)
+    two = np.flatnonzero(cl > 0)
+    cigar[at[two] + 1] = np.where(left[two], m_len[two] << 4, (cl[two] << 4) | 4)
+    words = (L + 7) // 8
+    ref = random_contig(rng, contig_len)
+    ref_pad = np.concatenate([ref, np.zeros(words * 8, dtype=np.uint8)])
+    parts, scores, quals = [], [], []
+    for s0 in range(0, n, 1 << 18):
+        w = win[s0:s0 + (1 << 18)]
+        nib = ref_pad[w[:, None] + np.arange(words * 8, dtype=np.int64)[None, :]]
+        nib[:, L:] = 0
+        n_sub = rng.binomial(w.shape[0] * L, sub_rate)
+        nib[rng.integers(0, w.shape[0], size=n_sub), rng.integers(0, L, size=n_sub)] = _CODE[rng.integers(0, 5, size=n_sub)]
+        parts.append(_pack_rows(nib))
+        q = qualities(seed * 1000003 + s0, np.full(w.shape[0], L)).reshape(-1, L)
+        scores.append(np.where(q >= 15, q, 0).sum(axis=1, dtype=np.int64).astype(np.int32))
+        if want_qual:
+            quals.append(q.reshape(-1))
+    seq4 = np.concatenate(parts).reshape(-1) if parts else np.zeros(0, dtype=np.uint32)
+    roles = np.where((flag & 0x40) != 0, 1, 2).astype(np.uint8)
+    mates = (_fnv_rows(pair_names(frag)), mate_start, roles)
+    batch = bamio.finalize(["ctg0"], np.array([contig_len]), np.array([0, n]), start,
+                           np.arange(n, dtype=np.int64) * words, np.full(n, L, dtype=np.int64), cig_off, cigar, seq4,
+                           n_records=n, reverse=((flag & 0x10) != 0).astype(np.uint8), mates=mates,
+                           dup_score=np.concatenate(scores) if scores else np.zeros(0, dtype=np.int32))
+    qual = (np.concatenate(quals) if quals else np.zeros(0, dtype=np.uint8)) if want_qual else None
+    return batch, flag, frag, qual

@@ -34,10 +34,10 @@ def check_number(value, name):
 
 def header(contig_names, contig_len, abs_threshold, rel_threshold, filters, primers=None, mask_overlaps=False,
            reference_name=None, strand=False, max_sor=None, qual=False, min_qual=None, samples=None,
-           normalise=None) -> list:
+           normalise=None, dedup=False) -> list:
     """The header lines, the column line last.  filters: (min_base_quality, min_mapq, exclude_flags) or None; primers:
     the run's PrimerSet or None; samples: the FORMAT columns' names (a multi-sample VCF) or None; normalise: the
-    --normalise cap N or None."""
+    --normalise cap N or None; dedup: the run went through --dedup."""
     from . import __version__
 
     mbq, mapq, flags = filters if filters is not None else (0, 0, 0)
@@ -46,6 +46,8 @@ def header(contig_names, contig_len, abs_threshold, rel_threshold, filters, prim
              .format(abs_threshold, rel_threshold, mbq, mapq, flags)]
     if primers is not None:
         lines.append("##kindelPrimers={}".format(primers.name))
+    if dedup:
+        lines.append("##kindelDedup=fragment ends, base-quality score")
     if normalise is not None:
         lines.append("##kindelNormalise={}".format(normalise))
     if mask_overlaps:

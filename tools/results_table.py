@@ -58,6 +58,8 @@ def row(path: str, d: dict) -> str:
         work += ", + per-amplicon report (K12, label counts, K12d)"
     if d.get("normalise_ms"):
         work += ", + depth normalisation (K12, K13) at N = %d" % cfg.get("cap", 0)
+    if d.get("dedup_ms"):
+        work += ", + duplicate removal (K10p, K14k, sort, K14s)"
     if d.get("mates_ms"):
         work += ", + mate-overlap masking (K10p, K10, K10u)"
     if d.get("cohort_ms"):
