@@ -401,7 +401,9 @@ def pileup_run(bam_path, devices=None, min_depth=1, min_base_quality=0, min_mapq
     read's unclipped 5' end and strand, both mates' for a pair) and a base-quality score, the best of each duplicate set
     staying (K14, include/kindel_b200.h has the rule).  The removed reads are taken out as if they were not in the
     file, on this process's GPU before any sharding; the run's `deduplicated` holds (pairs removed, singles removed,
-    kept, before).  A 0x400 flag in the file is not read: `exclude_flags=0x400` honours it."""
+    kept, before).  A 0x400 flag in the file is not read: `exclude_flags=0x400` honours it.  A read that dedup or
+    normalise removes still counts for the first-seen order of contigs, as a filtered record does: the run reports
+    the whole file's contigs in the whole file's order."""
     iupac_threshold = check_iupac_threshold(iupac_threshold)
     normalise = check_normalise(normalise)
     dedup = check_dedup(dedup)

@@ -150,8 +150,8 @@ def keep_by_record(path, contig_names, min_mapq=0, exclude_flags=0):
     return keep, totals, _file_indices(path, contig_names, min_mapq, exclude_flags, keep)
 
 
-def _file_indices(path, contig_names, min_mapq, exclude_flags, keep):
-    """The file indices of the kept records with keep 0 (same filter and order as py_moracle.kept)."""
+def read_order(path, contig_names, min_mapq=0, exclude_flags=0):
+    """The file indices of the kept records in the engine's read order (same filter and order as py_moracle.kept)."""
     from . import samdecode
 
     _, records = samdecode.read_alignment_file(path)
@@ -159,5 +159,10 @@ def _file_indices(path, contig_names, min_mapq, exclude_flags, keep):
     for i, r in enumerate(records):
         if r.mapped and len(r.seq) > 1 and not (r.flag & exclude_flags) and not (min_mapq and r.mapq < min_mapq):
             groups.setdefault(r.rname, []).append(i)
-    order = [i for nm in contig_names for i in groups.get(nm, [])]
+    return [i for nm in contig_names for i in groups.get(nm, [])]
+
+
+def _file_indices(path, contig_names, min_mapq, exclude_flags, keep):
+    """The file indices of the kept records with keep 0."""
+    order = read_order(path, contig_names, min_mapq, exclude_flags)
     return {i for i, k in zip(order, keep.tolist()) if not k}

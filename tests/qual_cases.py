@@ -20,13 +20,17 @@ def _alt(b):
 
 
 def write_sam(path, contigs, recs):
-    """SAM text of records (ref_id, pos0, flag, cigar words, seq, name, mapq, qual or None)."""
+    """SAM text of records (ref_id, pos0, flag, cigar words, seq, name, mapq, qual or None[, next ref_id, next pos0]),
+    as bamio.write_bam takes them: RNEXT / PNEXT `*` / 0 without a mate, CIGAR `*` without ops."""
     lines = ["@HD\tVN:1.6\tSO:unsorted"] + ["@SQ\tSN:%s\tLN:%d" % c for c in contigs]
-    for ref_id, pos, flag, cig, seq, name, mapq, qual in recs:
-        cig_text = "".join("%d%s" % (w >> 4, "MIDNSHP=X"[w & 15]) for w in cig)
+    for rec in recs:
+        ref_id, pos, flag, cig, seq, name, mapq, qual = rec[:8]
+        nref, npos = rec[8:10] if len(rec) >= 10 else (-1, -1)
+        cig_text = "".join("%d%s" % (w >> 4, "MIDNSHP=X"[w & 15]) for w in cig) or "*"
         qtext = "*" if qual is None else "".join(chr(33 + x) for x in qual)
-        lines.append("\t".join([name, str(flag), contigs[ref_id][0], str(pos + 1), str(mapq), cig_text, "*", "0", "0",
-                                seq, qtext]))
+        rnext = "*" if nref < 0 else ("=" if nref == ref_id else contigs[nref][0])
+        lines.append("\t".join([name, str(flag), contigs[ref_id][0], str(pos + 1), str(mapq), cig_text, rnext,
+                                str(npos + 1) if nref >= 0 else "0", "0", seq, qtext]))
     with open(path, "w") as fh:
         fh.write("\n".join(lines) + "\n")
 
