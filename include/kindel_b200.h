@@ -345,6 +345,23 @@ int kdl_deletion_count(const kdl_batch* batch, uint32_t* block_sums, void* strea
 int kdl_deletion_scatter(const kdl_batch* batch, const uint32_t* block_sums, int64_t n_events, int64_t* ev_slot,
                          int32_t* ev_len, void* stream);
 
+/* K15d / K15i -- indel events left-aligned against the reference (extension: `variants --vcf --reference
+ * --left-align`).  ref[n_slots]: K6r's codes (0-3 = A, C, G, T, 4 = anything else and every slot that is not a
+ * position); s0 = contig_slot of the event's contig (the last contig with contig_slot <= the event's slot).
+ * kdl_left_align_deletions: keys[i] = r << 28 | n, a K7 event (slot r, length n) or a group of them; while r > s0,
+ * ref[r-1] < 4 and ref[r-1] == ref[r+n-1], r -= 1; keys_out[i] = the moved key (keys_out may be keys).  The caller
+ * groups the moved keys again (equal keys: one group, the counts summed).
+ * kdl_left_align_insertions: ins_events[n_events][4] = kdl_pileup's rows (slot p, read, q_off, len) of `batch`, 16-byte
+ * aligned; t = the read's bases q_off .. min(q_off + len, SEQ) - 1 in seq4, m of them.  With k = 0: while m > 0,
+ * p > s0, ref[p-1] < 4 and the base t[(m-1-k) mod m] is that code (A, C, G, T; any other nibble matches nothing),
+ * p -= 1 and k += 1.  norm_slot[i] = p, rot[i] = k mod m (0 at m = 0): the normalised string is t rotated right by
+ * rot[i]; hist[p] += 1 (atomics: hist is int32[n_slots], zeroed by the caller).  A row with dead[i] != 0 (dead may be
+ * NULL) gets norm_slot -1, rot 0 and counts in no slot.  One thread per key / row.  Device pointers. */
+int kdl_left_align_deletions(const int64_t* keys, int64_t n_keys, const int64_t* contig_slot, int32_t n_contigs,
+                             const uint8_t* ref, int64_t* keys_out, void* stream);
+int kdl_left_align_insertions(const kdl_batch* batch, const int32_t* ins_events, int64_t n_events, const uint8_t* dead,
+                              const uint8_t* ref, int64_t* norm_slot, int32_t* rot, int32_t* hist, void* stream);
+
 /* K8 (extension: `variants --vcf --strand`): the sub-batch of the reads with keep[r] != 0, built on the device.  The
  * result equals what the host's bamio.select_reads gives for np.flatnonzero(keep), field for field: the kept reads in
  * their order; seq_off dense; l_seq the parent's word (classification is per read); seq4 each kept read's bases and, for

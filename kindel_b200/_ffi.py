@@ -172,6 +172,10 @@ _PROTOTYPES = {
     "kdl_deletion_count": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_void_p]),
     "kdl_deletion_scatter": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                        C.c_void_p]),
+    "kdl_left_align_deletions": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                           C.c_void_p]),
+    "kdl_left_align_insertions": (C.c_int, [C.POINTER(KdlBatch), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_select_scratch_words": (C.c_int64, [C.c_int64]),
     "kdl_select_count": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_void_p, C.c_void_p]),
     "kdl_select_scatter": (C.c_int, [C.POINTER(KdlBatch), C.POINTER(KdlQmask), C.c_void_p, C.c_void_p,

@@ -6,7 +6,8 @@ extension one FASTQ record per contig instead),
 `weights` / `features` write TSV to stdout (cli.py:44,50), `version` prints `kindel <version>`;
 `variants` (in the reference's README only) is an extension, see kindel.variants; its `--vcf` writes a sites-only VCF
 (kindel.variants_vcf), against a FASTA with `--reference`, with per-strand counts and a strand odds ratio with
-`--strand` / `--max-sor`, with a base-quality QUAL with `--qual` / `--min-qual`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
+`--strand` / `--max-sor`, with a base-quality QUAL with `--qual` / `--min-qual`, with its indels left-aligned with
+`--left-align`.  `--primers scheme.bed` (consensus, weights, features, variants) masks the amplicon primer
 bases of every read before the pileup (kindel_b200/primers.py); `--mask-overlaps` counts each read pair once where
 its mates overlap (include/kindel_b200.h K10); `--normalise N` with a named scheme keeps at most N reads of each
 amplicon and strand (K12 + K13, include/kindel_b200.h); `--dedup` removes duplicate reads and read pairs (K14).  `amplicons --primers scheme.bed` (an extension) writes a TSV row per
@@ -57,7 +58,7 @@ def features(bam_path, gpus=None, **filters):
 
 
 def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False, absolute=False, gpus=None, vcf=False,
-             reference=None, strand=False, max_sor=None, qual=False, min_qual=None, **filters):
+             reference=None, strand=False, max_sor=None, qual=False, min_qual=None, left_align=False, **filters):
     """Output variants exceeding specified absolute and relative frequency thresholds"""
     from . import kindel
 
@@ -67,6 +68,8 @@ def variants(bam_path, abs_threshold=1, rel_threshold=0.01, only_variants=False,
             extra.update(strand=True, max_sor=max_sor)
         if qual or min_qual is not None:  # extension: QUAL, BQ / AQ (and FILTER lowqual)
             extra.update(qual=True, min_qual=min_qual)
+        if left_align:  # extension: indels moved to their leftmost place against the reference
+            extra.update(left_align=True)
         sys.stdout.write(kindel.variants_vcf(bam_path, abs_threshold, rel_threshold, devices=gpus, **filters, **extra))
         return
     kindel.variants(bam_path, abs_threshold, rel_threshold, only_variants, absolute, devices=gpus, **filters).to_csv(
@@ -268,9 +271,13 @@ def build_parser() -> argparse.ArgumentParser:
                    help="with --vcf: QUAL from the base qualities (Poisson error model), BQ / AQ in INFO")
     p.add_argument("--min-qual", type=_min_qual, default=None, metavar="X",
                    help="with --vcf: FILTER `lowqual` where QUAL is below X (implies --qual)")
+    # extension: every indel moved to its leftmost place against the reference before the events are counted
+    p.add_argument("--left-align", action="store_true",
+                   help="with --vcf --reference: left-align insertions and deletions against the reference before they "
+                        "are grouped and counted")
     p.set_defaults(func=lambda a: variants(a.bam_path[0] if len(a.bam_path) == 1 else a.bam_path, a.abs_threshold,
                                            a.rel_threshold, a.only_variants, a.absolute, a.gpus, a.vcf, a.reference,
-                                           a.strand, a.max_sor, a.qual, a.min_qual, **_filters(a)))
+                                           a.strand, a.max_sor, a.qual, a.min_qual, a.left_align, **_filters(a)))
 
     # extension: per-amplicon reads and depth of a tiled primer scheme (the BED's name column says which primers pair)
     p = sub.add_parser("amplicons", help=amplicons.__doc__, description=amplicons.__doc__, formatter_class=fmt)
@@ -306,6 +313,8 @@ def _check_variants_args(parser, args):
             parser.error("variants: --strand and --max-sor take one alignment file")
         if args.qual or args.min_qual is not None:
             parser.error("variants: --qual and --min-qual take one alignment file")
+    if getattr(args, "left_align", False) and (not args.vcf or args.reference is None):
+        parser.error("variants: --left-align needs --vcf and --reference (the indels move against its bases)")
     if getattr(args, "vcf", False):
         for flag, on in (("--absolute", args.absolute), ("--only-variants", args.only_variants)):
             if on:

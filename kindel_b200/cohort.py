@@ -14,7 +14,10 @@ writes:
   sites     K6m (engine.variant_sites_multi) over T: the slots where some sample passes, with the OR of the bits.
   records   vcf.records over every sample's rows at the sites, with FORMAT DP:AD:AF per sample: the deletions are
             engine.deletion_union's union of the (slot, length) keys that pass in some sample, the insertions the
-            union of the samples' strings at a candidate slot (vcf.records has the rules)."""
+            union of the samples' strings at a candidate slot (vcf.records has the rules).
+  left_align  (extension) each sample's deletion groups (K15d) and insertion rows (K15i) are left-aligned against the
+            reference in the sample's own slots before its run is dropped; T's column 6 is then K15i's per-slot count
+            of the sample's moved rows, and the unions run over the moved keys and strings."""
 from __future__ import annotations
 
 import os
@@ -87,7 +90,9 @@ class Cohort:
     each: its deletion groups (device) and its insertion events (host), both in shared slots."""
 
     def __init__(self, paths, devices=None, filters=(0, 0, 0), primers=None, mask_overlaps=False, normalise=None,
-                 dedup=False):
+                 dedup=False, left_align=None):
+        """left_align (extension): None, or a callable giving the reference codes (uint8 numpy) of a sample's batch
+        from (batch, its shared slots of each contig slot, those slots) -- the samples are then left-aligned."""
         from .kindel import _normalise_scheme, check_dedup, check_normalise, pileup_run
 
         import torch
@@ -122,24 +127,35 @@ class Cohort:
             src = np.concatenate([np.arange(s, s + n) for s, n in zip(src_slot.tolist(), span.tolist())]
                                  or [np.zeros(0, dtype=np.int64)]).astype(np.int64)
             dst = src + np.repeat(offset, span)
+            columns, codes, ins = counts[0:7], None, run.ins_table if left_align is None else None
+            if left_align is not None:
+                codes = torch.from_numpy(np.ascontiguousarray(left_align(batch, src, dst), dtype=np.uint8)).to(dev)
+                hist, ins = run.left_aligned_insertions(codes)
+                columns = torch.cat([counts[0:6], hist[None]])
             if src.size:
-                self.table[i, :, torch.from_numpy(dst).to(dev)] = counts[0:7].index_select(
-                    1, torch.from_numpy(src).to(dev))
-            self.deletions.append(self._deletion_keys(dbatch, src_slot, offset))
-            ev = run.ins_table.events
-            ev_slot = ev[:, 0].astype(np.int64)
+                self.table[i, :, torch.from_numpy(dst).to(dev)] = columns.index_select(1, torch.from_numpy(src).to(dev))
+            self.deletions.append(self._deletion_keys(dbatch, src_slot, offset, codes))
+            ev_slot = ins.slots
             c_of = np.searchsorted(src_slot, ev_slot, side="right") - 1
             ins_slot = ev_slot + offset[c_of] if ev_slot.size else ev_slot
             order = np.argsort(ins_slot, kind="stable")
-            strings = decode_events(batch, ev)
+            strings = self._strings(ins)
             self.insertions.append((ins_slot[order], [strings[k] for k in order.tolist()]))
             del run, counts, dbatch  # the sample's device batch and table go before the next one is piled
 
     @staticmethod
-    def _deletion_keys(dbatch, src_slot, offset):
+    def _strings(ins) -> list:
+        """The strings of every row of an insertion table, in its row order (rotated where it has rotations)."""
+        strings = decode_events(ins.batch, ins.events)
+        if ins.rot is None:
+            return strings
+        return [t[len(t) - k:] + t[:len(t) - k] if k else t for t, k in zip(strings, ins.rot.tolist())]
+
+    @staticmethod
+    def _deletion_keys(dbatch, src_slot, offset, codes=None):
         import torch
 
-        key, cnt = engine._deletion_groups(dbatch)
+        key, cnt = engine._deletion_groups(dbatch, codes)
         if key.numel() == 0:
             return key, cnt
         slot = key >> _LEN_BITS
@@ -176,23 +192,43 @@ class Cohort:
 # ---------------------------------------------------------------------------------------------------- text
 def variants_vcf(paths, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
                  exclude_flags=0, reference=None, primers=None, mask_overlaps=False, samples=None,
-                 normalise=None, dedup=False) -> str:
-    """The multi-sample VCF of kindel.variants_vcf given a list of paths (see there for the rules)."""
+                 normalise=None, dedup=False, left_align=False) -> str:
+    """The multi-sample VCF of kindel.variants_vcf given a list of paths (see there for the rules).  left_align
+    (extension) needs a reference (ValueError otherwise); a Reference given with it must be the one of the samples'
+    shared layout."""
+    from .reference import Reference, load_reference, read_fasta, reference_codes
+
+    if left_align and reference is None:
+        raise ValueError("left_align needs a reference: the indels are moved against its bases")
     paths = [os.fspath(p) for p in paths]
     if not paths:
         raise ValueError("variants_vcf needs at least one alignment file")
     names = sample_names(paths, samples)
     filters = (min_base_quality, min_mapq, exclude_flags)
-    cohort = Cohort(paths, devices, filters, primers, mask_overlaps, normalise, dedup)
+    fasta = codes_of = None
+    if left_align:
+        if isinstance(reference, Reference):
+            def codes_of(batch, src, dst):  # the shared layout's codes, gathered into the sample's slots
+                out = np.full(int(batch.n_slots), 4, dtype=np.uint8)
+                out[src] = reference.codes[dst]
+                return out
+        else:
+            fasta = read_fasta(reference)  # one parse for every sample and the shared layout
+
+            def codes_of(batch, src, dst):
+                return reference_codes(fasta, batch, reference)
+    cohort = Cohort(paths, devices, filters, primers, mask_overlaps, normalise, dedup, codes_of)
     lay = cohort.layout
     ref = None
-    if reference is not None:
-        from .reference import Reference, load_reference
-
-        ref = reference if isinstance(reference, Reference) else load_reference(reference, lay)
+    if isinstance(reference, Reference):
+        ref = reference
+    elif fasta is not None:
+        ref = Reference(reference_codes(fasta, lay, reference), os.path.basename(os.fspath(reference)))
+    elif reference is not None:
+        ref = load_reference(reference, lay)
     lines = vcf.header(lay.contig_names, lay.contig_len, abs_threshold, rel_threshold, filters, cohort.primers,
                        cohort.mask_overlaps, reference_name=None if ref is None else ref.name, samples=names,
-                       normalise=cohort.normalise, dedup=cohort.dedup)
+                       normalise=cohort.normalise, dedup=cohort.dedup, left_align=bool(left_align))
     return "\n".join(lines + records(cohort, None if ref is None else ref.codes, abs_threshold, rel_threshold)) + "\n"
 
 

@@ -20,6 +20,7 @@
 #include "amplicons.cu"
 #include "normalise.cu"
 #include "dedup.cu"
+#include "left_align.cu"
 
 namespace {
 
@@ -618,6 +619,31 @@ int kdl_deletion_scatter(const kdl_batch* batch, const uint32_t* block_sums, int
     if (n_blocks == 0) return KDL_OK;
     KDL_LAUNCH(kdl::deletion_scatter_kernel, (unsigned)n_blocks, kdl::A_THREADS, 0, (cudaStream_t)stream,
                *batch, block_sums, n_events, ev_slot, ev_len);
+    return check_launch();
+}
+
+int kdl_left_align_deletions(const int64_t* keys, int64_t n_keys, const int64_t* contig_slot, int32_t n_contigs,
+                             const uint8_t* ref, int64_t* keys_out, void* stream) {
+    if (n_keys < 0 || n_contigs < 0 || (n_keys > 0 && (!keys || !ref || !keys_out || (n_contigs > 0 && !contig_slot))))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_keys + kdl::LA_THREADS - 1) / kdl::LA_THREADS;
+    if (n_blocks == 0) return KDL_OK;
+    KDL_LAUNCH(kdl::left_align_deletions_kernel, (unsigned)n_blocks, kdl::LA_THREADS, 0, (cudaStream_t)stream,
+               keys, n_keys, contig_slot, n_contigs, ref, keys_out);
+    return check_launch();
+}
+
+int kdl_left_align_insertions(const kdl_batch* batch, const int32_t* ins_events, int64_t n_events, const uint8_t* dead,
+                              const uint8_t* ref, int64_t* norm_slot, int32_t* rot, int32_t* hist, void* stream) {
+    int rc = validate_batch(batch);
+    if (rc != KDL_OK) return rc;
+    if (n_events < 0 || (n_events > 0 && (!ins_events || (reinterpret_cast<uintptr_t>(ins_events) & 15) || !ref ||
+                                          !norm_slot || !rot || !hist)))
+        return KDL_ERR_INVALID_ARG;
+    const long long n_blocks = (n_events + kdl::LA_THREADS - 1) / kdl::LA_THREADS;
+    if (n_blocks == 0) return KDL_OK;
+    KDL_LAUNCH(kdl::left_align_insertions_kernel, (unsigned)n_blocks, kdl::LA_THREADS, 0, (cudaStream_t)stream,
+               *batch, ins_events, n_events, dead, ref, norm_slot, rot, hist);
     return check_launch();
 }
 

@@ -29,6 +29,10 @@ implementation behind these functions: without a CUDA device they raise.
                                (extension: `--normalise N`)
     dedup(dbatch, mate)        K10p + K14k + sort + K14s: the reads and read pairs duplicate removal keeps (extension:
                                `--dedup`)
+    left_align_deletions(key, cnt, ref, ...)  K15d + regrouping: deletion groups moved to their leftmost place against
+                               the reference (extension: `--left-align`)
+    left_align_insertions(dbatch, events, ref)  K15i: each insertion row's leftmost slot and string rotation, and the
+                               per-slot count of the moved rows (extension: `--left-align`)
 """
 from __future__ import annotations
 
@@ -963,24 +967,85 @@ def deletion_events(dbatch: DeviceBatch):
 _LEN_BITS = 28  # a CIGAR op length has 28 bits
 
 
-def _deletion_groups(dbatch: DeviceBatch):
+def _deletion_groups(dbatch: DeviceBatch, ref: torch.Tensor = None):
     """K7's events grouped by (slot, length) on the device: (key = slot << 28 | length, count), keys ascending.  The
-    deletions K10 dropped (mask_overlaps) are subtracted by the same key, and groups left empty are removed."""
+    deletions K10 dropped (mask_overlaps) are subtracted by the same key, and groups left empty are removed.  ref
+    (extension: left_align): the device reference codes of the batch's slots; the groups are then left-aligned
+    against them (left_align_deletions) after the drops are subtracted."""
     ev_slot, ev_len = deletion_events(dbatch)
     with torch.cuda.device(dbatch.device):
         key, cnt = torch.unique((ev_slot << _LEN_BITS) | ev_len.to(torch.int64), sorted=True, return_counts=True)
         d = dbatch.drops
-        if d is None or key.numel() == 0:
+        if d is not None and key.numel():
+            d = d[d[:, 3] < 0]
+        if d is not None and key.numel() and d.shape[0]:
+            dk, dc = torch.unique((d[:, 0].to(torch.int64) << _LEN_BITS) | d[:, 1].to(torch.int64), return_counts=True)
+            at = torch.searchsorted(key, dk).clamp(max=key.numel() - 1)
+            cnt = cnt.clone()
+            cnt.index_add_(0, at, torch.where(key[at] == dk, -dc, torch.zeros_like(dc)))  # (each is one of the events)
+            live = cnt > 0
+            key, cnt = key[live], cnt[live]
+        if ref is None:
             return key, cnt
-        d = d[d[:, 3] < 0]
-        if d.shape[0] == 0:
+        return left_align_deletions(key, cnt, ref, dbatch.tensors["contig_slot"], int(dbatch.struct.n_contigs))
+
+
+def left_align_deletions(key: torch.Tensor, cnt: torch.Tensor, ref: torch.Tensor, contig_slot: torch.Tensor,
+                         n_contigs: int):
+    """K15d (extension: left_align): deletion groups (key = slot << 28 | length, count; device tensors) moved to their
+    leftmost place against the device reference codes `ref` (uint8 [n_slots]) over the layout's first slots
+    (contig_slot, int64 device), and grouped again: (key, count) with the counts of keys that met summed, keys
+    ascending.  include/kindel_b200.h has the rule."""
+    lib = _ffi.load()
+    dev = key.device
+    with torch.cuda.device(dev):
+        n = int(key.numel())
+        if n == 0:
             return key, cnt
-        dk, dc = torch.unique((d[:, 0].to(torch.int64) << _LEN_BITS) | d[:, 1].to(torch.int64), return_counts=True)
-        at = torch.searchsorted(key, dk).clamp(max=key.numel() - 1)
-        cnt = cnt.clone()
-        cnt.index_add_(0, at, torch.where(key[at] == dk, -dc, torch.zeros_like(dc)))  # (each is one of the events)
-        live = cnt > 0
-        return key[live], cnt[live]
+        key = key.contiguous()
+        moved = torch.empty_like(key)
+        rc = lib.kdl_left_align_deletions(key.data_ptr(), n, contig_slot.data_ptr(), int(n_contigs), ref.data_ptr(),
+                                          moved.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_left_align_deletions")
+        out, inv = torch.unique(moved, sorted=True, return_inverse=True)
+        total = torch.zeros(out.numel(), dtype=cnt.dtype, device=dev).index_add_(0, inv, cnt)
+    return out, total
+
+
+def left_align_insertions(dbatch: DeviceBatch, events: torch.Tensor, ref: torch.Tensor, dead: torch.Tensor = None):
+    """K15i (extension: left_align): (norm_slot int64 [n], rot int32 [n], hist int32 [n_slots]) on the device for the
+    insertion event rows `events` (int32 [n, 4] on the device, the batch's pileup rows in their order): each row's
+    leftmost slot against the device reference codes `ref` (uint8 [n_slots]), the right rotation of its string there,
+    and per slot the number of live rows moved to it.  dead (uint8 [n] or None): rows K10 dropped, which get norm_slot
+    -1 and count nowhere.  include/kindel_b200.h has the rule."""
+    lib = _ffi.load()
+    dev = dbatch.device
+    n = int(events.shape[0])
+    with torch.cuda.device(dev):
+        events = events.to(dev, torch.int32).contiguous()
+        norm_slot = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+        rot = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        hist = torch.zeros(dbatch.n_slots, dtype=torch.int32, device=dev)
+        if dead is not None:
+            dead = dead.to(dev, torch.uint8).contiguous()
+        rc = lib.kdl_left_align_insertions(C.byref(dbatch.struct), events.data_ptr() if n else None, n,
+                                           dead.data_ptr() if dead is not None and n else None, ref.data_ptr(),
+                                           norm_slot.data_ptr(), rot.data_ptr(), hist.data_ptr(), _stream_ptr(dev))
+        _ffi.check(rc, "kdl_left_align_insertions")
+    return norm_slot[:n], rot[:n], hist
+
+
+def dead_event_rows(dbatch: DeviceBatch, n_events: int):
+    """uint8 [n_events] on the device, 1 at the insertion-event rows K10 dropped (mask_overlaps); None when none."""
+    d = dbatch.drops
+    if d is None or d.shape[0] == 0:
+        return None
+    evt = d[:, 3].to(torch.int64)
+    evt = evt[evt >= 0]
+    if evt.numel() == 0:
+        return None
+    with torch.cuda.device(dbatch.device):
+        return torch.zeros(n_events, dtype=torch.uint8, device=dbatch.device).index_fill_(0, evt, 1)
 
 
 def _group_counts(key, cnt, q):
@@ -991,10 +1056,12 @@ def _group_counts(key, cnt, q):
     return torch.where(key[at] == q, cnt[at], torch.zeros_like(cnt[at]))
 
 
-def deletion_alleles(dbatch: DeviceBatch, counts: torch.Tensor, abs_threshold, rel_threshold):
+def deletion_alleles(dbatch: DeviceBatch, counts: torch.Tensor, abs_threshold, rel_threshold, ref=None):
     """deletion_union of one sample: K7's events of `dbatch` grouped on the device against `counts`, a device table
-    of the same batch; (slot, length, count, depth), int64 numpy arrays sorted by slot, then length."""
-    slot, length, cnt, depth = deletion_union([_deletion_groups(dbatch)], counts[None], abs_threshold, rel_threshold)
+    of the same batch; (slot, length, count, depth), int64 numpy arrays sorted by slot, then length.  ref (extension:
+    left_align): device reference codes, the groups left-aligned against them (_deletion_groups)."""
+    slot, length, cnt, depth = deletion_union([_deletion_groups(dbatch, ref)], counts[None], abs_threshold,
+                                              rel_threshold)
     return slot, length, cnt[0], depth[0]
 
 
@@ -1022,13 +1089,14 @@ def deletion_union(groups, table: torch.Tensor, abs_threshold, rel_threshold):
                 counts.cpu().numpy().astype(np.int64), depths.cpu().numpy())
 
 
-def deletion_counts(dbatch: DeviceBatch, slot, length) -> np.ndarray:
+def deletion_counts(dbatch: DeviceBatch, slot, length, ref=None) -> np.ndarray:
     """K7 over `dbatch` grouped on the device: how many of its deletion events are (slot[i], length[i]), for each
-    queried pair (host int64 arrays); int64 numpy.  `variants --vcf --strand` asks it of the reverse-strand reads."""
+    queried pair (host int64 arrays); int64 numpy.  `variants --vcf --strand` asks it of the reverse-strand reads.
+    ref (extension: left_align): device reference codes, the events left-aligned against them (_deletion_groups)."""
     q = (np.asarray(slot, dtype=np.int64) << _LEN_BITS) | np.asarray(length, dtype=np.int64)
     if q.size == 0:
         return np.zeros(0, dtype=np.int64)
-    key, cnt = _deletion_groups(dbatch)
+    key, cnt = _deletion_groups(dbatch, ref)
     with torch.cuda.device(dbatch.device):
         return _group_counts(key, cnt, torch.from_numpy(q).to(key.device)).cpu().numpy().astype(np.int64)
 

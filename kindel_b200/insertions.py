@@ -42,24 +42,39 @@ def decode_events(batch: ReadBatch, rows: np.ndarray) -> list:
 
 
 class InsertionTable:
-    """Events of one pileup, indexed by slot."""
+    """Events of one pileup, indexed by slot.
 
-    def __init__(self, batch: ReadBatch, events: np.ndarray):
+    slots / rot (extension: left-aligned insertions, K15i): each row's slot is then slots[i] instead of its column 0,
+    and its string is the decoded one rotated right by rot[i]."""
+
+    def __init__(self, batch: ReadBatch, events: np.ndarray, slots: np.ndarray = None, rot: np.ndarray = None):
         self.batch = batch
         events = np.ascontiguousarray(events, dtype=np.int32).reshape(-1, 4)
-        order = np.argsort(events[:, 0], kind="stable")  # keep iteration order inside a slot
+        slots = events[:, 0].astype(np.int64) if slots is None else np.asarray(slots, dtype=np.int64)
+        order = np.argsort(slots, kind="stable")  # keep iteration order inside a slot
         self.events = events[order]
-        self.slots = self.events[:, 0].astype(np.int64)
+        self.slots = slots[order]
+        self.rot = None if rot is None else np.asarray(rot, dtype=np.int64)[order]
+
+    def _span(self, slot: int):
+        return (np.searchsorted(self.slots, slot, side="left"), np.searchsorted(self.slots, slot, side="right"))
 
     def rows_at(self, slot: int) -> np.ndarray:
-        lo = np.searchsorted(self.slots, slot, side="left")
-        hi = np.searchsorted(self.slots, slot, side="right")
+        lo, hi = self._span(slot)
         return self.events[lo:hi]
+
+    def strings_at(self, slot: int) -> list:
+        """The strings of the rows at a slot, in their order (rotated where the table has rotations)."""
+        lo, hi = self._span(slot)
+        texts = decode_events(self.batch, self.events[lo:hi])
+        if self.rot is None:
+            return texts
+        return [t[len(t) - k:] + t[:len(t) - k] if k else t for t, k in zip(texts, self.rot[lo:hi].tolist())]
 
     def dict_at(self, slot: int) -> dict:
         """{string: count} in first-seen order (what `insertions[pos]` is in the reference)."""
         out = {}
-        for s in decode_events(self.batch, self.rows_at(slot)):
+        for s in self.strings_at(slot):
             out[s] = out.get(s, 0) + 1
         return out
 

@@ -23,7 +23,7 @@ import numpy as np
 
 from . import bamio, engine, quality, vcf
 from .primers import AmpliconScheme, PrimerSet, amplicon_arrays, as_primer_set, as_scheme, primer_arrays
-from .insertions import InsertionTable, decode_events, dict_consensus
+from .insertions import InsertionTable, dict_consensus
 from .views import Alignment, BaseCounts, Insertions
 from .vcf import QUAL_CAP, allele_quality, strand_odds_ratio  # noqa: F401  (kindel's VCF names)
 
@@ -63,6 +63,7 @@ class PileupRun:
     primers = None   # the PrimerSet whose primer bases the pileup masked (extension), None when off
     mask_overlaps = False  # the pileup counted each read pair once where its mates overlap (extension, K10)
     _dropped_events = None  # K10's dropped insertion-event rows of host tables
+    _host_events = None  # the event rows of host tables in their order, K10's dropped rows included (left_align)
     _overlap_stats = None   # K10's (pairs, bases, deletions, insertions) of host tables
     normalised = None  # (N, dropped, kept) of the --normalise cap the batch went through (extension), None when off
     deduplicated = None  # (pairs removed, singles removed, kept, before) of --dedup (extension), None when off
@@ -96,6 +97,7 @@ class PileupRun:
         run._host_counts = np.ascontiguousarray(counts, dtype=np.int32)
         run._host_derived = np.ascontiguousarray(derived, dtype=np.int32)
         run._ins = None
+        run._host_events = np.ascontiguousarray(events, dtype=np.int32).reshape(-1, 4)
         run._ins = run._insertion_table(events)
         return run
 
@@ -184,15 +186,40 @@ class PileupRun:
             self._ins = self._insertion_table(self.events.cpu().numpy())
         return self._ins
 
-    def _insertion_table(self, events) -> InsertionTable:
-        """The one place the run's event rows become its insertion table: without the rows K10 dropped
-        (mask_overlaps), so that no insertion string, VCF record or `alignment` view reads them."""
+    def _dropped_rows(self):
+        """The insertion-event rows K10 dropped (mask_overlaps), or None."""
         dropped = self._dropped_events
         if dropped is None and self.dbatch is not None:
             dropped = engine.dropped_event_rows(self.dbatch)
+        return dropped
+
+    def _insertion_table(self, events) -> InsertionTable:
+        """The one place the run's event rows become its insertion table: without the rows K10 dropped
+        (mask_overlaps), so that no insertion string, VCF record or `alignment` view reads them."""
+        dropped = self._dropped_rows()
         if dropped is not None and len(dropped):
             events = np.delete(np.asarray(events).reshape(-1, 4), np.asarray(dropped, dtype=np.int64), axis=0)
         return InsertionTable(self.batch, events)
+
+    def left_aligned_insertions(self, ref):
+        """(hist int32 [n_slots] on the device, InsertionTable) of the insertions left-aligned against the device
+        reference codes `ref` (extension: left_align): K15i over the run's event rows in their order -- host tables'
+        rows uploaded next to device_tables()' batch -- with the rows K10 dropped excluded first.  hist counts the live
+        rows per left-aligned slot; the table holds the live rows at those slots with their strings' rotations."""
+        import torch
+
+        _, dbatch = self.device_tables()
+        events = self.events if self.events is not None else torch.from_numpy(self._host_events).to(dbatch.device)
+        n = int(events.shape[0])
+        dead = None
+        dropped = self._dropped_rows()
+        if dropped is not None and len(dropped):
+            dead = torch.zeros(n, dtype=torch.uint8, device=dbatch.device)
+            dead[torch.from_numpy(np.asarray(dropped, dtype=np.int64)).to(dbatch.device)] = 1
+        norm_slot, rot, hist = engine.left_align_insertions(dbatch, events, ref, dead)
+        slots, rot, rows = norm_slot.cpu().numpy(), rot.cpu().numpy(), events.cpu().numpy()
+        live = slots >= 0
+        return hist, InsertionTable(self.batch, rows[live], slots[live], rot[live])
 
     @property
     def overlap_stats(self):
@@ -1258,7 +1285,7 @@ def _vcf_header(run, abs_threshold, rel_threshold, filters, **options):
 
 def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, min_base_quality=0, min_mapq=0,
                  exclude_flags=0, reference=None, strand=False, max_sor=None, primers=None, mask_overlaps=False,
-                 samples=None, qual=False, min_qual=None, normalise=None, dedup=False) -> str:
+                 samples=None, qual=False, min_qual=None, normalise=None, dedup=False, left_align=False) -> str:
     """Sites-only VCF 4.2 text of the sites of `variants --only-variants` (extension; `kindel variants --vcf`).
 
     kindel takes no reference sequence, so REF is the sample's own most frequent allele at the position: this is a
@@ -1303,7 +1330,14 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
     capped as it would be alone, and the header gets `##kindelNormalise=N` after `##kindelPrimers`.
 
     dedup (extension: `--dedup`): see pileup_run; every sample's duplicates are removed as they would be alone, and the
-    header gets `##kindelDedup=fragment ends, base-quality score` after `##kindelPrimers`, before `##kindelNormalise`."""
+    header gets `##kindelDedup=fragment ends, base-quality score` after `##kindelPrimers`, before `##kindelNormalise`.
+
+    left_align (extension: `--left-align`, needs `reference`; ValueError otherwise): every deletion and insertion event
+    is moved to its leftmost place against the reference before the events are grouped and tested, so that one indel
+    an aligner placed at several offsets of a repeat is one record with the count of all its placements
+    (variants_vcf_from_run has the rule).  The header gets `##kindelLeftAlign=leftmost against the reference` after
+    `##reference`."""
+    left_align = check_left_align(left_align, reference)
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
     min_qual = check_min_qual(min_qual)
@@ -1317,14 +1351,22 @@ def variants_vcf(bam_path, abs_threshold=1, rel_threshold=0.01, devices=None, mi
 
         return cohort.variants_vcf(bam_path, abs_threshold, rel_threshold, devices, min_base_quality, min_mapq,
                                    exclude_flags, reference=reference, primers=primers, mask_overlaps=mask_overlaps,
-                                   samples=samples, normalise=normalise, dedup=dedup)
+                                   samples=samples, normalise=normalise, dedup=dedup,
+                                   **({"left_align": True} if left_align else {}))
     if samples is not None:
         raise ValueError("samples= names the columns of several samples: pass the alignment files as a list")
     filters = (min_base_quality, min_mapq, exclude_flags)
     run = pileup_run(bam_path, devices, 1, *filters, strand=strand, primers=primers, mask_overlaps=mask_overlaps,
                      qual=qual, normalise=normalise, dedup=dedup)[0]
     return variants_vcf_from_run(run, abs_threshold, rel_threshold, filters, reference=reference, strand=strand,
-                                 max_sor=max_sor, qual=qual, min_qual=min_qual)
+                                 max_sor=max_sor, qual=qual, min_qual=min_qual, left_align=left_align)
+
+
+def check_left_align(left_align, reference) -> bool:
+    """left_align as a bool; on without a reference raises ValueError (the shift is against its bases)."""
+    if left_align and reference is None:
+        raise ValueError("left_align needs a reference: the indels are moved against its bases")
+    return bool(left_align)
 
 
 def _quality_at(run, slots):
@@ -1351,10 +1393,12 @@ def _rows_at(table, slots):
     return table[0:6].index_select(1, idx).cpu().numpy().astype(np.int64)
 
 
-def _reverse_strand(run, slot, deletions):
+def _reverse_strand(run, slot, deletions, ins=None, ref=None):
     """The strand option of vcf.records from the run's reverse-strand reads: their rows at the sites and, with a
     reference (deletions given), their DPa at the sites, each deletion's reverse count and depth and each insertion
-    string's reverse reads at a slot (the event rows whose read is reverse)."""
+    string's reverse reads at a slot (the event rows whose read is reverse).  ins / ref (extension: left_align): the
+    insertion table the records read (default: the run's) and the device reference codes the reverse reads'
+    deletion events are left-aligned against (None: as the aligner placed them)."""
     rev_table, rev_batch = run.reverse_table()
     rows = _rows_at(rev_table, slot)
     if deletions is None:
@@ -1362,19 +1406,20 @@ def _reverse_strand(run, slot, deletions):
     batch = run.batch
 
     def strings_at(s):
-        events = run.ins_table.rows_at(s)
+        table = run.ins_table if ins is None else ins
+        events = table.rows_at(s)
         out = {}
-        for text, r in zip(decode_events(batch, events), batch.reverse[events[:, 1].astype(np.int64)].tolist()):
+        for text, r in zip(table.strings_at(s), batch.reverse[events[:, 1].astype(np.int64)].tolist()):
             out[text] = out.get(text, 0) + r
         return out
 
     return (rows, _rows_at(rev_table, vcf.dpa_slots(batch, slot)).sum(axis=0),
-            engine.deletion_counts(rev_batch, deletions[0], deletions[1]),
+            engine.deletion_counts(rev_batch, deletions[0], deletions[1], **({} if ref is None else {"ref": ref})),
             _rows_at(rev_table, deletions[0]).sum(axis=0), strings_at)
 
 
 def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None, reference=None, strand=False,
-                          max_sor=None, qual=False, min_qual=None) -> str:
+                          max_sor=None, qual=False, min_qual=None, left_align=False) -> str:
     """Host half of variants_vcf (see there): the VCF text of a finished pileup.  filters: (min_base_quality,
     min_mapq, exclude_flags) as the pileup applied them, for the header.  reference, strand, max_sor: see variants_vcf;
     vcf.records has the rules of the records.  Strand needs a run whose batch has `reverse`
@@ -1386,7 +1431,17 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
     the total's minus those, so ADF + ADR == AD.  With one, an SNV's the same (REF 0 where the reference has no A, C,
     G or T); an indel's ALT entry is its reads on that strand (the reverse sub-batch's deletion events, the insertion
     events of reverse reads) and its REF entry max(DP_s - AO_s, 0), DP_s the record's DP taken from strand s's table,
-    so ADF[1] + ADR[1] == AO.  qual / min_qual: see variants_vcf; needs a run whose batch has `qual8`."""
+    so ADF[1] + ADR[1] == AO.  qual / min_qual: see variants_vcf; needs a run whose batch has `qual8`.
+
+    left_align (extension, needs a reference): with g the reference codes and s0 the contig's first slot, a deletion
+    event (r, n) moves left while r > s0, g[r-1] is A, C, G or T and g[r-1] == g[r+n-1] (K15d, on the K7 groups, whose
+    keys that meet are summed); an insertion event at p with string t moves left while p > s0, g[p-1] is a base and the
+    last base of the string rotated so far equals it, the string rotating right by one each step (K15i, on every event
+    row K10 did not drop; a base that is not A, C, G or T stops it).  The groups, the tests, DP / DPa, the strand
+    counts and the records are then the rules above over the moved events; the strings at a slot are in the order of
+    their rows.  The insertion candidates come from K6r over the table with column 6 replaced by K15i's per-slot count
+    of moved rows.  Columns 0-6 of the table and the SNV records do not change."""
+    left_align = check_left_align(left_align, reference)
     max_sor = check_max_sor(max_sor)
     strand = bool(strand) or max_sor is not None
     min_qual = check_min_qual(min_qual)
@@ -1402,22 +1457,34 @@ def variants_vcf_from_run(run, abs_threshold=1, rel_threshold=0.01, filters=None
 
         ref = reference if isinstance(reference, Reference) else load_reference(reference, batch)
     lines = _vcf_header(run, abs_threshold, rel_threshold, filters, reference_name=None if ref is None else ref.name,
-                        strand=strand, max_sor=max_sor, qual=qual, min_qual=min_qual)
-    dpa = dels = None
+                        strand=strand, max_sor=max_sor, qual=qual, min_qual=min_qual, left_align=left_align)
+    dpa = dels = codes = None
+    ins = None  # the left-aligned insertion table (left_align), else the run's
     if ref is None:
         slot, site_counts, mask = variant_sites(run, abs_threshold, rel_threshold)
     else:
         # host tables (the multi-GPU result): the reduced table and the batch go to this process's GPU
         counts, dbatch = run.device_tables()
-        slot, site_counts, dpa, mask = engine.variant_sites_ref(counts, batch.contig_slot, batch.contig_len, ref.codes,
-                                                                abs_threshold, rel_threshold)
+        sites_table, codes = counts, ref.codes
+        if left_align:
+            import torch
+
+            codes = torch.from_numpy(np.ascontiguousarray(ref.codes, dtype=np.uint8)).to(counts.device)
+            hist, ins = run.left_aligned_insertions(codes)
+            sites_table = torch.empty((7, counts.shape[1]), dtype=torch.int32, device=counts.device)
+            sites_table[0:6] = counts[0:6]
+            sites_table[6] = hist
+        slot, site_counts, dpa, mask = engine.variant_sites_ref(sites_table, batch.contig_slot, batch.contig_len,
+                                                                codes, abs_threshold, rel_threshold)
         dpa = dpa[None]
-        d_slot, d_len, d_cnt, d_depth = engine.deletion_alleles(dbatch, counts, abs_threshold, rel_threshold)
+        moved = {"ref": codes} if left_align else {}  # (the keyword only when on: the call stays as it was otherwise)
+        d_slot, d_len, d_cnt, d_depth = engine.deletion_alleles(dbatch, counts, abs_threshold, rel_threshold, **moved)
         dels = d_slot, d_len, d_cnt[None], d_depth[None]
     lines += vcf.records(batch, abs_threshold, rel_threshold, slot, mask, site_counts[None, 0:6].astype(np.int64),
                          ref_codes=None if ref is None else ref.codes, dpa=dpa,
-                         strings_at=lambda j, s: run.ins_table.dict_at(s), deletions=dels,
-                         strand=_reverse_strand(run, slot, dels) if strand else None, max_sor=max_sor,
+                         strings_at=lambda j, s: (run.ins_table if ins is None else ins).dict_at(s), deletions=dels,
+                         strand=_reverse_strand(run, slot, dels, ins, codes if left_align else None) if strand else None,
+                         max_sor=max_sor,
                          qual=_quality_at(run, slot) if qual else None, min_qual=min_qual)
     return "\n".join(lines) + "\n"
 

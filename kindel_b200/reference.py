@@ -72,7 +72,12 @@ def sequence_codes(raw: bytes, name: str) -> np.ndarray:
 
 def load_reference(path, batch) -> Reference:
     """Base codes of `batch`'s contigs from the FASTA at `path`, laid out over the batch's slots (see the module)."""
-    records = read_fasta(path)
+    return Reference(reference_codes(read_fasta(path), batch, path), os.path.basename(os.fspath(path)))
+
+
+def reference_codes(records, batch, path) -> np.ndarray:
+    """uint8 codes [n_slots] of `batch`'s contigs from read_fasta's `records` of the FASTA at `path` (see the module;
+    one parse serves several layouts)."""
     codes = np.full(int(batch.n_slots), 4, dtype=np.uint8)
     for name, s0, L in zip(batch.contig_names, np.asarray(batch.contig_slot).tolist(),
                            np.asarray(batch.contig_len).tolist()):
@@ -84,4 +89,4 @@ def load_reference(path, batch) -> Reference:
             raise ValueError("contig %r: the reference FASTA holds %d bases, the alignment's @SQ LN is %d"
                              % (name, c.shape[0], L))
         codes[s0:s0 + L] = c
-    return Reference(codes, os.path.basename(os.fspath(path)))
+    return codes

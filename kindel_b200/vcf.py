@@ -34,10 +34,11 @@ def check_number(value, name):
 
 def header(contig_names, contig_len, abs_threshold, rel_threshold, filters, primers=None, mask_overlaps=False,
            reference_name=None, strand=False, max_sor=None, qual=False, min_qual=None, samples=None,
-           normalise=None, dedup=False) -> list:
+           normalise=None, dedup=False, left_align=False) -> list:
     """The header lines, the column line last.  filters: (min_base_quality, min_mapq, exclude_flags) or None; primers:
     the run's PrimerSet or None; samples: the FORMAT columns' names (a multi-sample VCF) or None; normalise: the
-    --normalise cap N or None; dedup: the run went through --dedup."""
+    --normalise cap N or None; dedup: the run went through --dedup; left_align: the indels were left-aligned against
+    the reference (`##kindelLeftAlign` after `##reference`)."""
     from . import __version__
 
     mbq, mapq, flags = filters if filters is not None else (0, 0, 0)
@@ -58,6 +59,8 @@ def header(contig_names, contig_len, abs_threshold, rel_threshold, filters, prim
         lines.append("##kindelQual=model=poisson;min_qual={}".format("." if min_qual is None else min_qual))
     if reference_name is not None:
         lines.append("##reference={}".format(reference_name))
+        if left_align:
+            lines.append("##kindelLeftAlign=leftmost against the reference")
     lines += ["##contig=<ID={},length={}>".format(name, int(L)) for name, L in zip(contig_names, contig_len)]
     lines += ['##INFO=<ID=DP,Number=1,Type=Integer,Description="Depth: A + C + G + T + N + deletions">',
               '##INFO=<ID=AD,Number=R,Type=Integer,Description="Count of REF (the most frequent allele) and of each '
